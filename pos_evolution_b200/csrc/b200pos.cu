@@ -17,15 +17,6 @@
 
 using namespace b2;
 
-// dynamic shared memory of the tree phase in its shared-memory form: votes/prefix/weights u64[n+1], packed word u32[n], marks u32[n+1],
-// and -- when it still fits -- the work list u32[n] of the marking phase
-static size_t tree_smem_bytes(ghost_tree_args& A) {
-    const size_t base = ((size_t)A.n + 1) * 8 + (size_t)A.n * 8 + 8;
-    const size_t with_list = base + (size_t)A.n * 4;
-    A.hard_list = with_list <= 226 * 1024 ? 1 : 0;
-    return A.hard_list ? with_list : base;
-}
-
 struct dbuf {
     void* p = nullptr;
     size_t cap = 0;
@@ -33,7 +24,7 @@ struct dbuf {
 
 struct vslot {
     dbuf haff, hflag, pkjac, pkst, saff, sflag, f, sumjac;
-    dbuf g2aff, g2st;                                      // the slot's own decompressed signatures (pipelined epochs, B2_SEGSUM_TAIL)
+    dbuf g2aff, g2st;                                      // the slot's own decompressed signatures (pipelined epochs)
     uint64_t n_sig_tail = 0;                               // signatures of the epoch whose segment sums the tail still has to run
     bool segsum_pending = false;
     dbuf pkjac_r, rscal, sg_aff, sg_flag, f_g, gpass;      // RLC batch mode: [r]PK, r, per-group signature sums, group Miller values / verdicts
@@ -79,13 +70,6 @@ struct b2_ctx {
     unsigned k2_block = 32;    // threads per aggregate of k_g1_aggregate under the epoch pipeline (B2_K2_BLOCK: 32/64/128)
     // K2 through the TMA-staged gather kernel (gather.cuh) instead of the LDG form; B2_K2_TMA=0 selects the LDG form (A/B)
     bool k2_tma = true;
-    // sliding-window tables of the decompression's exponentiations: B2_POW_SMEM=1 puts them in shared memory (halves the kernel's DRAM
-    // traffic, 1.40 -> 0.73 GB per launch, measured on an earlier GPU) -- but the 48 KB per block compete with the tail
-    // kernels' shared memory under the pipeline and the step was 0.6 ms SLOWER there (36.11 vs 35.48 ms), so the
-    // default keeps them in local memory
-    bool pow_smem = false;
-    // pipelined epochs: per-segment signature sums on the slot's tail stream instead of the caller's (B2_SEGSUM_TAIL=0: round-1 form)
-    bool segsum_tail = true;
     // FastAggregateVerify mode: 0 = one pairing check per aggregate; 1 = random-linear-combination batches of B2_RLC_GROUP
     // aggregates with per-aggregate fallback (b2_set_verify_mode); d_rlc_seed = the verifier's secret 32-byte seed
     int verify_mode = 0;
@@ -94,11 +78,6 @@ struct b2_ctx {
     // threads per block of k_g2_decompress: its blocks fill the register file, so a smaller block is what a pairing warp of the
     // previous epoch displaces when the two overlap
     unsigned dec_block = 128;
-    // SMs the persistent decompression kernel of the pipelined epoch path leaves empty for the pairing tails (kernels.cuh).
-    // 0 = off (the default: measured slower, see DESIGN.md); B2_RESERVE_SMS=n turns the experiment on.
-    unsigned reserve_sms = 0;
-    sm_mask reserved = {{0, 0, 0, 0}};
-    unsigned long long* d_dec_counter = nullptr;      // one work counter per epoch slot
     // one-launch get_head (k_get_head_fused): ticket counter, and the result slot in mapped pinned host memory (head, sequence)
     bool head_fused = true;                           // B2_HEAD_FUSED=0: the two-launch + memcpy form of round 1
     unsigned int* d_ticket = nullptr;
@@ -181,6 +160,13 @@ template <class T> static int dev_alloc(b2_ctx* ctx, T** p, size_t count) {
 }
 #define B2_TEAM_SMEM (B2_TEAMS_PER_WARP * sizeof(team_ws))
 static inline unsigned blocks_for(uint64_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
+// true when environment variable `name` is set; *v = its value as atoi reads it
+static bool env_int(const char* name, int* v) {
+    const char* s = getenv(name);
+    if (s) *v = atoi(s);
+    return s != nullptr;
+}
+static bool is_block_knob(int v) { return v == 32 || v == 64 || v == 128; }
 
 extern "C" {
 
@@ -210,11 +196,6 @@ int b2_init(int device, b2_ctx** out) {
     cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
     cudaError_t e = cudaStreamCreateWithPriority(&ctx->s_main, cudaStreamNonBlocking, prio_lo);
     for (int i = 0; i < 4 && e == cudaSuccess; i++) e = cudaStreamCreateWithPriority(&ctx->s_dec[i], cudaStreamNonBlocking, prio_lo);
-    if (const char* ev = getenv("B2_DEC_STREAMS")) {
-        unsigned v = (unsigned)atoi(ev);
-        if (v >= 2 && v <= 4) ctx->n_dec_streams = v;
-    }
-    if (const char* ev = getenv("B2_DEC_ALTERNATE")) ctx->dec_alternate = atoi(ev) != 0 ? 1 : 0;
     for (int i = 0; i < B2_EPOCH_SLOTS && e == cudaSuccess; i++) {
         e = cudaStreamCreateWithPriority(&ctx->slot[i].s_tail, cudaStreamNonBlocking, prio_hi);
         for (int k = 0; k < 2 && e == cudaSuccess; k++) e = cudaStreamCreateWithPriority(&ctx->slot[i].s_aux[k], cudaStreamNonBlocking, prio_hi);
@@ -228,28 +209,9 @@ int b2_init(int device, b2_ctx** out) {
     }
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_ghost_tree, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_ghost_votes_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_g2_decompress, cudaFuncAttributeMaxDynamicSharedMemorySize, 432 * 128);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_g1_gather_tma<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * (int)sizeof(gather_ws));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_g1_gather_tma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * (int)sizeof(gather_ws));
     ctx->n_sm = prop.multiProcessorCount;
-    if (const char* e = getenv("B2_TAIL_BLOCK")) {          // tuning knob (32/64/128); the default is the measured best
-        unsigned v = (unsigned)atoi(e);
-        if (v == 32 || v == 64 || v == 128) ctx->tail_block = v;
-    }
-    if (const char* e = getenv("B2_K2_BLOCK")) {
-        unsigned v = (unsigned)atoi(e);
-        if (v == 32 || v == 64 || v == 128) ctx->k2_block = v;
-    }
-    if (const char* e = getenv("B2_K2_TMA")) ctx->k2_tma = atoi(e) != 0;
-    if (const char* e = getenv("B2_POW_SMEM")) ctx->pow_smem = atoi(e) != 0;
-    if (const char* e = getenv("B2_SEGSUM_TAIL")) ctx->segsum_tail = atoi(e) != 0;
-    if (const char* e = getenv("B2_PAIRING_FORM")) ctx->pairing_form = !strcmp(e, "team") ? 1 : (!strcmp(e, "thread") ? 2 : 0);
-    if (const char* e = getenv("B2_RESERVE_SMS")) {
-        unsigned v = (unsigned)atoi(e);
-        if (v < (unsigned)ctx->n_sm / 2) ctx->reserve_sms = v;
-    }
-    if (ctx->reserve_sms >= (unsigned)ctx->n_sm / 2) ctx->reserve_sms = ctx->n_sm / 9;
-    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_dec_counter, sizeof(unsigned long long) * B2_EPOCH_SLOTS);
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_dbg, 32 * 8);
     if (e == cudaSuccess) e = cudaMemset(ctx->d_dbg, 0, 32 * 8);
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_ticket, 64);
@@ -261,40 +223,20 @@ int b2_init(int device, b2_ctx** out) {
     }
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_get_head_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_get_head_fused_nvl, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
-    if (const char* ev = getenv("B2_HEAD_FUSED")) ctx->head_fused = atoi(ev) != 0;
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_rlc_seed, 32);
     if (e == cudaSuccess) e = cudaMemset(ctx->d_rlc_seed, 0, 32);
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_guard, 256);
     if (e == cudaSuccess) e = cudaMemset(ctx->d_guard, 0, 256);
-    if (e == cudaSuccess && ctx->reserve_sms > 0) {
-        // the SM ids that exist (they need not be 0..n_sm-1); reserve the highest `reserve_sms` of them
-        unsigned int* d_seen = nullptr;
-        unsigned int seen[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-        e = cudaMalloc(&d_seen, sizeof(seen));
-        if (e == cudaSuccess) e = cudaMemset(d_seen, 0, sizeof(seen));
-        if (e == cudaSuccess) {
-            k_probe_smid<<<ctx->n_sm * 8, 64>>>(d_seen);
-            e = cudaMemcpy(seen, d_seen, sizeof(seen), cudaMemcpyDeviceToHost);
-        }
-        if (d_seen) cudaFree(d_seen);
-        unsigned left = ctx->reserve_sms, found = 0;
-        for (int id = 255; id >= 0; id--) {
-            if (!((seen[id >> 5] >> (id & 31)) & 1u)) continue;
-            found++;
-            if (left) {
-                ctx->reserved.w[id >> 6] |= 1ull << (id & 63);
-                left--;
-            }
-        }
-        if (found < (unsigned)ctx->n_sm) {          // the probe did not reach every SM: do not reserve blindly
-            ctx->reserved = sm_mask{{0, 0, 0, 0}};
-            ctx->reserve_sms = 0;
-        }
-    }
-    if (const char* e = getenv("B2_DEC_BLOCK")) {
-        unsigned v = (unsigned)atoi(e);
-        if (v == 32 || v == 64 || v == 128) ctx->dec_block = v;
-    }
+    // diagnostic knobs (INTEGRATION.md); unset or out-of-range values keep the defaults, which are the measured best
+    int v = 0;
+    if (env_int("B2_DEC_STREAMS", &v) && v >= 2 && v <= 4) ctx->n_dec_streams = (unsigned)v;
+    if (env_int("B2_DEC_ALTERNATE", &v)) ctx->dec_alternate = v != 0 ? 1 : 0;
+    if (env_int("B2_TAIL_BLOCK", &v) && is_block_knob(v)) ctx->tail_block = (unsigned)v;
+    if (env_int("B2_K2_BLOCK", &v) && is_block_knob(v)) ctx->k2_block = (unsigned)v;
+    if (env_int("B2_DEC_BLOCK", &v) && is_block_knob(v)) ctx->dec_block = (unsigned)v;
+    if (env_int("B2_K2_TMA", &v)) ctx->k2_tma = v != 0;
+    if (env_int("B2_HEAD_FUSED", &v)) ctx->head_fused = v != 0;
+    if (const char* form = getenv("B2_PAIRING_FORM")) ctx->pairing_form = !strcmp(form, "team") ? 1 : (!strcmp(form, "thread") ? 2 : 0);
     if (e != cudaSuccess) {
         delete ctx;
         return B2_ECUDA;
@@ -333,7 +275,6 @@ void b2_destroy(b2_ctx* ctx) {
     for (int i = 0; i < 4; i++)
         if (ctx->s_dec[i]) cudaStreamDestroy(ctx->s_dec[i]);
     if (ctx->ev_lmd_done) cudaEventDestroy(ctx->ev_lmd_done);
-    if (ctx->d_dec_counter) cudaFree(ctx->d_dec_counter);
     if (ctx->d_guard) cudaFree(ctx->d_guard);
     if (ctx->d_rlc_seed) cudaFree(ctx->d_rlc_seed);
     if (ctx->d_ticket) cudaFree(ctx->d_ticket);
@@ -530,19 +471,13 @@ int b2_gather_probe_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* 
 // is the slot's TAIL stream: the decompressed points then live in the slot's own buffer and the caller's stream goes straight on to
 // the next epoch's decompression instead of waiting ~2 ms for a 2 048-warp kernel that cannot fill the chip.
 static int aggregate_front(b2_ctx* ctx, vslot& V, const uint8_t* d_sig96, const uint32_t* d_seg_off, uint32_t n_seg, uint64_t n_sig,
-                           int32_t* d_seg_status, cudaStream_t s, int reserve_slot = -1, bool own_buffers = false) {
+                           int32_t* d_seg_status, cudaStream_t s, bool own_buffers = false) {
     int rc;
     dbuf& aff = own_buffers ? V.g2aff : ctx->sc_g2aff;
     dbuf& st = own_buffers ? V.g2st : ctx->sc_g2st;
     if ((rc = ensure(ctx, aff, (size_t)n_sig * 192 + 16)) || (rc = ensure(ctx, st, n_sig + 16)) || (rc = ensure(ctx, V.sumjac, (size_t)n_seg * 288))) return rc;
-    if (n_sig && reserve_slot >= 0 && ctx->reserve_sms > 0 && n_sig >= (uint64_t)ctx->n_sm * 512) {
-        unsigned long long* ctr = ctx->d_dec_counter + reserve_slot;
-        CK(cudaMemsetAsync(ctr, 0, sizeof(unsigned long long), s));
-        k_g2_decompress_persistent<<<ctx->n_sm * 4, 128, 0, s>>>(d_sig96, n_sig, (uint32_t*)aff.p, (uint8_t*)st.p, ctr, ctx->reserved);
-        CKL(ctx);
-    } else if (n_sig) {
-        k_g2_decompress<<<blocks_for(n_sig, ctx->dec_block), ctx->dec_block, ctx->pow_smem ? 432 * ctx->dec_block : 0, s>>>(
-            d_sig96, n_sig, (uint32_t*)aff.p, (uint8_t*)st.p, ctx->pow_smem ? 1 : 0);
+    if (n_sig) {
+        k_g2_decompress<<<blocks_for(n_sig, ctx->dec_block), ctx->dec_block, 0, s>>>(d_sig96, n_sig, (uint32_t*)aff.p, (uint8_t*)st.p);
         CKL(ctx);
     }
     if (own_buffers) return B2_OK;          // the segment sums follow on the tail stream (aggregate_segments)
@@ -772,7 +707,7 @@ static int epoch_start(b2_ctx* ctx, int slot, const uint8_t* d_sig96, const uint
         CK(cudaEventRecord(V.ev_in, s));                // inputs ready, slot drained
         CK(cudaStreamWaitEvent(sd, V.ev_in, 0));
     }
-    if ((rc = aggregate_front(ctx, V, d_sig96, d_off, n_agg, n_sig, d_agg_status, sd, team ? -1 : slot, own_buffers))) return rc;
+    if ((rc = aggregate_front(ctx, V, d_sig96, d_off, n_agg, n_sig, d_agg_status, sd, own_buffers))) return rc;
     CK(cudaEventRecord(V.ev_seg, sd));
     return B2_OK;
 }
@@ -823,7 +758,7 @@ int b2_epoch_start_dev(b2_ctx* ctx, int slot, const uint8_t* d_sig96, const uint
     REQUIRE(ctx->n_val > 0, "epoch_start_dev: registry not loaded");
     CK(cudaSetDevice(ctx->device));
     return epoch_start(ctx, slot, d_sig96, d_members, d_off, d_bits, bits_stride, d_msg32, n_agg, n_sig, d_agg_status, (cudaStream_t)stream,
-                       ctx->epoch_team, ctx->segsum_tail);
+                       ctx->epoch_team, true);
 }
 int b2_epoch_tail_dev(b2_ctx* ctx, int slot, const uint32_t* d_members, const uint32_t* d_off, const uint8_t* d_bits, uint32_t bits_stride,
                       const uint64_t* d_target_epoch, const uint32_t* d_block_idx, uint32_t n_agg, uint8_t* d_agg_sig96, int32_t* d_agg_status,
@@ -1329,6 +1264,63 @@ int b2_tree_load(b2_ctx* ctx, const uint32_t* parent, const uint64_t* slot, cons
     return B2_OK;
 }
 
+// the vote scatter's view of the validators [v_begin, v_end) under the context's fork-choice variant
+static ghost_votes_args votes_args(const b2_ctx* ctx, uint64_t v_begin, uint64_t v_end) {
+    return {v_end - v_begin, ctx->d_lmd_key + v_begin, ctx->d_lmd_block + v_begin, ctx->d_equiv + v_begin, ctx->d_flags + v_begin, ctx->d_eff + v_begin,
+            ctx->fc_min_key, 1u, ctx->fc_exclude_slashed ? 3u : 1u};
+}
+
+// Arguments of the tree phase (K9); returns the dynamic shared memory to launch it with.  The shared-memory form (use_smem) holds
+// votes/prefix/weights u64[n+1], packed word u32[n] and marks u32[n+1] in 226 KB (227 KB per block minus the kernel's static shared
+// memory) and at most 15 elements per thread; when it still fits, the launch also reserves the work list u32[n] of the marking phase
+// (hard_list).  Trees that do not fit run the generic form on global scratch (0 bytes).
+static size_t fill_tree_args(b2_ctx* ctx, ghost_tree_args& A, uint64_t* d_votes_preorder, uint32_t justified_idx, int32_t boost_idx, uint64_t boost_score,
+                             uint64_t* d_weight_out, uint32_t* d_head_idx_out) {
+    A.n = ctx->n_blocks;
+    A.pre = ctx->d_pre;
+    A.inv = ctx->d_inv;
+    A.size_keep = ctx->d_size_keep;
+    A.rank = ctx->d_rank;
+    A.packed = ctx->packed_ok ? ctx->d_packed : nullptr;
+    A.votes = (unsigned long long*)d_votes_preorder;
+    A.g_w = ctx->d_prefix;
+    A.g_w2 = ctx->d_w2;
+    A.g_size = ctx->d_gsize;
+    A.g_next = ctx->d_next;
+    A.weight_out = (unsigned long long*)d_weight_out;
+    A.head_out = d_head_idx_out;
+    A.justified = justified_idx;
+    A.boost_idx = boost_idx;
+    A.boost_score = boost_score;
+    A.dbg = ctx->d_dbg;
+    const size_t base = ((size_t)A.n + 1) * 8 + (size_t)A.n * 8 + 8;
+    const size_t with_list = base + (size_t)A.n * 4;
+    A.use_smem = base <= 226 * 1024 && A.n <= 15 * 1024;
+    A.hard_list = A.use_smem && A.packed && with_list <= 226 * 1024;
+    return !A.use_smem ? 0 : A.hard_list ? with_list : base;
+}
+
+// Spins on the mapped (head, sequence) slot until the get_head kernel on `s` has published call `seq`.  Every 2^20 polls it checks that
+// the kernel is still alive; if it finished without publishing (should not happen), the head is copied from d_head instead.
+static int wait_head(b2_ctx* ctx, uint32_t seq, cudaStream_t s, const char* what, uint32_t* head_idx_out) {
+    volatile unsigned long long* slot64 = reinterpret_cast<volatile unsigned long long*>(ctx->h_head);
+    unsigned long long got = 0;
+    for (uint64_t spins = 0; (uint32_t)((got = *slot64) >> 32) != seq; spins++) {
+        if ((spins & 0xfffff) == 0xfffff) {
+            cudaError_t q = cudaStreamQuery(s);
+            if (q != cudaErrorNotReady && q != cudaSuccess) return fail_cuda(ctx, q, what);
+            if (q == cudaSuccess && (uint32_t)(*slot64 >> 32) != seq) {
+                uint32_t h = 0;
+                CK(cudaMemcpy(&h, ctx->d_head, 4, cudaMemcpyDeviceToHost));
+                *head_idx_out = h;
+                return B2_OK;
+            }
+        }
+    }
+    *head_idx_out = (uint32_t)got;
+    return B2_OK;
+}
+
 int b2_vote_weights_range_dev(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, uint64_t* d_votes_preorder, void* stream) {
     B2_NVTX;
     REQUIRE(ctx && d_votes_preorder, "vote_weights_dev: bad arguments");
@@ -1336,20 +1328,15 @@ int b2_vote_weights_range_dev(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, uin
     REQUIRE(v_begin <= v_end && v_end <= ctx->n_val, "vote_weights_range: validator range outside the registry");
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
-    const uint64_t n = v_end - v_begin;
+    const ghost_votes_args V = votes_args(ctx, v_begin, v_end);
     const size_t bins_bytes = (size_t)ctx->n_blocks * 8;
-    if (n == 0) {
-        // nothing to scatter; the accumulator is clean by contract
-    } else if (bins_bytes <= 200 * 1024) {
-        const unsigned grid = (unsigned)std::min<uint64_t>((uint64_t)ctx->n_sm, (n + 1023) / 1024);
-        k_ghost_votes_smem<<<grid, 1024, bins_bytes, s>>>(n, ctx->d_lmd_key + v_begin, ctx->d_lmd_block + v_begin, ctx->d_equiv + v_begin, ctx->d_flags + v_begin,
-                                                         ctx->d_eff + v_begin, ctx->d_pre, ctx->n_blocks, (unsigned long long*)d_votes_preorder, ctx->fc_min_key, 1u,
-                                                         ctx->fc_exclude_slashed ? 3u : 1u);
-        CKL(ctx);
-    } else {
-        k_ghost_votes<<<blocks_for(n, 256), 256, 0, s>>>(n, ctx->d_lmd_key + v_begin, ctx->d_lmd_block + v_begin, ctx->d_equiv + v_begin, ctx->d_flags + v_begin,
-                                                         ctx->d_eff + v_begin, ctx->d_pre, ctx->n_blocks, (unsigned long long*)d_votes_preorder, ctx->fc_min_key, 1u,
-                                                         ctx->fc_exclude_slashed ? 3u : 1u);
+    if (V.n > 0) {          // else nothing to scatter; the accumulator is clean by contract
+        // the bins in shared memory when they fit (a persistent grid of at most one CTA per SM), else the global-atomic form
+        const bool smem = bins_bytes <= 200 * 1024;
+        const unsigned grid = smem ? (unsigned)std::min<uint64_t>((uint64_t)ctx->n_sm, (V.n + 1023) / 1024) : blocks_for(V.n, 256);
+        (smem ? k_ghost_votes_smem : k_ghost_votes)<<<grid, smem ? 1024 : 256, smem ? bins_bytes : 0, s>>>(
+            V.n, V.lmd_key, V.lmd_block, V.equiv, V.flags, V.eff, ctx->d_pre, ctx->n_blocks, (unsigned long long*)d_votes_preorder, V.min_key, V.flag_need,
+            V.flag_mask);
         CKL(ctx);
     }
     CK(cudaEventRecord(ctx->ev_votes_done, s));
@@ -1370,28 +1357,8 @@ int b2_head_from_votes_dev(b2_ctx* ctx, uint64_t* d_votes_preorder, uint32_t jus
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
     ghost_tree_args A;
-    A.n = ctx->n_blocks;
-    A.pre = ctx->d_pre;
-    A.inv = ctx->d_inv;
-    A.size_keep = ctx->d_size_keep;
-    A.rank = ctx->d_rank;
-    A.packed = ctx->packed_ok ? ctx->d_packed : nullptr;
-    A.votes = (unsigned long long*)d_votes_preorder;
-    A.g_w = ctx->d_prefix;
-    A.g_w2 = ctx->d_w2;
-    A.g_size = ctx->d_gsize;
-    A.g_next = ctx->d_next;
-    A.weight_out = (unsigned long long*)d_weight_out;
-    A.head_out = d_head_idx_out;
-    A.justified = justified_idx;
-    A.boost_idx = boost_idx;
-    A.boost_score = boost_score;
-    size_t smem = ((size_t)A.n + 1) * 8 + (size_t)A.n * 8 + 8;
-    A.use_smem = smem <= 226 * 1024 && A.n <= 15 * 1024;   // 227 KB per block minus the kernel's static shared memory
-    A.dbg = ctx->d_dbg;
-    A.hard_list = 0;
-    if (A.use_smem && A.packed) smem = tree_smem_bytes(A);
-    k_ghost_tree<<<1, 1024, A.use_smem ? smem : 0, s>>>(A);
+    const size_t smem = fill_tree_args(ctx, A, d_votes_preorder, justified_idx, boost_idx, boost_score, d_weight_out, d_head_idx_out);
+    k_ghost_tree<<<1, 1024, smem, s>>>(A);
     CKL(ctx);
     return B2_OK;
 }
@@ -1408,9 +1375,6 @@ int b2_get_weights(b2_ctx* ctx, int32_t boost_idx, uint64_t boost_score, uint64_
     CK(cudaStreamSynchronize(s));
     return B2_OK;
 }
-
-static void fill_tree_args(b2_ctx* ctx, ghost_tree_args& A, uint64_t* d_votes_preorder, uint32_t justified_idx, int32_t boost_idx, uint64_t boost_score,
-                           uint64_t* d_weight_out, uint32_t* d_head_idx_out);
 
 // ---- multi-GPU get_head with the all-reduce fused in over NVLink peer memory (k_get_head_fused_nvl)
 static size_t fc_acc_bytes(uint32_t n_blocks) { return ((size_t)2 * n_blocks * 8 + 255) & ~(size_t)255; }
@@ -1467,11 +1431,9 @@ int b2_get_head_multi(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, uint32_t ju
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->s_main;
     ghost_tree_args A;
-    fill_tree_args(ctx, A, (uint64_t*)ctx->d_votes, justified_idx, boost_idx, boost_score, nullptr, ctx->d_head);
+    const size_t smem = fill_tree_args(ctx, A, (uint64_t*)ctx->d_votes, justified_idx, boost_idx, boost_score, nullptr, ctx->d_head);
     REQUIRE(A.use_smem && A.packed, "get_head_multi: the tree does not fit the shared-memory form (< ~14 500 blocks)");
-    const uint64_t n = v_end - v_begin;
-    ghost_votes_args V = {n, ctx->d_lmd_key + v_begin, ctx->d_lmd_block + v_begin, ctx->d_equiv + v_begin, ctx->d_flags + v_begin, ctx->d_eff + v_begin,
-                          ctx->fc_min_key, 1u, ctx->fc_exclude_slashed ? 3u : 1u};
+    const ghost_votes_args V = votes_args(ctx, v_begin, v_end);
     ghost_peer_args P;
     const uint32_t seq = ++ctx->fc_seq ? ctx->fc_seq : ++ctx->fc_seq;                  // the collective call number (same on every rank)
     const uint32_t hseq = ++ctx->head_seq ? ctx->head_seq : ++ctx->head_seq;            // this context's host-slot sequence number
@@ -1482,45 +1444,11 @@ int b2_get_head_multi(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, uint32_t ju
     P.rank = (uint32_t)ctx->fc_rank;
     P.world = (uint32_t)ctx->fc_world;
     P.seq = seq;
-    const size_t smem = tree_smem_bytes(A);
-    const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)ctx->n_sm, (n + 1023) / 1024));
+    const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)ctx->n_sm, (V.n + 1023) / 1024));
     k_get_head_fused_nvl<<<grid, 1024, smem, s>>>(V, A, P, ctx->d_ticket, (unsigned long long*)ctx->d_votes, ctx->d_head_host, hseq);
     CKL(ctx);
     CK(cudaEventRecord(ctx->ev_votes_done, s));
-    volatile unsigned long long* slot64 = reinterpret_cast<volatile unsigned long long*>(ctx->h_head);
-    unsigned long long got = 0;
-    for (uint64_t spins = 0; (uint32_t)((got = *slot64) >> 32) != hseq; spins++) {
-        if ((spins & 0xfffff) == 0xfffff) {
-            cudaError_t q = cudaStreamQuery(s);
-            if (q != cudaErrorNotReady && q != cudaSuccess) return fail_cuda(ctx, q, "get_head_multi kernel");
-        }
-    }
-    *head_idx_out = (uint32_t)got;
-    return B2_OK;
-}
-
-static void fill_tree_args(b2_ctx* ctx, ghost_tree_args& A, uint64_t* d_votes_preorder, uint32_t justified_idx, int32_t boost_idx, uint64_t boost_score,
-                           uint64_t* d_weight_out, uint32_t* d_head_idx_out) {
-    A.n = ctx->n_blocks;
-    A.pre = ctx->d_pre;
-    A.inv = ctx->d_inv;
-    A.size_keep = ctx->d_size_keep;
-    A.rank = ctx->d_rank;
-    A.packed = ctx->packed_ok ? ctx->d_packed : nullptr;
-    A.votes = (unsigned long long*)d_votes_preorder;
-    A.g_w = ctx->d_prefix;
-    A.g_w2 = ctx->d_w2;
-    A.g_size = ctx->d_gsize;
-    A.g_next = ctx->d_next;
-    A.weight_out = (unsigned long long*)d_weight_out;
-    A.head_out = d_head_idx_out;
-    A.justified = justified_idx;
-    A.boost_idx = boost_idx;
-    A.boost_score = boost_score;
-    const size_t smem = ((size_t)A.n + 1) * 8 + (size_t)A.n * 8 + 8;
-    A.use_smem = smem <= 226 * 1024 && A.n <= 15 * 1024;   // 227 KB per block minus the kernel's static shared memory
-    A.dbg = ctx->d_dbg;
-    A.hard_list = 0;
+    return wait_head(ctx, hseq, s, "get_head_multi kernel", head_idx_out);
 }
 
 // Diagnostics: SM-clock stamps (clock64) of the phases of the LAST b2_get_head / b2_head_from_votes_dev of this context: out32[0..7] =
@@ -1542,34 +1470,17 @@ int b2_get_head(b2_ctx* ctx, uint32_t justified_idx, int32_t boost_idx, uint64_t
     int rc;
     cudaStream_t s = ctx->s_main;
     ghost_tree_args A;
-    fill_tree_args(ctx, A, (uint64_t*)ctx->d_votes, justified_idx, boost_idx, boost_score, nullptr, ctx->d_head);
+    const size_t smem = fill_tree_args(ctx, A, (uint64_t*)ctx->d_votes, justified_idx, boost_idx, boost_score, nullptr, ctx->d_head);
     if (ctx->head_fused && A.use_smem && A.packed) {
         // one launch; the kernel writes (head, sequence) into mapped pinned memory and the host spins on the sequence number
         CK(cudaSetDevice(ctx->device));
-        ghost_votes_args V = {ctx->n_val, ctx->d_lmd_key, ctx->d_lmd_block, ctx->d_equiv, ctx->d_flags, ctx->d_eff, ctx->fc_min_key, 1u,
-                              ctx->fc_exclude_slashed ? 3u : 1u};
+        const ghost_votes_args V = votes_args(ctx, 0, ctx->n_val);
         const uint32_t seq = ++ctx->head_seq ? ctx->head_seq : ++ctx->head_seq;       // never 0
-        const size_t smem = tree_smem_bytes(A);
-        const unsigned grid = (unsigned)std::min<uint64_t>((uint64_t)ctx->n_sm, (ctx->n_val + 1023) / 1024);
+        const unsigned grid = (unsigned)std::min<uint64_t>((uint64_t)ctx->n_sm, (V.n + 1023) / 1024);
         k_get_head_fused<<<grid, 1024, smem, s>>>(V, A, ctx->d_ticket, ctx->d_head_host, seq);
         CKL(ctx);
         CK(cudaEventRecord(ctx->ev_votes_done, s));
-        volatile unsigned long long* slot64 = reinterpret_cast<volatile unsigned long long*>(ctx->h_head);
-        unsigned long long got = 0;
-        for (uint64_t spins = 0; (uint32_t)((got = *slot64) >> 32) != seq; spins++) {
-            if ((spins & 0xfffff) == 0xfffff) {                 // every ~1M polls: has the kernel died?
-                cudaError_t q = cudaStreamQuery(s);
-                if (q != cudaErrorNotReady && q != cudaSuccess) return fail_cuda(ctx, q, "get_head kernel");
-                if (q == cudaSuccess && (uint32_t)(*slot64 >> 32) != seq) {    // finished without publishing: should not happen; fall back to a copy
-                    uint32_t h = 0;
-                    CK(cudaMemcpy(&h, ctx->d_head, 4, cudaMemcpyDeviceToHost));
-                    *head_idx_out = h;
-                    return B2_OK;
-                }
-            }
-        }
-        *head_idx_out = (uint32_t)got;
-        return B2_OK;
+        return wait_head(ctx, seq, s, "get_head kernel", head_idx_out);
     }
     if ((rc = b2_vote_weights_dev(ctx, (uint64_t*)ctx->d_votes, s))) return rc;
     if ((rc = b2_head_from_votes_dev(ctx, (uint64_t*)ctx->d_votes, justified_idx, boost_idx, boost_score, nullptr, ctx->d_head, s))) return rc;

@@ -249,7 +249,7 @@ HD void g1_compress(const g1_jac& p, uint8_t* out) {
 }
 
 // 96 bytes (x.c1 || x.c0) -> affine G2 point.  On-curve implied; subgroup NOT checked.
-HDN int g2_decompress(const uint8_t* in, g2_aff& out, uint32_t* tab = nullptr, uint32_t tab_stride = 0) {
+HDN int g2_decompress(const uint8_t* in, g2_aff& out) {
     fp x1c, x0c;
     uint8_t b0;
 #if defined(__CUDA_ARCH__) && defined(B2_SIG_VECTOR_LOADS)
@@ -284,7 +284,7 @@ HDN int g2_decompress(const uint8_t* in, g2_aff& out, uint32_t* tab = nullptr, u
     x.c0 = fp_to_mont(x0c);
     x.c1 = fp_to_mont(x1c);
     fp2 y;
-    if (!fp2_sqrt(fp2_add(fp2_mul(fp2_sqr(x), x), fp2_load_const(C_B2)), y, tab, tab_stride)) return DEC_BAD;
+    if (!fp2_sqrt(fp2_add(fp2_mul(fp2_sqr(x), x), fp2_load_const(C_B2)), y)) return DEC_BAD;
     if (fp2_is_lex_large(y) != ((b0 & 0x20) != 0)) y = fp2_neg(y);
     out.x = x;
     out.y = y;

@@ -319,26 +319,14 @@ HD fp fp_mul8(const fp& a) { return fp_dbl(fp_mul4(a)); }
 // window-4 parse of round 1 needed 376 + 85, the fixed-window version 380 + 106.
 // Where the eight odd powers live.  pow_tbl_local: a per-thread array -- dynamically indexed, so the compiler puts it in LOCAL memory
 // (384 B per thread; with 16 resident warps per SM these tables overflow L1 and their evicted lines are what made k_g2_decompress
-// write 1.2 GB to DRAM per launch, as measured on an earlier GPU).  pow_tbl_strided: caller-provided SHARED memory, word (i, limb) of
-// thread t at base[(12 i + limb) * stride + t]: conflict-free, never leaves the SM.
+// write 1.2 GB to DRAM per launch, as measured on an earlier GPU).  A shared-memory form of the table (108 words per thread,
+// conflict-free) was measured and dropped: it halved the decompression's DRAM traffic (1.40 -> 0.73 GB per launch), but its 48 KB
+// per block competed with the tail kernels' shared memory under the epoch pipeline, and the step was 0.6 ms slower there (36.11 vs
+// 35.48 ms, on an earlier GPU).
 struct pow_tbl_local {
     fp t[9];
     HD void set(int i, const fp& v) { t[i] = v; }
     HD fp get(uint32_t i) const { return t[i]; }
-};
-struct pow_tbl_strided {
-    uint32_t* base;
-    uint32_t stride;
-    HD void set(int i, const fp& v) {
-#pragma unroll
-        for (int k = 0; k < 12; k++) base[(12 * i + k) * stride] = v.l[k];
-    }
-    HD fp get(uint32_t i) const {
-        fp r;
-#pragma unroll
-        for (int k = 0; k < 12; k++) r.l[k] = base[(12 * i + k) * stride];
-        return r;
-    }
 };
 template <class TBL> HDN fp fp_pow_prog_t(const fp& a, int off, TBL& tbl) {
     const uint32_t* prog = const_table() + off;
@@ -370,12 +358,7 @@ template <class TBL> HDN fp fp_pow_prog_t(const fp& a, int off, TBL& tbl) {
     }
     return r;
 }
-// tab == nullptr: table in a per-thread array; else 108 words per thread (nine entries) in shared memory at tab[(12 i + limb) * tab_stride]
-HD fp fp_pow_prog(const fp& a, int off, uint32_t* tab = nullptr, uint32_t tab_stride = 0) {
-    if (tab) {
-        pow_tbl_strided t = {tab, tab_stride};
-        return fp_pow_prog_t(a, off, t);
-    }
+HD fp fp_pow_prog(const fp& a, int off) {
     pow_tbl_local t;
     return fp_pow_prog_t(a, off, t);
 }
@@ -384,7 +367,7 @@ HD fp fp_inv(const fp& a) { return fp_pow_prog(a, C_PROG_PM2); }        // 0 -> 
 
 // d = a^((p-3)/4).  Then a*d = a^((p+1)/4) is the square-root candidate and, when a is a
 // non-zero square, d = 1/sqrt(a).
-HD fp fp_pow_pm3d4(const fp& a, uint32_t* tab = nullptr, uint32_t tab_stride = 0) { return fp_pow_prog(a, C_PROG_PM3D4, tab, tab_stride); }
+HD fp fp_pow_pm3d4(const fp& a) { return fp_pow_prog(a, C_PROG_PM3D4); }
 
 // sqrt in Fp: returns true and writes a root when `a` is a square
 HD bool fp_sqrt(const fp& a, fp& root) {

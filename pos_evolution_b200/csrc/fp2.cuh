@@ -114,7 +114,7 @@ HDN fp2 fp2_inv(const fp2& a) {
 //   If x^2 == t:  root = x + (a1*d/2) i          (d = 1/x)
 //   else       :  root = (a1*d/2) - x i          (d^2 = -1/t, so (a1*d/2)^2 = (a0 - s)/2)
 // Returns false when `a` is not a square.  Any root; callers fix the sign.
-HDN bool fp2_sqrt(const fp2& a, fp2& r, uint32_t* tab = nullptr, uint32_t tab_stride = 0) {
+HDN bool fp2_sqrt(const fp2& a, fp2& r) {
     if (fp_is_zero(a.c1)) {                      // a in Fp: always a square in Fp2
         fp x;
         bool qr = fp_sqrt(a.c0, x);              // x = a0^((p+1)/4); x^2 = -a0 when a0 is a non-residue
@@ -123,11 +123,11 @@ HDN bool fp2_sqrt(const fp2& a, fp2& r, uint32_t* tab = nullptr, uint32_t tab_st
         return true;
     }
     fp n = fp_add(fp_sqr(a.c0), fp_sqr(a.c1));
-    fp s = fp_mul(fp_pow_pm3d4(n, tab, tab_stride), n);
+    fp s = fp_mul(fp_pow_pm3d4(n), n);
     if (!fp_eq(fp_sqr(s), n)) return false;
     fp half = fp_load_const(C_TWO_INV);
     fp t = fp_mul(fp_add(a.c0, s), half);
-    fp d = fp_pow_pm3d4(t, tab, tab_stride);
+    fp d = fp_pow_pm3d4(t);
     fp x = fp_mul(d, t);
     fp y = fp_mul(fp_mul(a.c1, half), d);
     bool direct = fp_eq(fp_sqr(x), t);

@@ -128,65 +128,18 @@ __global__ void __launch_bounds__(128) k_g1_segment_sum(const uint32_t* __restri
 
 // ------------------------------------------------------------------------------------------ K3: bls.Aggregate
 // stage 1: one thread per signature: ZCash decode + Fp2 square root (two Fp exponentiations) -> affine point
-// use_smem != 0: the sliding-window tables of the two exponentiations live in dynamic shared memory (108 words per thread, launch with
-// 432 B * blockDim.x) instead of local memory -- see pow_tbl_strided in fp.cuh
-__global__ void __launch_bounds__(128, 4) k_g2_decompress(const uint8_t* __restrict__ sig96, uint64_t n, uint32_t* aff_out, uint8_t* st_out, int use_smem) {
-    extern __shared__ uint32_t pow_tab[];
+__global__ void __launch_bounds__(128, 4) k_g2_decompress(const uint8_t* __restrict__ sig96, uint64_t n, uint32_t* aff_out, uint8_t* st_out) {
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     g2_aff s;
     s.x = fp2_zero();
     s.y = fp2_zero();
-    int st = g2_decompress(sig96 + 96 * i, s, use_smem ? pow_tab + threadIdx.x : nullptr, blockDim.x);
+    int st = g2_decompress(sig96 + 96 * i, s);
     uint4* o = reinterpret_cast<uint4*>(aff_out + 48 * i);
     const uint32_t* w = reinterpret_cast<const uint32_t*>(&s);
 #pragma unroll
     for (int k = 0; k < 12; k++) o[k] = make_uint4(w[4 * k], w[4 * k + 1], w[4 * k + 2], w[4 * k + 3]);
     st_out[i] = (uint8_t)st;
-}
-// stage 1, pipelined form.  Same work, but as a PERSISTENT grid (4 blocks per SM -- these blocks fill the register file, so nothing
-// else fits beside them) whose warps take 32 signatures at a time from a global counter, and whose blocks EXIT at once when they
-// find themselves on one of the SMs named in `reserved` (bit i of word i/64 <-> %smid i).  The reserved SMs stay empty for the
-// pairing tail of the previous epochs (whose blocks fit nowhere else while this grid is resident): a tail warp that has a scheduler
-// to itself runs the multiply pipe at ~90 %, one that shares it with four decompression warps crawls and, worse, evicts them
-// (measured on an earlier GPU).  Which SM ends up doing how much is decided by the counter, not by the launch geometry.
-struct sm_mask {
-    unsigned long long w[4];
-};
-__global__ void __launch_bounds__(128, 4) k_g2_decompress_persistent(const uint8_t* __restrict__ sig96, uint64_t n, uint32_t* aff_out, uint8_t* st_out,
-                                                                      unsigned long long* counter, sm_mask reserved) {
-    uint32_t smid;
-    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-    if (smid < 256 && ((reserved.w[smid >> 6] >> (smid & 63)) & 1ull)) return;
-    const uint32_t lane = threadIdx.x & 31;
-    for (;;) {
-        unsigned long long base = 0;
-        if (lane == 0) base = atomicAdd(counter, 32ull);
-        base = __shfl_sync(0xffffffffu, base, 0);
-        if (base >= n) break;
-        const uint64_t i = base + lane;
-        if (i < n) {
-            g2_aff s;
-            s.x = fp2_zero();
-            s.y = fp2_zero();
-            int st = g2_decompress(sig96 + 96 * i, s);
-            uint4* o = reinterpret_cast<uint4*>(aff_out + 48 * i);
-            const uint32_t* w = reinterpret_cast<const uint32_t*>(&s);
-#pragma unroll
-            for (int k = 0; k < 12; k++) o[k] = make_uint4(w[4 * k], w[4 * k + 1], w[4 * k + 2], w[4 * k + 3]);
-            st_out[i] = (uint8_t)st;
-        }
-    }
-}
-// which SM ids exist on this device (b2_init: the reserved set is chosen among the ids actually seen)
-__global__ void k_probe_smid(unsigned int* seen) {
-    uint32_t smid;
-    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-    if (threadIdx.x == 0 && smid < 256) atomicOr(&seen[smid >> 5], 1u << (smid & 31));
-    // stay resident for a moment so that the grid spreads over every SM
-    const long long t0 = clock64();
-    while (clock64() - t0 < 20000) {
-    }
 }
 // stage 2: one WARP per segment (each lane adds every 32nd point, then a 5-round shuffle tree) -> Jacobian sum (72 words) + status.  The inversion needed for
 // the compressed encoding is NOT done here (127 threads would idle behind it): stage 3 does it with a thread per segment.
@@ -532,16 +485,24 @@ __global__ void __launch_bounds__(256) k_ghost_votes(uint64_t n, const unsigned 
     if (on && lane == __ffs(peers) - 1) atomicAdd(&votes[b], sum);
 }
 
+// The validators [v_begin, v_end) of a vote scatter: their latest-message, equivocation, flag and balance tables offset to v_begin
+// (n = v_end - v_begin), and the fork-choice variant (votes below min_key expire; flags & flag_mask must equal flag_need)
+struct ghost_votes_args {
+    uint64_t n;
+    const unsigned long long* lmd_key;
+    const uint32_t* lmd_block;
+    const uint8_t *equiv, *flags;
+    const uint64_t* eff;
+    unsigned long long min_key;
+    uint32_t flag_need, flag_mask;
+};
 // Same scatter with the per-block bins privatised in shared memory (used when n_blocks * 8 B fits): a persistent grid
 // of one CTA per SM strides over the validators; lanes of a warp voting for the same block are combined first, the
 // leader adds into the CTA's shared bins, and only non-zero bins are flushed to global memory -- one atomic per
 // (CTA, voted block) instead of one per (warp, voted block), which matters when a million validators agree on a
 // handful of recent blocks (the realistic case) and the global atomics would serialise on those addresses.
-__device__ __forceinline__ void ghost_votes_body(unsigned long long* bins, uint64_t n, const unsigned long long* __restrict__ lmd_key,
-                                                 const uint32_t* __restrict__ lmd_block, const uint8_t* __restrict__ equiv,
-                                                 const uint8_t* __restrict__ flags, const uint64_t* __restrict__ eff,
-                                                 const uint32_t* __restrict__ pre, uint32_t n_blocks, unsigned long long* votes, unsigned long long min_key, uint32_t flag_need, uint32_t flag_mask,
-                                                 unsigned long long* dbg = nullptr) {
+__device__ __forceinline__ void ghost_votes_body(unsigned long long* bins, const ghost_votes_args& V, const uint32_t* __restrict__ pre, uint32_t n_blocks,
+                                                 unsigned long long* votes, unsigned long long* dbg = nullptr) {
 #define B2_VOTE_STAMP(k) do { if (dbg && blockIdx.x == 0 && threadIdx.x == 0) dbg[k] = clock64(); } while (0)
     B2_VOTE_STAMP(16);
     for (uint32_t i = threadIdx.x; i < n_blocks; i += blockDim.x) bins[i] = 0;
@@ -549,7 +510,7 @@ __device__ __forceinline__ void ghost_votes_body(unsigned long long* bins, uint6
     B2_VOTE_STAMP(17);
     const int lane = threadIdx.x & 31;
     const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
-    const uint64_t n_round = (n + stride - 1) / stride * stride;            // whole warps stay converged for the shuffles
+    const uint64_t n_round = (V.n + stride - 1) / stride * stride;          // whole warps stay converged for the shuffles
     // Four validators per thread and trip: all twenty table loads (key, block, balance, flags, equivocation byte -- addresses depend on
     // the validator index only) are issued before the first is used, then the one dependent gather (block -> pre-order position, a
     // 40 KB table that lives in L1).  The round-1 form tested `key != 0 && ...` load by load, i.e. four dependent round trips per
@@ -561,18 +522,18 @@ __device__ __forceinline__ void ghost_votes_body(unsigned long long* bins, uint6
 #pragma unroll
         for (int u = 0; u < U; u++) {
             const uint64_t v = v0 + u * stride;
-            const bool in = v < n;
-            key[u] = in ? lmd_key[v] : 0ull;
-            blk[u] = in ? lmd_block[v] : 0u;
-            bal[u] = in ? eff[v] : 0ull;
-            fl[u] = in ? flags[v] : 0u;
-            eq[u] = in ? equiv[v] : 1u;
+            const bool in = v < V.n;
+            key[u] = in ? V.lmd_key[v] : 0ull;
+            blk[u] = in ? V.lmd_block[v] : 0u;
+            bal[u] = in ? V.eff[v] : 0ull;
+            fl[u] = in ? V.flags[v] : 0u;
+            eq[u] = in ? V.equiv[v] : 1u;
         }
         uint32_t b[U];
         bool on[U];
 #pragma unroll
         for (int u = 0; u < U; u++) {
-            on[u] = key[u] != 0 && key[u] >= min_key && !eq[u] && ((fl[u] & flag_mask) == flag_need) && blk[u] < n_blocks;
+            on[u] = key[u] != 0 && key[u] >= V.min_key && !eq[u] && ((fl[u] & V.flag_mask) == V.flag_need) && blk[u] < n_blocks;
             b[u] = on[u] ? pre[blk[u]] : 0xffffffffu;
         }
 #pragma unroll
@@ -602,12 +563,14 @@ __device__ __forceinline__ void ghost_votes_body(unsigned long long* bins, uint6
     }
     B2_VOTE_STAMP(19);
 }
+// The two scatter kernels take the tables as separate __restrict__ parameters rather than a ghost_votes_args: only a restrict-qualified
+// kernel parameter lets the compiler read them through the read-only path (LDG.CONSTANT).
 __global__ void __launch_bounds__(1024) k_ghost_votes_smem(uint64_t n, const unsigned long long* __restrict__ lmd_key,
                                                             const uint32_t* __restrict__ lmd_block, const uint8_t* __restrict__ equiv,
                                                             const uint8_t* __restrict__ flags, const uint64_t* __restrict__ eff,
                                                             const uint32_t* __restrict__ pre, uint32_t n_blocks, unsigned long long* votes, unsigned long long min_key, uint32_t flag_need, uint32_t flag_mask) {
     extern __shared__ unsigned long long bins[];
-    ghost_votes_body(bins, n, lmd_key, lmd_block, equiv, flags, eff, pre, n_blocks, votes, min_key, flag_need, flag_mask);
+    ghost_votes_body(bins, ghost_votes_args{n, lmd_key, lmd_block, equiv, flags, eff, min_key, flag_need, flag_mask}, pre, n_blocks, votes);
 }
 
 // ------------------------------------------------------------------------------------------ K9: subtree weights + head
@@ -1006,7 +969,7 @@ __device__ __forceinline__ void ghost_tree_smem(const ghost_tree_args& A, unsign
     __shared__ uint32_t warp_tot32[32];
     __shared__ uint32_t cells[2];                                           // head position, length of the work list
     if (A.n <= 11u * blockDim.x) ghost_tree_smem_t<11>(A, smem_u64, host_out, host_seq, warp_tot, warp_tot32, cells);
-    else ghost_tree_smem_t<15>(A, smem_u64, host_out, host_seq, warp_tot, warp_tot32, cells);      // n <= 15 * 1024: b2_head_from_votes_dev's use_smem test
+    else ghost_tree_smem_t<15>(A, smem_u64, host_out, host_seq, warp_tot, warp_tot32, cells);      // n <= 15 * 1024: fill_tree_args's use_smem test
 }
 
 __global__ void __launch_bounds__(1024) k_ghost_tree(ghost_tree_args A) {
@@ -1019,28 +982,25 @@ __global__ void __launch_bounds__(1024) k_ghost_tree(ghost_tree_args A) {
 // get_head in ONE launch (b2_get_head): every CTA scatters its share of the votes (K8), the CTA that finishes last -- elected by a
 // ticket counter -- runs the tree phase (K9) on the completed vote array and writes the head straight into mapped pinned host memory
 // (head, then a sequence number the host spins on): no second launch, no device-to-host copy, no stream synchronisation.
-struct ghost_votes_args {
-    uint64_t n;
-    const unsigned long long* lmd_key;
-    const uint32_t* lmd_block;
-    const uint8_t *equiv, *flags;
-    const uint64_t* eff;
-    unsigned long long min_key;
-    uint32_t flag_need, flag_mask;
-};
-__global__ void __launch_bounds__(1024) k_get_head_fused(ghost_votes_args V, ghost_tree_args A, unsigned int* ticket, uint32_t* host_out, uint32_t host_seq) {
-    extern __shared__ unsigned long long smem_u64[];
-    __shared__ bool is_last;
-    ghost_votes_body(smem_u64, V.n, V.lmd_key, V.lmd_block, V.equiv, V.flags, V.eff, A.pre, A.n, A.votes, V.min_key, V.flag_need, V.flag_mask, A.dbg);
+// Called by every thread after its CTA's scatter: true in the CTA whose ticket completes the grid, which re-arms the ticket for the
+// next call.  `is_last` is a __shared__ flag of the calling kernel (declared there, the kernel keeps its shared-memory layout).
+__device__ __forceinline__ bool last_cta(unsigned int* ticket, bool& is_last) {
     __syncthreads();                                   // every flush atomic of this CTA has been issued
     if (threadIdx.x == 0) {
         __threadfence();
         is_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
     }
     __syncthreads();
-    if (!is_last) return;
+    if (!is_last) return false;
     __threadfence();                                   // the other CTAs' vote atomics are visible (they live in L2)
     if (threadIdx.x == 0) *ticket = 0;                 // re-armed for the next call
+    return true;
+}
+__global__ void __launch_bounds__(1024) k_get_head_fused(ghost_votes_args V, ghost_tree_args A, unsigned int* ticket, uint32_t* host_out, uint32_t host_seq) {
+    extern __shared__ unsigned long long smem_u64[];
+    __shared__ bool is_last;
+    ghost_votes_body(smem_u64, V, A.pre, A.n, A.votes, A.dbg);
+    if (!last_cta(ticket, is_last)) return;
     ghost_tree_smem(A, smem_u64, host_out, host_seq);  // (the fused kernel is only launched for trees in the shared-memory form)
 }
 
@@ -1064,16 +1024,8 @@ __global__ void __launch_bounds__(1024) k_get_head_fused_nvl(ghost_votes_args V,
                                                               unsigned long long* local_votes, uint32_t* host_out, uint32_t host_seq) {
     extern __shared__ unsigned long long smem_u64[];
     __shared__ bool is_last;
-    ghost_votes_body(smem_u64, V.n, V.lmd_key, V.lmd_block, V.equiv, V.flags, V.eff, A.pre, A.n, local_votes, V.min_key, V.flag_need, V.flag_mask, A.dbg);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        is_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
-    }
-    __syncthreads();
-    if (!is_last) return;
-    __threadfence();
-    if (threadIdx.x == 0) *ticket = 0;
+    ghost_votes_body(smem_u64, V, A.pre, A.n, local_votes, A.dbg);
+    if (!last_cta(ticket, is_last)) return;
     const uint32_t par = P.seq & 1u, n = A.n;
     // push: this rank's direct votes into every rank's accumulator (own included); the local vector is left clean for the next call
     for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {

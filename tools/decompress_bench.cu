@@ -1,31 +1,21 @@
-// decompress_bench.cu -- A/B harness for the G2 decompression kernel body (two Fp exponentiations per signature), compiled against
-// whichever csrc/ tree -I points to.  -DVARIANT=0: window table in local memory; 1: in shared memory (needs the round-2 headers).
+// decompress_bench.cu -- timing harness for the G2 decompression kernel body (two Fp exponentiations per signature, window tables in
+// local memory), compiled against whichever csrc/ tree -I points to (A/B of two trees, or of -DB2_SIG_VECTOR_LOADS).
 // Inputs: 2^20 valid compressed G2 points (x = 1 + k*u scanned until on-curve), so both exponentiations run for every thread.
-// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -I pos_evolution_b200/csrc -DVARIANT=0 -o tools/decompress_bench_v0.bin tools/decompress_bench.cu
+// Build: nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -I pos_evolution_b200/csrc -o tools/decompress_bench.bin tools/decompress_bench.cu
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
 #include <cuda_runtime.h>
 #include "cores.cuh"
 using namespace b2;
-#ifndef VARIANT
-#define VARIANT 0
-#endif
 
 __global__ void __launch_bounds__(128, 4) k_dec(const uint8_t* __restrict__ sig96, uint64_t n, uint32_t* aff_out, uint8_t* st_out) {
-#if VARIANT == 1
-    extern __shared__ uint32_t pow_tab[];
-#endif
     uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     g2_aff s;
     s.x = fp2_zero();
     s.y = fp2_zero();
-#if VARIANT == 1
-    int st = g2_decompress(sig96 + 96 * i, s, pow_tab + threadIdx.x, blockDim.x);
-#else
     int st = g2_decompress(sig96 + 96 * i, s);
-#endif
     uint4* o = reinterpret_cast<uint4*>(aff_out + 48 * i);
     const uint32_t* w = reinterpret_cast<const uint32_t*>(&s);
 #pragma unroll
@@ -52,9 +42,7 @@ int main() {
     cudaMalloc(&d_st, cand);
     cudaMalloc(&d_aff, cand * 192);
     cudaMemcpy(d_sig, h.data(), cand * 96, cudaMemcpyHostToDevice);
-    const size_t smem = VARIANT == 1 ? 432 * 128 : 0;
-    if (smem) cudaFuncSetAttribute(k_dec, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    k_dec<<<(unsigned)((cand + 127) / 128), 128, smem>>>(d_sig, cand, d_aff, d_st);
+    k_dec<<<(unsigned)((cand + 127) / 128), 128>>>(d_sig, cand, d_aff, d_st);
     std::vector<uint8_t> st(cand);
     cudaMemcpy(st.data(), d_st, cand, cudaMemcpyDeviceToHost);
     std::vector<uint8_t> good(want * 96);
@@ -73,7 +61,7 @@ int main() {
     const int reps = 6;
     for (int r = 0; r < reps + 1; r++) {
         cudaEventRecord(e0);
-        k_dec<<<(unsigned)(want / 128), 128, smem>>>(d_sig, want, d_aff, d_st);
+        k_dec<<<(unsigned)(want / 128), 128>>>(d_sig, want, d_aff, d_st);
         cudaEventRecord(e1);
         cudaDeviceSynchronize();
         float ms;
@@ -90,7 +78,7 @@ int main() {
     cudaMemcpy(aff.data(), d_aff, aff.size() * 4, cudaMemcpyDeviceToHost);
     uint32_t chk = 0;
     for (uint32_t w : aff) chk = chk * 31 + w;
-    printf("{\"variant\": %d, \"n\": %llu, \"valid\": %llu, \"ms_mean\": %.3f, \"ms_best\": %.3f, \"checksum\": %u, \"cuda\": \"%s\"}\n", VARIANT, (unsigned long long)want,
+    printf("{\"n\": %llu, \"valid\": %llu, \"ms_mean\": %.3f, \"ms_best\": %.3f, \"checksum\": %u, \"cuda\": \"%s\"}\n", (unsigned long long)want,
            (unsigned long long)ok, sum / reps, best, chk, cudaGetErrorString(cudaGetLastError()));
     return 0;
 }
