@@ -250,7 +250,8 @@ int b2_fc_exchange_open(b2_ctx* ctx, int rank, int world, const uint8_t* handles
 int b2_get_head_multi(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, uint32_t justified_idx, int32_t boost_idx, uint64_t boost_score,
                       uint32_t* head_idx_out);
 uint32_t b2_tree_size(b2_ctx* ctx);
-/* profiling aid: SM-clock stamps of the phases of the context's last get_head (vote scatter of CTA 0, tree phases); u64[32] */
+/* profiling aid: SM-clock stamps of the phases of the context's last get_head (vote scatter of CTA 0, tree phases); u64[32].
+ * Reading clears them: a slot that no call since the last read has written reads 0. */
 int b2_debug_head_clocks(b2_ctx* ctx, uint64_t* out32);
 
 #ifdef __cplusplus

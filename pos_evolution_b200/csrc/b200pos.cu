@@ -1454,11 +1454,14 @@ int b2_get_head_multi(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, uint32_t ju
 // Diagnostics: SM-clock stamps (clock64) of the phases of the LAST b2_get_head / b2_head_from_votes_dev of this context: out32[0..7] =
 // tree phase boundaries (start, staged, scanned, weights, weights stored, marked, counted, head found), out32[15] = tree end,
 // out32[16..19] = vote scatter of CTA 0 (start, bins zeroed, scattered, flushed).  For profiling (tools/), not for results.
+// Only some forms write some slots (out32[3]: the shared-memory tree phase; out32[8]: its work-list marking; out32[16..19]: the one-launch
+// kernels), so reading clears the stamps: a slot that no call since the last read has written reads 0.
 int b2_debug_head_clocks(b2_ctx* ctx, uint64_t* out32) {
     REQUIRE(ctx && out32, "debug_head_clocks: bad arguments");
     CK(cudaSetDevice(ctx->device));
     CK(cudaDeviceSynchronize());
     CK(cudaMemcpy(out32, ctx->d_dbg, 32 * 8, cudaMemcpyDeviceToHost));
+    CK(cudaMemset(ctx->d_dbg, 0, 32 * 8));
     return B2_OK;
 }
 

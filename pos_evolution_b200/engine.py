@@ -302,7 +302,7 @@ class Engine:
         return int(out.value)
 
     def debug_head_clocks(self):
-        """clock64 stamps of the phases of the last get_head (profiling aid) -> uint64[32]"""
+        """clock64 stamps of the phases of the last get_head (profiling aid) -> uint64[32]; reading clears them (unwritten slots read 0)"""
         out = np.zeros(32, dtype=np.uint64)
         self._ck(self.lib.b2_debug_head_clocks(self.h, _p(out)))
         return out

@@ -107,6 +107,83 @@ def fork_tree(n_blocks: int, seed: int = 4):
     return parent, slot, roots, leaf_viable
 
 
+def _shape_roots(n_blocks: int, tag: bytes):
+    """distinct 32-byte roots whose lexicographic order is unrelated to the block index"""
+    return np.frombuffer(b"".join(_h(tag + i.to_bytes(8, "little")) for i in range(n_blocks)), dtype=np.uint8).reshape(n_blocks, 32).copy()
+
+
+def leaves(parent):
+    """bool[n]: True where the block has no child"""
+    has_child = np.zeros(len(parent), dtype=bool)
+    has_child[np.asarray(parent[1:], dtype=np.int64)] = True
+    return ~has_child
+
+
+def depths(parent):
+    d = np.zeros(len(parent), dtype=np.int64)
+    for i in range(1, len(parent)):
+        d[i] = d[parent[i]] + 1
+    return d
+
+
+def deep_side_leaf(parent) -> int:
+    """the deepest leaf other than the last block (the lowest index among equals); the last block when it is the only leaf"""
+    leaf = leaves(parent)
+    leaf[len(parent) - 1] = leaf[len(parent) - 1] and leaf.sum() == 1
+    d = np.where(leaf, depths(parent), -1)
+    return int(np.argmax(d))
+
+
+def tree_shape(shape: str, n_blocks: int, viability: str = "random", seed: int = 5):
+    """Block trees of the adversarial shapes for the fork-choice kernels, in topological order (parent[b] < b) with distinct roots:
+      chain   parent[i] = i - 1 (depth n - 1);
+      star    block 0 with n - 1 children;
+      broom   a chain of n - n//2 blocks ending in a fan of n//2 leaves;
+      binary  complete binary tree, parent[i] = (i - 1) // 2;
+      random  parent[i] ~ U[0, i);
+      comb    a chain (the even blocks) with one leaf (the odd blocks) hanging off every chain block.
+    viability: "random" (95 % of the leaves viable), "all", "none" (no leaf viable) or "deep" (only deep_side_leaf viable).
+    -> (parent u32[n], slot u64[n], roots u8[n, 32], leaf_viable u8[n])"""
+    rng = np.random.default_rng(seed)
+    i = np.arange(n_blocks, dtype=np.int64)
+    if shape == "chain":
+        parent = np.maximum(i - 1, 0)
+    elif shape == "star":
+        parent = np.zeros(n_blocks, dtype=np.int64)
+    elif shape == "broom":
+        stem = n_blocks - n_blocks // 2
+        parent = np.where(i < stem, np.maximum(i - 1, 0), stem - 1)
+    elif shape == "binary":
+        parent = np.maximum((i - 1) // 2, 0)
+    elif shape == "random":
+        parent = np.zeros(n_blocks, dtype=np.int64)
+        parent[1:] = rng.integers(0, i[1:])
+    elif shape == "comb":
+        parent = np.where(i % 2 == 1, i - 1, np.maximum(i - 2, 0))
+    else:
+        raise ValueError(shape)
+    parent = parent.astype(np.uint32)
+    parent[0] = 0
+    slot = (depths(parent) + 1).astype(np.uint64)
+    slot[0] = 0
+    roots = _shape_roots(n_blocks, shape.encode() + seed.to_bytes(4, "little"))
+    if viability == "random":
+        leaf_viable = (rng.random(n_blocks) >= 0.05).astype(np.uint8)
+    elif viability == "all":
+        leaf_viable = np.ones(n_blocks, dtype=np.uint8)
+    elif viability == "none":
+        leaf_viable = np.zeros(n_blocks, dtype=np.uint8)
+    elif viability == "deep":
+        leaf_viable = np.zeros(n_blocks, dtype=np.uint8)
+        leaf_viable[deep_side_leaf(parent)] = 1
+    else:
+        raise ValueError(viability)
+    return parent, slot, roots, leaf_viable
+
+
+TREE_SHAPES = ("chain", "star", "broom", "binary", "random", "comb")
+
+
 def votes(n_validators: int, n_blocks: int, seed: int = 4):
     rng = np.random.default_rng(seed + 1000)
     msg_block = (n_blocks - 1 - np.minimum(n_blocks - 1, rng.geometric(0.002, size=n_validators))).astype(np.uint32)

@@ -25,7 +25,11 @@ def _registry(eng, n, eff, active):
     eng.registry_load(pk, eff, active)
 
 
-@pytest.mark.parametrize("n_val,n_blk,seed", [(64, 1, 1), (64, 2, 2), (1000, 50, 3), (5000, 300, 4), (1 << 20, 10000, 4), (3000, 14000, 6), (3000, 20000, 7)])
+@pytest.mark.parametrize("n_val,n_blk,seed", [(64, 1, 1), (64, 2, 2), (1000, 50, 3), (5000, 300, 4), (1 << 20, 10000, 4), (3000, 14000, 6), (3000, 20000, 7),
+                                              # the edges of every form of the tree phase and the vote scatter (tests/test_gpu_forkchoice_forms.py)
+                                              (64, 3, 8), (3000, 1023, 9), (3000, 1024, 10), (3000, 1025, 11), (3000, 11264, 12), (3000, 11265, 13),
+                                              (3000, 11570, 14), (3000, 11571, 15), (3000, 14463, 16), (3000, 14464, 17), (3000, 25600, 18),
+                                              (3000, 25601, 19), (3000, 32767, 20), (3000, 32768, 21), (3000, 65537, 22)])
 def test_weights_and_head(eng, n_val, n_blk, seed):
     parent, slot, roots, leaf_viable = scenarios.fork_tree(n_blk, seed)
     msg_block, has_msg, equiv, active, eff = scenarios.votes(n_val, n_blk, seed)

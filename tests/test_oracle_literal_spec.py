@@ -157,6 +157,120 @@ def test_get_head_literal_vs_oracle_vs_numpy(env):
     assert rb[fast.ghost_head(parent, roots, keep, w, 0)] == head_lit
 
 
+def _shape_store(state, parent, slot, roots, leaf_viable, justified, boost_idx, msg_block, has_msg, equiv):
+    """A Store holding the block tree of scenarios.tree_shape with store.justified_checkpoint on block `justified`: the leaves that
+    leaf_viable marks non-viable carry a different current_justified_checkpoint in their block state (get_filtered_block_tree's test),
+    the others the store's.  Latest messages, equivocations and the proposer boost (boost_idx < 0: none) as the array form has them."""
+    rb = [bytes(r) for r in roots]
+    just = S.Checkpoint(1, rb[justified])
+    fin = S.Checkpoint(1, rb[0])
+    store = S.Store(time=0, genesis_time=0, justified_checkpoint=just, finalized_checkpoint=fin, best_justified_checkpoint=just,
+                    proposer_boost_root=rb[boost_idx] if boost_idx >= 0 else S.ZERO32,
+                    equivocating_indices=set(int(v) for v in np.nonzero(equiv)[0]))
+    leaf = scenarios.leaves(parent)
+    for b in range(len(rb)):
+        store.blocks[rb[b]] = S.BeaconBlock(int(slot[b]), rb[parent[b]] if b else bytes(32))
+        bs = copy.copy(state)
+        bs.current_justified_checkpoint = S.Checkpoint(0, b"\x01" * 32) if leaf[b] and not leaf_viable[b] else just
+        bs.finalized_checkpoint = fin
+        store.block_states[rb[b]] = bs
+    store.checkpoint_states[just] = state
+    for v in np.nonzero(has_msg)[0]:
+        store.latest_messages[int(v)] = S.LatestMessage(1, rb[msg_block[v]])
+    return store
+
+
+def _shape_cases(shape, n):
+    """(viability, justified, boost_idx, votes) combinations of test_fast_vs_spec_on_tree_shapes for one tree shape"""
+    parent = scenarios.tree_shape(shape, n)[0]
+    leaf = scenarios.leaves(parent)
+    inner = [b for b in range(1, n) if not leaf[b]]
+    mid = inner[len(inner) // 2] if inner else 0                   # a justified block other than 0 with a subtree below it
+    first_leaf = int(np.nonzero(leaf)[0][0])
+    return [("random", 0, -1, "random"), ("random", 0, n - 1, "random"), ("random", mid, n - 1, "random"), ("random", mid, mid, "tie"),
+            ("all", 0, -1, "tie"), ("all", mid, -1, "tie"), ("all", 0, first_leaf, "tie"), ("none", 0, n - 1, "random"),
+            ("none", mid, -1, "tie"), ("deep", 0, -1, "random"), ("deep", 0, -1, "tie"), ("deep", mid, 0, "tie"),
+            ("random", first_leaf, -1, "random"), ("deep", n - 1, n - 1, "random")]
+
+
+def _shape_votes(parent, roots, kind, n_val, justified, rng):
+    """random: 90 % of the validators vote for a uniformly drawn block.  tie: the two children of the justified block's first
+    multi-child descendant with the highest roots (or of any multi-child block) get the same non-zero weight -- equal numbers of
+    validators, all of equal balance (the caller's), voting for blocks inside each child's subtree -- so get_head's root tie-break decides.
+    -> (msg_block, has_msg, the tied pair or None)"""
+    n = len(parent)
+    msg_block = np.zeros(n_val, dtype=np.uint32)
+    has_msg = np.zeros(n_val, dtype=np.uint8)
+    if kind == "random":
+        has_msg[:] = rng.random(n_val) < 0.9
+        msg_block[:] = rng.integers(0, n, size=n_val)
+        return msg_block, has_msg, None
+    children = [[] for _ in range(n)]
+    for b in range(1, n):
+        children[parent[b]].append(b)
+    below = set()
+    todo = [justified]
+    while todo:
+        b = todo.pop()
+        below.add(b)
+        todo += children[b]
+    forks = [b for b in sorted(below) if len(children[b]) >= 2] or [b for b in range(n) if len(children[b]) >= 2]
+    if not forks:
+        return msg_block, has_msg, None                               # a chain has no siblings: all weights zero
+    kids = sorted(children[forks[0]], key=lambda c: bytes(roots[c]))[-2:]
+    for side, c in enumerate(kids):
+        sub = [c]
+        for b in range(c + 1, n):                                    # topological order: a block's subtree lies behind it
+            if parent[b] in sub:
+                sub.append(b)
+        for v in range(side, n_val, 2):
+            has_msg[v] = 1
+            msg_block[v] = sub[int(rng.integers(0, len(sub)))]
+    return msg_block, has_msg, kids
+
+
+@pytest.mark.parametrize("shape", scenarios.TREE_SHAPES)
+def test_fast_vs_spec_on_tree_shapes(env, shape):
+    """The numpy array form (fast.ghost_weights / ghost_viable / ghost_head), which the GPU fork-choice tests trust on the adversarial tree
+    shapes of scenarios.tree_shape, against the oracle's spec restatement (get_weight / get_filtered_block_tree / get_head) on the same
+    trees at 40 blocks: every viability mode, a justified block other than 0 (inner block, leaf, last block), with and without the
+    proposer boost (also on the justified block and on a block outside its subtree), and siblings tied at non-zero weight."""
+    spec, state0, _ = env
+    n, n_val = 40, 64
+    rng = np.random.default_rng(len(shape))
+    for case, (viability, justified, boost_idx, kind) in enumerate(_shape_cases(shape, n)):
+        state = copy.deepcopy(state0)
+        parent, slot, roots, leaf_viable = scenarios.tree_shape(shape, n, viability, seed=case)
+        if kind == "tie":
+            for v in state.validators:
+                v.effective_balance = 32 * 10**9
+        else:
+            state.validators[5].exit_epoch = 0                        # an inactive validator is not counted
+        msg_block, has_msg, tied = _shape_votes(parent, roots, kind, n_val, justified, rng)
+        equiv = np.zeros(n_val, dtype=np.uint8)
+        if kind == "random":
+            equiv[[3, 17]] = 1
+        eff = np.array([v.effective_balance for v in state.validators], dtype=np.uint64)
+        active = np.array([spec.is_active_validator(v, spec.get_current_epoch(state)) for v in state.validators], dtype=np.uint8)
+        boost = fast.proposer_boost_score(eff, active, spec.p.SLOTS_PER_EPOCH, spec.p.PROPOSER_SCORE_BOOST) if boost_idx >= 0 else 0
+        store = _shape_store(state, parent, slot, roots, leaf_viable, justified, boost_idx, msg_block, has_msg, equiv)
+        rb = [bytes(r) for r in roots]
+        w = fast.ghost_weights(parent, msg_block, has_msg, eff, active, equiv, boost_idx, boost)
+        assert [int(x) for x in w] == [spec.get_weight(store, r) for r in rb], (shape, case)
+        keep = fast.ghost_viable(parent, leaf_viable)
+        filtered = spec.get_filtered_block_tree(store)
+        below = {justified}
+        for b in range(justified + 1, n):
+            if parent[b] in below:
+                below.add(b)
+        assert set(rb[b] for b in below if keep[b]) == set(filtered.keys()), (shape, case)
+        head = fast.ghost_head(parent, roots, keep, w, justified)
+        assert rb[head] == spec.get_head(store), (shape, case)
+        if tied is not None:                                          # the tie the case was built for is there (before the boost)
+            w0 = fast.ghost_weights(parent, msg_block, has_msg, eff, active, equiv, -1, 0)
+            assert w0[tied[0]] == w0[tied[1]] > 0, (shape, case)
+
+
 def test_update_latest_messages_literal_vs_numpy(env):
     spec, state, ref = env
     store, parent, slot, roots, leaf_viable, rb = _small_store(spec, state, n_blocks=50)
