@@ -11,7 +11,8 @@
  *     registry / block-tree / latest-message tables it allocated on the device.
  *   - return value: 0 = ok, negative = B2_E* (environment / argument errors).  Cryptographic
  *     invalidity is DATA (ok_out[i] = 0, seg_status[i] != 0), never an error code.  On error no
- *     output buffer and no device table is modified (pos-evolution.md:1041).
+ *     output buffer and no device table is modified (pos-evolution.md:1041).  This includes the
+ *     table loads: a failed b2_registry_load / b2_tree_load leaves the previous tables in place.
  *   - functions without the _dev suffix take HOST pointers, are synchronous and do their own
  *     host<->device copies.  *_dev functions take DEVICE pointers plus a cudaStream_t (as void*)
  *     and only enqueue work (used by bench.py and by the multi-GPU path, where the u64 vote

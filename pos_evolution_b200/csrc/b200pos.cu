@@ -17,9 +17,37 @@
 
 using namespace b2;
 
+// A device allocation with one owner: freed on destruction, moved (never copied) between owners, and passed to kernels and copies
+// as whatever pointer type they take.  cudaFree waits for the device, so replacing a buffer that queued work still reads is safe.
 struct dbuf {
     void* p = nullptr;
     size_t cap = 0;
+    dbuf() = default;
+    dbuf(dbuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr, o.cap = 0; }
+    dbuf& operator=(dbuf o) noexcept {      // the previous allocation leaves with `o`
+        std::swap(p, o.p);
+        std::swap(cap, o.cap);
+        return *this;
+    }
+    ~dbuf() {
+        if (p) cudaFree(p);
+    }
+    explicit operator bool() const { return p != nullptr; }
+    template <class T> operator T*() const { return static_cast<T*>(p); }
+};
+
+// validator registry, latest messages and participation flags: n_val entries each, replaced together by b2_registry_load
+struct registry_tables {
+    dbuf records, valid, eff, flags;          // u32[24] affine pubkey record, u8 KeyValidate, u64 effective balance, u8 flags
+    dbuf lmd_key, lmd_block, equiv;           // u64 epoch << 32 | 0xffffffff (0 = no message), u32 block, u8 equivocating
+    dbuf part[2], part_first;                 // epoch participation flags (0 = current, 1 = previous), per-(validator, flag) election table
+};
+// block tree (b2_tree_load): everything the tree kernel reads is stored in pre-order
+struct tree_tables {
+    dbuf pre, inv, size_keep, rank, next, gsize;      // u32
+    dbuf packed;                                      // u32 size | rank << 15 | keep << 31 (used for trees of < 32 768 blocks)
+    dbuf votes, prefix, weight, w2;                   // u64
+    dbuf head;                                        // u32
 };
 
 struct vslot {
@@ -53,16 +81,8 @@ struct b2_ctx {
     vslot slot[B2_EPOCH_SLOTS];
     char err[512] = {0};
     uint64_t launches = 0;
-    // registry
     uint64_t n_val = 0;
-    uint32_t* d_records = nullptr;
-    uint8_t* d_valid = nullptr;
-    uint64_t* d_eff = nullptr;
-    uint8_t* d_flags = nullptr;
-    // latest messages
-    unsigned long long* d_lmd_key = nullptr;
-    uint32_t* d_lmd_block = nullptr;
-    uint8_t* d_equiv = nullptr;
+    registry_tables reg;
     // fork-choice variants: votes older than fc_min_key (epoch << 32) expire; v1.3 get_weight skips slashed validators
     // threads per block of the thread-per-aggregate kernels when they run under the epoch pipeline (see launch_miller)
     unsigned tail_block = 128;
@@ -73,42 +93,35 @@ struct b2_ctx {
     // FastAggregateVerify mode: 0 = one pairing check per aggregate; 1 = random-linear-combination batches of B2_RLC_GROUP
     // aggregates with per-aggregate fallback (b2_set_verify_mode); d_rlc_seed = the verifier's secret 32-byte seed
     int verify_mode = 0;
-    uint8_t* d_rlc_seed = nullptr;
+    dbuf d_rlc_seed;
     int pairing_form = 0;      // 0: team kernels for the synchronous calls, thread-per-aggregate under the pipeline; 1: always team; 2: always thread
     // threads per block of k_g2_decompress: its blocks fill the register file, so a smaller block is what a pairing warp of the
     // previous epoch displaces when the two overlap
     unsigned dec_block = 128;
     // one-launch get_head (k_get_head_fused): ticket counter, and the result slot in mapped pinned host memory (head, sequence)
     bool head_fused = true;                           // B2_HEAD_FUSED=0: the two-launch + memcpy form of round 1
-    unsigned int* d_ticket = nullptr;
+    dbuf d_ticket;
     volatile uint32_t* h_head = nullptr;
     uint32_t* d_head_host = nullptr;
     uint32_t head_seq = 0;
     // multi-GPU get_head over NVLink peer memory (b2_fc_exchange_*): this rank's exchange block = accumulators 2 x n_blocks u64 followed by
     // flag rows 2 x B2_MAX_PEERS u32; peers' blocks opened through CUDA IPC
-    void* fc_block = nullptr;
-    size_t fc_block_bytes = 0;
+    dbuf fc_block;
     uint32_t fc_blocks_cap = 0;                       // n_blocks the block was sized for
     void* fc_peer[B2_MAX_PEERS] = {nullptr};
     int fc_rank = -1, fc_world = 0;
     uint32_t fc_seq = 0;
-    unsigned long long* d_dbg = nullptr;              // clock64() stamps of the last get_head's phases (b2_debug_head_clocks)
-    uint32_t* d_guard = nullptr;                      // device-side input guard word (kernels.cuh GuardBits), read by b2_guard_flags
+    dbuf d_dbg;                                       // clock64() stamps of the last get_head's phases (b2_debug_head_clocks)
+    dbuf d_guard;                                     // device-side input guard word (kernels.cuh GuardBits), read by b2_guard_flags
     unsigned long long fc_min_key = 0;
     int fc_exclude_slashed = 0;
-    // epoch participation flags (0 = current, 1 = previous) and the per-(validator, flag) election table
-    uint32_t* d_part[2] = {nullptr, nullptr};
-    uint32_t* d_part_first = nullptr;
     // block tree
     uint32_t n_blocks = 0;
-    uint32_t *d_pre = nullptr, *d_inv = nullptr, *d_size_keep = nullptr, *d_rank = nullptr, *d_next = nullptr, *d_gsize = nullptr;
-    bool packed_ok = false;
-    uint32_t* d_packed = nullptr;     // size | rank << 15 | keep << 31 in pre-order (trees of < 32 768 blocks), else nullptr
-    unsigned long long *d_votes = nullptr, *d_prefix = nullptr, *d_weight = nullptr, *d_w2 = nullptr;
-    uint32_t* d_head = nullptr;
+    bool packed_ok = false;                           // tree.packed is read only when set
+    tree_tables tree;
     // scratch
-    dbuf sc_pkjac, sc_pkst, sc_haff, sc_hflag, sc_g2aff, sc_g2st, sc_rec, sc_val;
-    dbuf in_a, in_b, in_c, in_d, in_e, in_f, in_g, out_a, out_b, sc_shuf, sc_pivot;
+    dbuf sc_pkjac, sc_pkst, sc_haff, sc_hflag, sc_g2aff, sc_g2st, sc_rec, sc_val, sc_shuf, sc_pivot;
+    std::vector<dbuf> stage;                          // the synchronous entry points' host inputs and outputs (struct staging)
 };
 
 struct nvtx_scope {
@@ -118,6 +131,7 @@ struct nvtx_scope {
 #define B2_NVTX nvtx_scope nvtx_scope_(__func__)
 
 static int fail_cuda(b2_ctx* c, cudaError_t e, const char* what) {
+    cudaGetLastError();      // consume a pending non-sticky error (a failed cudaMalloc sets one), so the next CKL sees only its own launch
     if (c) snprintf(c->err, sizeof(c->err), "%s: %s", what, cudaGetErrorString(e));
     return B2_ECUDA;
 }
@@ -150,13 +164,69 @@ static int ensure(b2_ctx* ctx, dbuf& b, size_t bytes) {
     b.cap = want;
     return B2_OK;
 }
-template <class T> static int dev_alloc(b2_ctx* ctx, T** p, size_t count) {
-    if (*p) {
-        CK(cudaFree(*p));
-        *p = nullptr;
+
+// One synchronous call's host traffic on s_main.  in() uploads a host array into the call's next staging buffer (grow-only, as ensure);
+// out() registers a host output with the device buffer that holds it (by default a staging buffer of its own); finish() copies every
+// output to host memory, synchronises, and only if all of that succeeded writes the caller's buffers.  The first error is kept in rc
+// and makes every later step a no-op, so a caller checks rc once before its launches and returns finish().
+struct staging {
+    struct output {
+        void* host;
+        const void* dev;
+        size_t bytes;
+    };
+    b2_ctx* ctx;
+    int rc = B2_OK;
+    size_t used = 0;
+    std::vector<output> outs;
+    explicit staging(b2_ctx* c) : ctx(c) {}
+    void* buf(size_t bytes) {
+        if (rc) return nullptr;
+        if (used == ctx->stage.size()) ctx->stage.emplace_back();
+        dbuf& b = ctx->stage[used++];
+        rc = ensure(ctx, b, bytes);
+        return rc ? nullptr : b.p;
     }
-    CK(cudaMalloc((void**)p, std::max<size_t>(count * sizeof(T), 256)));
-    return B2_OK;
+    // `pad` bytes past the end are allocated but not copied
+    template <class T> const T* in(const T* host, size_t count, size_t pad = 0) {
+        void* d = buf(count * sizeof(T) + pad);
+        cudaError_t e = d && count ? cudaMemcpyAsync(d, host, count * sizeof(T), cudaMemcpyHostToDevice, ctx->s_main) : cudaSuccess;
+        if (e != cudaSuccess) rc = fail_cuda(ctx, e, "staging upload");
+        return static_cast<const T*>(d);
+    }
+    template <class T> T* out(T* host, size_t count) {
+        T* d = static_cast<T*>(buf(count * sizeof(T)));
+        out(host, d, count);
+        return d;
+    }
+    template <class T> void out(T* host, const void* dev, size_t count) {
+        if (!rc) outs.push_back({host, dev, count * sizeof(T)});
+    }
+    int finish() {
+        if (rc) return rc;
+        size_t total = 0;
+        for (const output& o : outs) total += o.bytes;
+        std::vector<uint8_t> tmp(total);
+        uint8_t* h = tmp.data();
+        for (const output& o : outs) {
+            CK(cudaMemcpyAsync(h, o.dev, o.bytes, cudaMemcpyDeviceToHost, ctx->s_main));
+            h += o.bytes;
+        }
+        CK(cudaStreamSynchronize(ctx->s_main));
+        h = tmp.data();
+        for (const output& o : outs) {
+            memcpy(o.host, h, o.bytes);
+            h += o.bytes;
+        }
+        return B2_OK;
+    }
+};
+
+// host check of the offsets off[0..n]: they start at 0 and never decrease
+static int check_offsets(b2_ctx* ctx, const uint32_t* off, uint32_t n, const char* what) {
+    if (off[0] == 0 && std::is_sorted(off, off + n + 1)) return B2_OK;
+    snprintf(ctx->err, sizeof(ctx->err), "%s must start at 0 and never decrease", what);
+    return B2_EINVAL;
 }
 #define B2_TEAM_SMEM (B2_TEAMS_PER_WARP * sizeof(team_ws))
 static inline unsigned blocks_for(uint64_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
@@ -183,13 +253,10 @@ int b2_init(int device, b2_ctx** out) {
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return B2_ENODEVICE;
     if (prop.major != 9 || prop.minor != 0) return B2_ENODEVICE;      // sm_90a cubin only: loads on compute capability 9.0
+    if (cudaSetDevice(device) != cudaSuccess) return B2_ENODEVICE;
     b2_ctx* ctx = new (std::nothrow) b2_ctx();
     if (!ctx) return B2_ENOMEM;
     ctx->device = device;
-    if (cudaSetDevice(device) != cudaSuccess) {
-        delete ctx;
-        return B2_ENODEVICE;
-    }
     // side streams get the highest priority: their kernels are small and latency-bound and must be scheduled as soon
     // as SM resources free up while a grid-filling kernel (signature decompression) occupies the main stream
     int prio_lo = 0, prio_hi = 0;
@@ -212,9 +279,9 @@ int b2_init(int device, b2_ctx** out) {
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_g1_gather_tma<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * (int)sizeof(gather_ws));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_g1_gather_tma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * (int)sizeof(gather_ws));
     ctx->n_sm = prop.multiProcessorCount;
-    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_dbg, 32 * 8);
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_dbg.p, 32 * 8);
     if (e == cudaSuccess) e = cudaMemset(ctx->d_dbg, 0, 32 * 8);
-    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_ticket, 64);
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_ticket.p, 64);
     if (e == cudaSuccess) e = cudaMemset(ctx->d_ticket, 0, 64);
     if (e == cudaSuccess) e = cudaHostAlloc((void**)&ctx->h_head, 64, cudaHostAllocMapped);
     if (e == cudaSuccess) {
@@ -223,9 +290,9 @@ int b2_init(int device, b2_ctx** out) {
     }
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_get_head_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_get_head_fused_nvl, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
-    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_rlc_seed, 32);
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_rlc_seed.p, 32);
     if (e == cudaSuccess) e = cudaMemset(ctx->d_rlc_seed, 0, 32);
-    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_guard, 256);
+    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_guard.p, 256);
     if (e == cudaSuccess) e = cudaMemset(ctx->d_guard, 0, 256);
     // diagnostic knobs (INTEGRATION.md); unset or out-of-range values keep the defaults, which are the measured best
     int v = 0;
@@ -238,32 +305,22 @@ int b2_init(int device, b2_ctx** out) {
     if (env_int("B2_HEAD_FUSED", &v)) ctx->head_fused = v != 0;
     if (const char* form = getenv("B2_PAIRING_FORM")) ctx->pairing_form = !strcmp(form, "team") ? 1 : (!strcmp(form, "thread") ? 2 : 0);
     if (e != cudaSuccess) {
-        delete ctx;
+        b2_destroy(ctx);
         return B2_ECUDA;
     }
     *out = ctx;
     return B2_OK;
 }
 
+// also the failure path of b2_init: every handle may still be null
 void b2_destroy(b2_ctx* ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
-    void* ptrs[] = {ctx->d_packed, ctx->d_part[0], ctx->d_part[1], ctx->d_part_first, ctx->d_records, ctx->d_valid, ctx->d_eff, ctx->d_flags, ctx->d_lmd_key, ctx->d_lmd_block, ctx->d_equiv, ctx->d_pre,
-                    ctx->d_inv, ctx->d_size_keep, ctx->d_gsize, ctx->d_w2, ctx->d_rank, ctx->d_next, ctx->d_votes, ctx->d_prefix,
-                    ctx->d_weight, ctx->d_head};
-    for (void* p : ptrs)
-        if (p) cudaFree(p);
-    dbuf* bufs[] = {&ctx->sc_pkjac, &ctx->sc_pkst, &ctx->sc_haff, &ctx->sc_hflag,
-                    &ctx->sc_g2aff, &ctx->sc_g2st, &ctx->sc_rec, &ctx->sc_val, &ctx->in_a, &ctx->in_b, &ctx->in_c, &ctx->in_d,
-                    &ctx->in_e, &ctx->in_f, &ctx->in_g, &ctx->out_a, &ctx->out_b, &ctx->sc_shuf, &ctx->sc_pivot};
-    for (dbuf* b : bufs)
-        if (b->p) cudaFree(b->p);
+    for (int r = 0; r < B2_MAX_PEERS; r++)      // before this rank's own exchange block is freed
+        if (ctx->fc_peer[r] && r != ctx->fc_rank) cudaIpcCloseMemHandle(ctx->fc_peer[r]);
     for (int i = 0; i < B2_EPOCH_SLOTS; i++) {
         vslot& V = ctx->slot[i];
-        dbuf* vb[] = {&V.haff, &V.hflag, &V.pkjac, &V.pkst, &V.saff, &V.sflag, &V.f, &V.sumjac, &V.pkjac_r, &V.rscal, &V.sg_aff, &V.sg_flag, &V.f_g, &V.gpass, &V.g2aff, &V.g2st};
-        for (dbuf* b : vb)
-            if (b->p) cudaFree(b->p);
         cudaEvent_t evs[6] = {V.ev_join0, V.ev_join1, V.ev_seg, V.ev_tail_done, V.ev_fork, V.ev_in};
         for (cudaEvent_t ev : evs)
             if (ev) cudaEventDestroy(ev);
@@ -275,16 +332,9 @@ void b2_destroy(b2_ctx* ctx) {
     for (int i = 0; i < 4; i++)
         if (ctx->s_dec[i]) cudaStreamDestroy(ctx->s_dec[i]);
     if (ctx->ev_lmd_done) cudaEventDestroy(ctx->ev_lmd_done);
-    if (ctx->d_guard) cudaFree(ctx->d_guard);
-    if (ctx->d_rlc_seed) cudaFree(ctx->d_rlc_seed);
-    if (ctx->d_ticket) cudaFree(ctx->d_ticket);
-    if (ctx->d_dbg) cudaFree(ctx->d_dbg);
-    for (int r = 0; r < B2_MAX_PEERS; r++)
-        if (ctx->fc_peer[r] && r != ctx->fc_rank) cudaIpcCloseMemHandle(ctx->fc_peer[r]);
-    if (ctx->fc_block) cudaFree(ctx->fc_block);
-    if (ctx->h_head) cudaFreeHost((void*)ctx->h_head);
     if (ctx->ev_votes_done) cudaEventDestroy(ctx->ev_votes_done);
-    delete ctx;
+    if (ctx->h_head) cudaFreeHost((void*)ctx->h_head);
+    delete ctx;      // frees every device buffer
 }
 
 const char* b2_last_error(b2_ctx* ctx) { return ctx ? ctx->err : "null context"; }
@@ -315,32 +365,27 @@ int b2_registry_load(b2_ctx* ctx, const uint8_t* pk48, const uint64_t* eff, cons
     B2_NVTX;
     REQUIRE(ctx && pk48 && eff && flags && n > 0 && n < (1ull << 32), "registry_load: bad arguments");
     CK(cudaSetDevice(ctx->device));
+    // The new tables are built aside and replace the old ones only once complete, so a failed load leaves the registry as it was.
+    // Every allocation, the largest first, comes before the first read of the caller's arrays.
+    registry_tables t;
     int rc;
-    if ((rc = dev_alloc(ctx, &ctx->d_records, n * 24)) || (rc = dev_alloc(ctx, &ctx->d_valid, n)) || (rc = dev_alloc(ctx, &ctx->d_eff, n)) ||
-        (rc = dev_alloc(ctx, &ctx->d_flags, n)) || (rc = dev_alloc(ctx, &ctx->d_lmd_key, n)) || (rc = dev_alloc(ctx, &ctx->d_lmd_block, n)) ||
-        (rc = dev_alloc(ctx, &ctx->d_equiv, n)))
+    if ((rc = ensure(ctx, t.records, n * 96)) || (rc = ensure(ctx, t.valid, n)) || (rc = ensure(ctx, t.eff, n * 8)) || (rc = ensure(ctx, t.flags, n)) ||
+        (rc = ensure(ctx, t.lmd_key, n * 8)) || (rc = ensure(ctx, t.lmd_block, n * 4)) || (rc = ensure(ctx, t.equiv, n)))
         return rc;
-    if ((rc = ensure(ctx, ctx->in_a, n * 48))) return rc;
+    staging st(ctx);
+    const uint8_t* d_pk = st.in(pk48, n * 48);
+    if (st.rc) return st.rc;
     cudaStream_t s = ctx->s_main;
-    CK(cudaMemcpyAsync(ctx->in_a.p, pk48, n * 48, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->d_eff, eff, n * 8, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->d_flags, flags, n, cudaMemcpyHostToDevice, s));
-    CK(cudaMemsetAsync(ctx->d_lmd_key, 0, n * 8, s));
-    CK(cudaMemsetAsync(ctx->d_lmd_block, 0, n * 4, s));
-    CK(cudaMemsetAsync(ctx->d_equiv, 0, n, s));
-    k_registry_load<<<blocks_for(n, 128), 128, 0, s>>>((const uint8_t*)ctx->in_a.p, n, ctx->d_records, ctx->d_valid);
+    CK(cudaMemcpyAsync(t.eff, eff, n * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(t.flags, flags, n, cudaMemcpyHostToDevice, s));
+    CK(cudaMemsetAsync(t.lmd_key, 0, n * 8, s));
+    CK(cudaMemsetAsync(t.lmd_block, 0, n * 4, s));
+    CK(cudaMemsetAsync(t.equiv, 0, n, s));
+    k_registry_load<<<blocks_for(n, 128), 128, 0, s>>>(d_pk, n, t.records, t.valid);
     CKL(ctx);
-    if (pk_valid_out) CK(cudaMemcpyAsync(pk_valid_out, ctx->d_valid, n, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    for (int w = 0; w < 2; w++)
-        if (ctx->d_part[w]) {
-            cudaFree(ctx->d_part[w]);
-            ctx->d_part[w] = nullptr;
-        }
-    if (ctx->d_part_first) {
-        cudaFree(ctx->d_part_first);
-        ctx->d_part_first = nullptr;
-    }
+    if (pk_valid_out) st.out(pk_valid_out, t.valid, n);
+    if ((rc = st.finish())) return rc;
+    ctx->reg = std::move(t);        // the participation tables are dropped: t has none
     ctx->n_val = n;
     return B2_OK;
 }
@@ -350,52 +395,33 @@ int b2_key_validate(b2_ctx* ctx, const uint8_t* pk48, uint64_t n, uint8_t* valid
     B2_NVTX;
     REQUIRE(ctx && pk48 && valid_out && n > 0 && n < (1ull << 32), "key_validate: bad arguments");
     CK(cudaSetDevice(ctx->device));
-    cudaStream_t s = ctx->s_main;
+    staging st(ctx);
+    const uint8_t* d_pk = st.in(pk48, n * 48);
     int rc;
-    if ((rc = ensure(ctx, ctx->in_a, n * 48)) || (rc = ensure(ctx, ctx->sc_rec, n * 96 + 16)) || (rc = ensure(ctx, ctx->sc_val, n + 16))) return rc;
-    CK(cudaMemcpyAsync(ctx->in_a.p, pk48, n * 48, cudaMemcpyHostToDevice, s));
-    k_g1_decompress_validate<<<blocks_for(n, 128), 128, 0, s>>>((const uint8_t*)ctx->in_a.p, n, (uint32_t*)ctx->sc_rec.p, (uint8_t*)ctx->sc_val.p);
+    if ((rc = st.rc) || (rc = ensure(ctx, ctx->sc_rec, n * 96 + 16)) || (rc = ensure(ctx, ctx->sc_val, n + 16))) return rc;
+    k_g1_decompress_validate<<<blocks_for(n, 128), 128, 0, ctx->s_main>>>(d_pk, n, (uint32_t*)ctx->sc_rec.p, (uint8_t*)ctx->sc_val.p);
     CKL(ctx);
-    std::vector<uint8_t> tmp(n);
-    CK(cudaMemcpyAsync(tmp.data(), ctx->sc_val.p, n, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    memcpy(valid_out, tmp.data(), n);
-    return B2_OK;
+    st.out(valid_out, ctx->sc_val, n);
+    return st.finish();
 }
 
 int b2_registry_update_balances(b2_ctx* ctx, const uint64_t* eff, const uint8_t* flags, uint64_t n) {
     B2_NVTX;
     REQUIRE(ctx && eff && flags && n == ctx->n_val && n > 0, "registry_update_balances: registry not loaded or size mismatch");
     CK(cudaSetDevice(ctx->device));
-    CK(cudaMemcpyAsync(ctx->d_eff, eff, n * 8, cudaMemcpyHostToDevice, ctx->s_main));
-    CK(cudaMemcpyAsync(ctx->d_flags, flags, n, cudaMemcpyHostToDevice, ctx->s_main));
+    CK(cudaMemcpyAsync(ctx->reg.eff, eff, n * 8, cudaMemcpyHostToDevice, ctx->s_main));
+    CK(cudaMemcpyAsync(ctx->reg.flags, flags, n, cudaMemcpyHostToDevice, ctx->s_main));
     CK(cudaStreamSynchronize(ctx->s_main));
     return B2_OK;
 }
 
 // host-side validation of a committee batch (indices must address the registry)
 static int check_batch(b2_ctx* ctx, const uint32_t* members, const uint32_t* off, uint32_t bits_stride, uint32_t n_agg, uint64_t limit) {
-    REQUIRE(off[0] == 0, "off[0] must be 0");
-    for (uint32_t a = 0; a < n_agg; a++) {
-        REQUIRE(off[a + 1] >= off[a], "off must be non-decreasing");
-        REQUIRE((uint64_t)(off[a + 1] - off[a]) <= (uint64_t)bits_stride * 8, "committee larger than bits_stride*8");
-    }
+    int rc;
+    if ((rc = check_offsets(ctx, off, n_agg, "off"))) return rc;
+    for (uint32_t a = 0; a < n_agg; a++) REQUIRE((uint64_t)(off[a + 1] - off[a]) <= (uint64_t)bits_stride * 8, "committee larger than bits_stride*8");
     const uint32_t total = off[n_agg];
     for (uint32_t i = 0; i < total; i++) REQUIRE(members[i] < limit, "member index outside the registry");
-    return B2_OK;
-}
-
-// upload members/off/bits into in_a/in_b/in_c
-static int upload_batch(b2_ctx* ctx, const uint32_t* members, const uint32_t* off, const uint8_t* bits, uint32_t bits_stride, uint32_t n_agg,
-                        cudaStream_t s) {
-    int rc;
-    const uint32_t total = off[n_agg];
-    if ((rc = ensure(ctx, ctx->in_a, (size_t)total * 4 + 4)) || (rc = ensure(ctx, ctx->in_b, (size_t)(n_agg + 1) * 4)) ||
-        (rc = ensure(ctx, ctx->in_c, (size_t)n_agg * bits_stride + 16)))
-        return rc;
-    if (total) CK(cudaMemcpyAsync(ctx->in_a.p, members, (size_t)total * 4, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->in_b.p, off, (size_t)(n_agg + 1) * 4, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->in_c.p, bits, (size_t)n_agg * bits_stride, cudaMemcpyHostToDevice, s));
     return B2_OK;
 }
 
@@ -404,10 +430,10 @@ static int upload_batch(b2_ctx* ctx, const uint32_t* members, const uint32_t* of
 static int launch_k2(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_off, const uint8_t* d_bits, uint32_t bits_stride, uint32_t n_agg,
                      uint32_t* d_pkjac, uint8_t* d_pkst, unsigned wpb, unsigned ldg_block, cudaStream_t s) {
     if (ctx->k2_tma) {
-        k_g1_gather_tma<false><<<blocks_for(n_agg, wpb), wpb * 32, wpb * sizeof(gather_ws), s>>>(ctx->d_records, d_members, d_off, d_bits, bits_stride, n_agg,
+        k_g1_gather_tma<false><<<blocks_for(n_agg, wpb), wpb * 32, wpb * sizeof(gather_ws), s>>>(ctx->reg.records, d_members, d_off, d_bits, bits_stride, n_agg,
                                                                                              d_pkjac, d_pkst, ctx->n_val, ctx->d_guard, nullptr);
     } else {
-        k_g1_aggregate<<<n_agg, ldg_block, 0, s>>>(ctx->d_records, ctx->d_valid, d_members, d_off, d_bits, bits_stride, n_agg, d_pkjac, d_pkst, ctx->n_val,
+        k_g1_aggregate<<<n_agg, ldg_block, 0, s>>>(ctx->reg.records, ctx->reg.valid, d_members, d_off, d_bits, bits_stride, n_agg, d_pkjac, d_pkst, ctx->n_val,
                                                    ctx->d_guard);
     }
     CKL(ctx);
@@ -430,19 +456,16 @@ int b2_g1_aggregate(b2_ctx* ctx, const uint32_t* members, const uint32_t* off, c
     if ((rc = check_batch(ctx, members, off, bits_stride, n_agg, ctx->n_val))) return rc;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->s_main;
-    if ((rc = upload_batch(ctx, members, off, bits, bits_stride, n_agg, s))) return rc;
-    if ((rc = g1_aggregate_dev(ctx, (const uint32_t*)ctx->in_a.p, (const uint32_t*)ctx->in_b.p, (const uint8_t*)ctx->in_c.p, bits_stride, n_agg, s)))
-        return rc;
-    if ((rc = ensure(ctx, ctx->out_a, (size_t)n_agg * 48))) return rc;
-    k_g1_compress<<<blocks_for(n_agg, 64), 64, 0, s>>>((const uint32_t*)ctx->sc_pkjac.p, n_agg, (uint8_t*)ctx->out_a.p);
+    staging st(ctx);
+    const uint32_t* dm = st.in(members, off[n_agg], 4);
+    const uint32_t* dof = st.in(off, (size_t)n_agg + 1);
+    const uint8_t* db = st.in(bits, (size_t)n_agg * bits_stride, 16);
+    uint8_t* d48 = st.out(out48, (size_t)n_agg * 48);
+    if ((rc = st.rc) || (rc = g1_aggregate_dev(ctx, dm, dof, db, bits_stride, n_agg, s))) return rc;
+    k_g1_compress<<<blocks_for(n_agg, 64), 64, 0, s>>>((const uint32_t*)ctx->sc_pkjac.p, n_agg, d48);
     CKL(ctx);
-    std::vector<uint8_t> t48((size_t)n_agg * 48), tst(n_agg);
-    CK(cudaMemcpyAsync(t48.data(), ctx->out_a.p, t48.size(), cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(tst.data(), ctx->sc_pkst.p, n_agg, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    memcpy(out48, t48.data(), t48.size());
-    memcpy(status, tst.data(), n_agg);
-    return B2_OK;
+    st.out(status, ctx->sc_pkst, n_agg);
+    return st.finish();
 }
 
 // The gather stage of K2 ALONE (no additions): XOR checksum of the records each aggregate selects.  form 1: TMA-staged
@@ -455,10 +478,10 @@ int b2_gather_probe_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* 
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
     if (form == 1) {
-        k_g1_gather_tma<true><<<blocks_for(n_agg, 4), 128, 4 * sizeof(gather_ws), s>>>(ctx->d_records, d_members, d_off, d_bits, bits_stride, n_agg, nullptr,
+        k_g1_gather_tma<true><<<blocks_for(n_agg, 4), 128, 4 * sizeof(gather_ws), s>>>(ctx->reg.records, d_members, d_off, d_bits, bits_stride, n_agg, nullptr,
                                                                                     nullptr, ctx->n_val, ctx->d_guard, d_checksum_out);
     } else {
-        k_g1_gather_ldg_probe<<<n_agg, 128, 0, s>>>(ctx->d_records, d_members, d_off, d_bits, bits_stride, n_agg, ctx->n_val, d_checksum_out);
+        k_g1_gather_ldg_probe<<<n_agg, 128, 0, s>>>(ctx->reg.records, d_members, d_off, d_bits, bits_stride, n_agg, ctx->n_val, d_checksum_out);
     }
     CKL(ctx);
     return B2_OK;
@@ -514,29 +537,18 @@ int b2_aggregate_dev(b2_ctx* ctx, const uint8_t* d_sig96, const uint32_t* d_seg_
 int b2_aggregate(b2_ctx* ctx, const uint8_t* sig96, const uint32_t* seg_off, uint32_t n_seg, uint8_t* out96, int32_t* seg_status) {
     B2_NVTX;
     REQUIRE(ctx && seg_off && out96 && seg_status && n_seg > 0, "aggregate: bad arguments");
-    REQUIRE(seg_off[0] == 0, "aggregate: seg_off[0] must be 0");
-    for (uint32_t s = 0; s < n_seg; s++) REQUIRE(seg_off[s + 1] >= seg_off[s], "aggregate: seg_off must be non-decreasing");
+    int rc;
+    if ((rc = check_offsets(ctx, seg_off, n_seg, "aggregate: seg_off"))) return rc;
     const uint64_t n_sig = seg_off[n_seg];
     REQUIRE(n_sig == 0 || sig96, "aggregate: null signatures");
     CK(cudaSetDevice(ctx->device));
-    cudaStream_t s = ctx->s_main;
-    int rc;
-    if ((rc = ensure(ctx, ctx->in_d, n_sig * 96 + 16)) || (rc = ensure(ctx, ctx->in_b, (size_t)(n_seg + 1) * 4)) ||
-        (rc = ensure(ctx, ctx->out_a, (size_t)n_seg * 96)) || (rc = ensure(ctx, ctx->out_b, (size_t)n_seg * 4)))
-        return rc;
-    if (n_sig) CK(cudaMemcpyAsync(ctx->in_d.p, sig96, n_sig * 96, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->in_b.p, seg_off, (size_t)(n_seg + 1) * 4, cudaMemcpyHostToDevice, s));
-    if ((rc = b2_aggregate_dev(ctx, (const uint8_t*)ctx->in_d.p, (const uint32_t*)ctx->in_b.p, n_seg, n_sig, (uint8_t*)ctx->out_a.p,
-                               (int32_t*)ctx->out_b.p, s)))
-        return rc;
-    std::vector<uint8_t> t96((size_t)n_seg * 96);
-    std::vector<int32_t> tst(n_seg);
-    CK(cudaMemcpyAsync(t96.data(), ctx->out_a.p, t96.size(), cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(tst.data(), ctx->out_b.p, (size_t)n_seg * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    memcpy(out96, t96.data(), t96.size());
-    memcpy(seg_status, tst.data(), (size_t)n_seg * 4);
-    return B2_OK;
+    staging st(ctx);
+    const uint8_t* dsig = st.in(sig96, n_sig * 96, 16);
+    const uint32_t* doff = st.in(seg_off, (size_t)n_seg + 1);
+    uint8_t* d96 = st.out(out96, (size_t)n_seg * 96);
+    int32_t* dst = st.out(seg_status, n_seg);
+    if ((rc = st.rc) || (rc = b2_aggregate_dev(ctx, dsig, doff, n_seg, n_sig, d96, dst, ctx->s_main))) return rc;
+    return st.finish();
 }
 
 // ------------------------------------------------------------------------------------------ FastAggregateVerify
@@ -792,50 +804,39 @@ int b2_fast_aggregate_verify(b2_ctx* ctx, const uint32_t* members, const uint32_
     int rc;
     if ((rc = check_batch(ctx, members, off, bits_stride, n_agg, ctx->n_val))) return rc;
     CK(cudaSetDevice(ctx->device));
-    cudaStream_t s = ctx->s_main;
-    if ((rc = upload_batch(ctx, members, off, bits, bits_stride, n_agg, s))) return rc;
-    if ((rc = ensure(ctx, ctx->in_d, (size_t)n_agg * 96)) || (rc = ensure(ctx, ctx->in_e, (size_t)n_agg * 32)) || (rc = ensure(ctx, ctx->out_a, n_agg)))
-        return rc;
-    CK(cudaMemcpyAsync(ctx->in_d.p, sig96, (size_t)n_agg * 96, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->in_e.p, msg32, (size_t)n_agg * 32, cudaMemcpyHostToDevice, s));
-    if ((rc = b2_fast_aggregate_verify_dev(ctx, (const uint32_t*)ctx->in_a.p, (const uint32_t*)ctx->in_b.p, (const uint8_t*)ctx->in_c.p, bits_stride,
-                                           (const uint8_t*)ctx->in_e.p, (const uint8_t*)ctx->in_d.p, n_agg, (uint8_t*)ctx->out_a.p, s)))
-        return rc;
-    std::vector<uint8_t> tok(n_agg);
-    CK(cudaMemcpyAsync(tok.data(), ctx->out_a.p, n_agg, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    memcpy(ok_out, tok.data(), n_agg);
-    return B2_OK;
+    staging st(ctx);
+    const uint32_t* dm = st.in(members, off[n_agg], 4);
+    const uint32_t* dof = st.in(off, (size_t)n_agg + 1);
+    const uint8_t* db = st.in(bits, (size_t)n_agg * bits_stride, 16);
+    const uint8_t* dsig = st.in(sig96, (size_t)n_agg * 96);
+    const uint8_t* dmsg = st.in(msg32, (size_t)n_agg * 32);
+    uint8_t* dok = st.out(ok_out, n_agg);
+    if ((rc = st.rc) || (rc = b2_fast_aggregate_verify_dev(ctx, dm, dof, db, bits_stride, dmsg, dsig, n_agg, dok, ctx->s_main))) return rc;
+    return st.finish();
 }
 
 int b2_fast_aggregate_verify_pks(b2_ctx* ctx, const uint8_t* pk48, const uint32_t* pk_off, const uint8_t* msg32, const uint8_t* sig96,
                                  uint32_t n_agg, uint8_t* ok_out) {
     B2_NVTX;
     REQUIRE(ctx && pk_off && msg32 && sig96 && ok_out && n_agg > 0, "fast_aggregate_verify_pks: bad arguments");
-    REQUIRE(pk_off[0] == 0, "pk_off[0] must be 0");
-    for (uint32_t a = 0; a < n_agg; a++) REQUIRE(pk_off[a + 1] >= pk_off[a], "pk_off must be non-decreasing");
+    int rc;
+    if ((rc = check_offsets(ctx, pk_off, n_agg, "pk_off"))) return rc;
     const uint64_t n_pk = pk_off[n_agg];
     REQUIRE(n_pk == 0 || pk48, "null pubkeys");
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->s_main;
-    int rc;
-    if ((rc = ensure(ctx, ctx->in_a, n_pk * 48 + 16)) || (rc = ensure(ctx, ctx->in_b, (size_t)(n_agg + 1) * 4)) ||
-        (rc = ensure(ctx, ctx->in_d, (size_t)n_agg * 96)) || (rc = ensure(ctx, ctx->in_e, (size_t)n_agg * 32)) || (rc = ensure(ctx, ctx->out_a, n_agg)) ||
-        (rc = ensure(ctx, ctx->sc_rec, n_pk * 96 + 16)) || (rc = ensure(ctx, ctx->sc_val, n_pk + 16)) ||
+    if ((rc = ensure(ctx, ctx->sc_rec, n_pk * 96 + 16)) || (rc = ensure(ctx, ctx->sc_val, n_pk + 16)) ||
         (rc = ensure(ctx, ctx->sc_pkjac, (size_t)n_agg * 144)) || (rc = ensure(ctx, ctx->sc_pkst, n_agg)))
         return rc;
-    if (n_pk) CK(cudaMemcpyAsync(ctx->in_a.p, pk48, n_pk * 48, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->in_b.p, pk_off, (size_t)(n_agg + 1) * 4, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->in_d.p, sig96, (size_t)n_agg * 96, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->in_e.p, msg32, (size_t)n_agg * 32, cudaMemcpyHostToDevice, s));
-    pk_source P = {nullptr, (const uint32_t*)ctx->in_b.p, nullptr, 0, (const uint8_t*)ctx->in_a.p, n_pk};
-    if ((rc = verify_fork(ctx, ctx->slot[0], P, (const uint8_t*)ctx->in_e.p, n_agg, s))) return rc;
-    if ((rc = verify_main(ctx, ctx->slot[0], (const uint8_t*)ctx->in_d.p, n_agg, (uint8_t*)ctx->out_a.p, s))) return rc;
-    std::vector<uint8_t> tok(n_agg);
-    CK(cudaMemcpyAsync(tok.data(), ctx->out_a.p, n_agg, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    memcpy(ok_out, tok.data(), n_agg);
-    return B2_OK;
+    staging st(ctx);
+    const uint8_t* dpk = st.in(pk48, n_pk * 48, 16);
+    const uint32_t* dof = st.in(pk_off, (size_t)n_agg + 1);
+    const uint8_t* dsig = st.in(sig96, (size_t)n_agg * 96);
+    const uint8_t* dmsg = st.in(msg32, (size_t)n_agg * 32);
+    uint8_t* dok = st.out(ok_out, n_agg);
+    pk_source P = {nullptr, dof, nullptr, 0, dpk, n_pk};
+    if ((rc = st.rc) || (rc = verify_fork(ctx, ctx->slot[0], P, dmsg, n_agg, s)) || (rc = verify_main(ctx, ctx->slot[0], dsig, n_agg, dok, s))) return rc;
+    return st.finish();
 }
 
 // ------------------------------------------------------------------------------------------ SkToPk / Sign / hash_to_g2
@@ -843,15 +844,13 @@ int b2_sk_to_pk(b2_ctx* ctx, const uint32_t* sk8, uint64_t n, uint8_t* pk48_out)
     B2_NVTX;
     REQUIRE(ctx && sk8 && pk48_out && n > 0, "sk_to_pk: bad arguments");
     CK(cudaSetDevice(ctx->device));
-    cudaStream_t s = ctx->s_main;
-    int rc;
-    if ((rc = ensure(ctx, ctx->in_f, n * 32)) || (rc = ensure(ctx, ctx->out_a, n * 48))) return rc;
-    CK(cudaMemcpyAsync(ctx->in_f.p, sk8, n * 32, cudaMemcpyHostToDevice, s));
-    k_sk_to_pk<<<blocks_for(n, 64), 64, 0, s>>>((const uint32_t*)ctx->in_f.p, n, (uint8_t*)ctx->out_a.p);
+    staging st(ctx);
+    const uint32_t* dsk = st.in(sk8, n * 8);
+    uint8_t* dpk = st.out(pk48_out, n * 48);
+    if (st.rc) return st.rc;
+    k_sk_to_pk<<<blocks_for(n, 64), 64, 0, ctx->s_main>>>(dsk, n, dpk);
     CKL(ctx);
-    CK(cudaMemcpyAsync(pk48_out, ctx->out_a.p, n * 48, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return B2_OK;
+    return st.finish();
 }
 
 int b2_hash_to_g2(b2_ctx* ctx, const uint8_t* msg32, uint32_t n_msg, uint8_t* out96) {
@@ -859,18 +858,16 @@ int b2_hash_to_g2(b2_ctx* ctx, const uint8_t* msg32, uint32_t n_msg, uint8_t* ou
     REQUIRE(ctx && msg32 && out96 && n_msg > 0, "hash_to_g2: bad arguments");
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->s_main;
+    staging st(ctx);
+    const uint8_t* dmsg = st.in(msg32, (size_t)n_msg * 32);
+    uint8_t* d96 = st.out(out96, (size_t)n_msg * 96);
     int rc;
-    if ((rc = ensure(ctx, ctx->in_e, (size_t)n_msg * 32)) || (rc = ensure(ctx, ctx->sc_haff, (size_t)n_msg * 192)) ||
-        (rc = ensure(ctx, ctx->sc_hflag, n_msg)) || (rc = ensure(ctx, ctx->out_a, (size_t)n_msg * 96)))
-        return rc;
-    CK(cudaMemcpyAsync(ctx->in_e.p, msg32, (size_t)n_msg * 32, cudaMemcpyHostToDevice, s));
-    k_hash_to_g2<<<blocks_for(2ull * n_msg, 32), 32, 0, s>>>((const uint8_t*)ctx->in_e.p, n_msg, (uint32_t*)ctx->sc_haff.p, (uint8_t*)ctx->sc_hflag.p);
+    if ((rc = st.rc) || (rc = ensure(ctx, ctx->sc_haff, (size_t)n_msg * 192)) || (rc = ensure(ctx, ctx->sc_hflag, n_msg))) return rc;
+    k_hash_to_g2<<<blocks_for(2ull * n_msg, 32), 32, 0, s>>>(dmsg, n_msg, (uint32_t*)ctx->sc_haff.p, (uint8_t*)ctx->sc_hflag.p);
     CKL(ctx);
-    k_g2_compress_aff<<<blocks_for(n_msg, 64), 64, 0, s>>>((const uint32_t*)ctx->sc_haff.p, (const uint8_t*)ctx->sc_hflag.p, n_msg, (uint8_t*)ctx->out_a.p);
+    k_g2_compress_aff<<<blocks_for(n_msg, 64), 64, 0, s>>>((const uint32_t*)ctx->sc_haff.p, (const uint8_t*)ctx->sc_hflag.p, n_msg, d96);
     CKL(ctx);
-    CK(cudaMemcpyAsync(out96, ctx->out_a.p, (size_t)n_msg * 96, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return B2_OK;
+    return st.finish();
 }
 
 int b2_sign(b2_ctx* ctx, const uint32_t* sk8, const uint32_t* msg_idx, uint64_t n, const uint8_t* msg32, uint32_t n_msg, uint8_t* sig96_out) {
@@ -879,20 +876,18 @@ int b2_sign(b2_ctx* ctx, const uint32_t* sk8, const uint32_t* msg_idx, uint64_t 
     for (uint64_t i = 0; i < n; i++) REQUIRE(msg_idx[i] < n_msg, "sign: msg_idx out of range");
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->s_main;
+    staging st(ctx);
+    const uint32_t* dsk = st.in(sk8, n * 8);
+    const uint32_t* didx = st.in(msg_idx, n);
+    const uint8_t* dmsg = st.in(msg32, (size_t)n_msg * 32);
+    uint8_t* dsig = st.out(sig96_out, n * 96);
     int rc;
-    if ((rc = ensure(ctx, ctx->in_f, n * 32)) || (rc = ensure(ctx, ctx->in_g, n * 4)) || (rc = ensure(ctx, ctx->in_e, (size_t)n_msg * 32)) ||
-        (rc = ensure(ctx, ctx->sc_haff, (size_t)n_msg * 192)) || (rc = ensure(ctx, ctx->sc_hflag, n_msg)) || (rc = ensure(ctx, ctx->out_a, n * 96)))
-        return rc;
-    CK(cudaMemcpyAsync(ctx->in_f.p, sk8, n * 32, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->in_g.p, msg_idx, n * 4, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->in_e.p, msg32, (size_t)n_msg * 32, cudaMemcpyHostToDevice, s));
-    k_hash_to_g2<<<blocks_for(2ull * n_msg, 32), 32, 0, s>>>((const uint8_t*)ctx->in_e.p, n_msg, (uint32_t*)ctx->sc_haff.p, (uint8_t*)ctx->sc_hflag.p);
+    if ((rc = st.rc) || (rc = ensure(ctx, ctx->sc_haff, (size_t)n_msg * 192)) || (rc = ensure(ctx, ctx->sc_hflag, n_msg))) return rc;
+    k_hash_to_g2<<<blocks_for(2ull * n_msg, 32), 32, 0, s>>>(dmsg, n_msg, (uint32_t*)ctx->sc_haff.p, (uint8_t*)ctx->sc_hflag.p);
     CKL(ctx);
-    k_sign<<<blocks_for(n, 64), 64, 0, s>>>((const uint32_t*)ctx->in_f.p, (const uint32_t*)ctx->in_g.p, n, (const uint32_t*)ctx->sc_haff.p, (uint8_t*)ctx->out_a.p);
+    k_sign<<<blocks_for(n, 64), 64, 0, s>>>(dsk, didx, n, (const uint32_t*)ctx->sc_haff.p, dsig);
     CKL(ctx);
-    CK(cudaMemcpyAsync(sig96_out, ctx->out_a.p, n * 96, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return B2_OK;
+    return st.finish();
 }
 
 // ------------------------------------------------------------------------------------------ batched SHA-256
@@ -900,15 +895,13 @@ int b2_sha256_batch(b2_ctx* ctx, const uint8_t* msgs, uint32_t msg_len, uint64_t
     B2_NVTX;
     REQUIRE(ctx && out32 && n > 0 && (msg_len == 0 || msgs), "sha256_batch: bad arguments");
     CK(cudaSetDevice(ctx->device));
-    cudaStream_t s = ctx->s_main;
-    int rc;
-    if ((rc = ensure(ctx, ctx->in_a, (size_t)n * msg_len + 16)) || (rc = ensure(ctx, ctx->out_a, (size_t)n * 32))) return rc;
-    if (msg_len) CK(cudaMemcpyAsync(ctx->in_a.p, msgs, (size_t)n * msg_len, cudaMemcpyHostToDevice, s));
-    k_sha256_fixed<<<blocks_for(n, 128), 128, 0, s>>>((const uint8_t*)ctx->in_a.p, msg_len, n, (uint8_t*)ctx->out_a.p);
+    staging st(ctx);
+    const uint8_t* dmsg = st.in(msgs, (size_t)n * msg_len, 16);
+    uint8_t* d32 = st.out(out32, (size_t)n * 32);
+    if (st.rc) return st.rc;
+    k_sha256_fixed<<<blocks_for(n, 128), 128, 0, ctx->s_main>>>(dmsg, msg_len, n, d32);
     CKL(ctx);
-    CK(cudaMemcpyAsync(out32, ctx->out_a.p, (size_t)n * 32, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return B2_OK;
+    return st.finish();
 }
 
 // ------------------------------------------------------------------------------------------ SSZ signing roots
@@ -916,18 +909,14 @@ int b2_signing_roots(b2_ctx* ctx, const uint8_t* data128, const uint8_t* domain3
     B2_NVTX;
     REQUIRE(ctx && data128 && domain32 && out32 && n > 0, "signing_roots: bad arguments");
     CK(cudaSetDevice(ctx->device));
-    cudaStream_t s = ctx->s_main;
-    int rc;
-    const size_t dom_bytes = per_attestation_domain ? (size_t)n * 32 : 32;
-    if ((rc = ensure(ctx, ctx->in_a, (size_t)n * 128)) || (rc = ensure(ctx, ctx->in_e, dom_bytes)) || (rc = ensure(ctx, ctx->out_a, (size_t)n * 32))) return rc;
-    CK(cudaMemcpyAsync(ctx->in_a.p, data128, (size_t)n * 128, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->in_e.p, domain32, dom_bytes, cudaMemcpyHostToDevice, s));
-    k_signing_roots<<<blocks_for(n, 64), 64, 0, s>>>((const uint8_t*)ctx->in_a.p, (const uint8_t*)ctx->in_e.p, per_attestation_domain ? 32u : 0u, n,
-                                                    (uint8_t*)ctx->out_a.p);
+    staging st(ctx);
+    const uint8_t* ddata = st.in(data128, (size_t)n * 128);
+    const uint8_t* ddom = st.in(domain32, per_attestation_domain ? (size_t)n * 32 : 32);
+    uint8_t* d32 = st.out(out32, (size_t)n * 32);
+    if (st.rc) return st.rc;
+    k_signing_roots<<<blocks_for(n, 64), 64, 0, ctx->s_main>>>(ddata, ddom, per_attestation_domain ? 32u : 0u, n, d32);
     CKL(ctx);
-    CK(cudaMemcpyAsync(out32, ctx->out_a.p, (size_t)n * 32, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return B2_OK;
+    return st.finish();
 }
 
 // ------------------------------------------------------------------------------------------ SSZ wire decode (:714-717)
@@ -936,30 +925,21 @@ int b2_attestations_decode(b2_ctx* ctx, const uint8_t* wire, const uint32_t* wof
     B2_NVTX;
     REQUIRE(ctx && wire && woff && n > 0 && bits_stride > 0 && bits_out && bit_len_out && data128_out && sig96_out && status_out,
             "attestations_decode: bad arguments");
-    REQUIRE(woff[0] == 0, "attestations_decode: woff[0] must be 0");
-    for (uint32_t i = 0; i < n; i++) REQUIRE(woff[i + 1] >= woff[i], "attestations_decode: woff must be non-decreasing");
-    CK(cudaSetDevice(ctx->device));
-    cudaStream_t s = ctx->s_main;
-    const size_t total = woff[n];
-    const size_t o_bits = 0, o_len = o_bits + (((size_t)n * bits_stride + 15) & ~(size_t)15), o_data = o_len + (size_t)n * 4,
-                 o_sig = o_data + (size_t)n * 128, o_st = o_sig + (size_t)n * 96, o_end = o_st + (size_t)n * 4;
     int rc;
-    if ((rc = ensure(ctx, ctx->in_a, total + 16)) || (rc = ensure(ctx, ctx->in_b, (size_t)(n + 1) * 4)) || (rc = ensure(ctx, ctx->out_a, o_end))) return rc;
-    if (total) CK(cudaMemcpyAsync(ctx->in_a.p, wire, total, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->in_b.p, woff, (size_t)(n + 1) * 4, cudaMemcpyHostToDevice, s));
-    uint8_t* o = (uint8_t*)ctx->out_a.p;
-    k_attestations_decode<<<blocks_for((uint64_t)n * 32, 128), 128, 0, s>>>((const uint8_t*)ctx->in_a.p, (const uint32_t*)ctx->in_b.p, n, bits_stride, max_bits,
-                                                                          o + o_bits, (uint32_t*)(o + o_len), o + o_data, o + o_sig, (int32_t*)(o + o_st));
+    if ((rc = check_offsets(ctx, woff, n, "attestations_decode: woff"))) return rc;
+    CK(cudaSetDevice(ctx->device));
+    staging st(ctx);
+    const uint8_t* dwire = st.in(wire, woff[n], 16);
+    const uint32_t* dwoff = st.in(woff, (size_t)n + 1);
+    uint8_t* dbits = st.out(bits_out, (size_t)n * bits_stride);
+    uint32_t* dlen = st.out(bit_len_out, n);
+    uint8_t* ddata = st.out(data128_out, (size_t)n * 128);
+    uint8_t* dsig = st.out(sig96_out, (size_t)n * 96);
+    int32_t* dst = st.out(status_out, n);
+    if (st.rc) return st.rc;
+    k_attestations_decode<<<blocks_for((uint64_t)n * 32, 128), 128, 0, ctx->s_main>>>(dwire, dwoff, n, bits_stride, max_bits, dbits, dlen, ddata, dsig, dst);
     CKL(ctx);
-    std::vector<uint8_t> host(o_end);                       // outputs stay untouched on error
-    CK(cudaMemcpyAsync(host.data(), o, o_end, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    memcpy(bits_out, host.data() + o_bits, (size_t)n * bits_stride);
-    memcpy(bit_len_out, host.data() + o_len, (size_t)n * 4);
-    memcpy(data128_out, host.data() + o_data, (size_t)n * 128);
-    memcpy(sig96_out, host.data() + o_sig, (size_t)n * 96);
-    memcpy(status_out, host.data() + o_st, (size_t)n * 4);
-    return B2_OK;
+    return st.finish();
 }
 
 // ------------------------------------------------------------------------------------------ committee shuffle
@@ -989,18 +969,13 @@ int b2_shuffle_committees(b2_ctx* ctx, const uint8_t* seed32, const uint32_t* ac
     REQUIRE(ctx && seed32 && members_out && rounds <= 255, "shuffle_committees: bad arguments");
     if (n_active == 0) return B2_OK;
     CK(cudaSetDevice(ctx->device));
-    cudaStream_t s = ctx->s_main;
+    staging st(ctx);
+    const uint8_t* dseed = st.in(seed32, 32);
+    const uint32_t* dact = active ? st.in(active, n_active) : nullptr;
+    uint32_t* dm = st.out(members_out, n_active);
     int rc;
-    if ((rc = ensure(ctx, ctx->in_e, 32)) || (rc = ensure(ctx, ctx->in_a, (size_t)n_active * 4)) || (rc = ensure(ctx, ctx->out_a, (size_t)n_active * 4)))
-        return rc;
-    CK(cudaMemcpyAsync(ctx->in_e.p, seed32, 32, cudaMemcpyHostToDevice, s));
-    if (active) CK(cudaMemcpyAsync(ctx->in_a.p, active, (size_t)n_active * 4, cudaMemcpyHostToDevice, s));
-    if ((rc = b2_shuffle_committees_dev(ctx, (const uint8_t*)ctx->in_e.p, active ? (const uint32_t*)ctx->in_a.p : nullptr, n_active, rounds,
-                                        (uint32_t*)ctx->out_a.p, s)))
-        return rc;
-    CK(cudaMemcpyAsync(members_out, ctx->out_a.p, (size_t)n_active * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return B2_OK;
+    if ((rc = st.rc) || (rc = b2_shuffle_committees_dev(ctx, dseed, dact, n_active, rounds, dm, ctx->s_main))) return rc;
+    return st.finish();
 }
 
 // ------------------------------------------------------------------------------------------ latest messages
@@ -1008,9 +983,9 @@ int b2_latest_messages_reset(b2_ctx* ctx) {
     B2_NVTX;
     REQUIRE(ctx && ctx->n_val > 0, "latest_messages_reset: registry not loaded");
     CK(cudaSetDevice(ctx->device));
-    CK(cudaMemsetAsync(ctx->d_lmd_key, 0, ctx->n_val * 8, ctx->s_main));
-    CK(cudaMemsetAsync(ctx->d_lmd_block, 0, ctx->n_val * 4, ctx->s_main));
-    CK(cudaMemsetAsync(ctx->d_equiv, 0, ctx->n_val, ctx->s_main));
+    CK(cudaMemsetAsync(ctx->reg.lmd_key, 0, ctx->n_val * 8, ctx->s_main));
+    CK(cudaMemsetAsync(ctx->reg.lmd_block, 0, ctx->n_val * 4, ctx->s_main));
+    CK(cudaMemsetAsync(ctx->reg.equiv, 0, ctx->n_val, ctx->s_main));
     CK(cudaStreamSynchronize(ctx->s_main));
     return B2_OK;
 }
@@ -1026,9 +1001,9 @@ int b2_latest_messages_load(b2_ctx* ctx, const uint64_t* epoch, const uint32_t* 
     }
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->s_main;
-    CK(cudaMemcpyAsync(ctx->d_lmd_key, key.data(), n * 8, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->d_lmd_block, block_idx, n * 4, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->d_equiv, equivocating, n, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(ctx->reg.lmd_key, key.data(), n * 8, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(ctx->reg.lmd_block, block_idx, n * 4, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(ctx->reg.equiv, equivocating, n, cudaMemcpyHostToDevice, s));
     CK(cudaStreamSynchronize(s));
     return B2_OK;
 }
@@ -1038,10 +1013,11 @@ int b2_latest_messages_read(b2_ctx* ctx, uint64_t* epoch, uint32_t* block_idx, u
     REQUIRE(ctx && epoch && block_idx && has_msg && n == ctx->n_val && n > 0, "latest_messages_read: bad arguments / registry size");
     std::vector<unsigned long long> key(n);
     CK(cudaSetDevice(ctx->device));
-    cudaStream_t s = ctx->s_main;
-    CK(cudaMemcpyAsync(key.data(), ctx->d_lmd_key, n * 8, cudaMemcpyDeviceToHost, s));
-    CK(cudaMemcpyAsync(block_idx, ctx->d_lmd_block, n * 4, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
+    staging st(ctx);
+    st.out(key.data(), ctx->reg.lmd_key, n);
+    st.out(block_idx, ctx->reg.lmd_block, n);
+    int rc;
+    if ((rc = st.finish())) return rc;
     for (uint64_t v = 0; v < n; v++) {
         has_msg[v] = key[v] != 0;
         epoch[v] = key[v] >> 32;
@@ -1057,11 +1033,11 @@ int b2_latest_messages_update_dev(b2_ctx* ctx, const uint32_t* d_members, const 
     REQUIRE(ctx->n_val > 0, "latest_messages_update: registry not loaded");
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
-    k_lmd_phase1<<<n_agg, 128, 0, s>>>(d_members, d_off, d_bits, bits_stride, d_target_epoch, d_accept, ctx->d_equiv, n_agg, ctx->d_lmd_key,
+    k_lmd_phase1<<<n_agg, 128, 0, s>>>(d_members, d_off, d_bits, bits_stride, d_target_epoch, d_accept, ctx->reg.equiv, n_agg, ctx->reg.lmd_key,
                                        ctx->n_val, ctx->d_guard);
     CKL(ctx);
-    k_lmd_phase2<<<n_agg, 128, 0, s>>>(d_members, d_off, d_bits, bits_stride, d_target_epoch, d_block_idx, d_accept, ctx->d_equiv, n_agg,
-                                       ctx->d_lmd_key, ctx->d_lmd_block, ctx->n_val);
+    k_lmd_phase2<<<n_agg, 128, 0, s>>>(d_members, d_off, d_bits, bits_stride, d_target_epoch, d_block_idx, d_accept, ctx->reg.equiv, n_agg,
+                                       ctx->reg.lmd_key, ctx->reg.lmd_block, ctx->n_val);
     CKL(ctx);
     return B2_OK;
 }
@@ -1075,19 +1051,15 @@ int b2_latest_messages_update(b2_ctx* ctx, const uint32_t* members, const uint32
     if ((rc = check_batch(ctx, members, off, bits_stride, n_agg, ctx->n_val))) return rc;
     for (uint32_t a = 0; a < n_agg; a++) REQUIRE(target_epoch[a] < 0xffffffffull, "latest_messages_update: epoch does not fit 32 bits");
     CK(cudaSetDevice(ctx->device));
-    cudaStream_t s = ctx->s_main;
-    if ((rc = upload_batch(ctx, members, off, bits, bits_stride, n_agg, s))) return rc;
-    if ((rc = ensure(ctx, ctx->in_d, (size_t)n_agg * 8)) || (rc = ensure(ctx, ctx->in_e, (size_t)n_agg * 4)) || (rc = ensure(ctx, ctx->in_f, n_agg)))
-        return rc;
-    CK(cudaMemcpyAsync(ctx->in_d.p, target_epoch, (size_t)n_agg * 8, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->in_e.p, block_idx, (size_t)n_agg * 4, cudaMemcpyHostToDevice, s));
-    if (accept) CK(cudaMemcpyAsync(ctx->in_f.p, accept, n_agg, cudaMemcpyHostToDevice, s));
-    if ((rc = b2_latest_messages_update_dev(ctx, (const uint32_t*)ctx->in_a.p, (const uint32_t*)ctx->in_b.p, (const uint8_t*)ctx->in_c.p, bits_stride,
-                                            (const uint64_t*)ctx->in_d.p, (const uint32_t*)ctx->in_e.p, accept ? (const uint8_t*)ctx->in_f.p : nullptr,
-                                            n_agg, s)))
-        return rc;
-    CK(cudaStreamSynchronize(s));
-    return B2_OK;
+    staging st(ctx);
+    const uint32_t* dm = st.in(members, off[n_agg], 4);
+    const uint32_t* dof = st.in(off, (size_t)n_agg + 1);
+    const uint8_t* db = st.in(bits, (size_t)n_agg * bits_stride, 16);
+    const uint64_t* dte = st.in(target_epoch, n_agg);
+    const uint32_t* dbi = st.in(block_idx, n_agg);
+    const uint8_t* dacc = accept ? st.in(accept, n_agg) : nullptr;
+    if ((rc = st.rc) || (rc = b2_latest_messages_update_dev(ctx, dm, dof, db, bits_stride, dte, dbi, dacc, n_agg, ctx->s_main))) return rc;
+    return st.finish();
 }
 
 // ------------------------------------------------------------------------------------------ participation flags (process_attestation :738-754)
@@ -1097,23 +1069,28 @@ int b2_participation_load(b2_ctx* ctx, int which, const uint8_t* participation, 
     CK(cudaSetDevice(ctx->device));
     int rc;
     const size_t words = (n + 3) / 4;
-    if (!ctx->d_part[which] && (rc = dev_alloc(ctx, &ctx->d_part[which], words))) return rc;
-    if (!ctx->d_part_first) {
-        if ((rc = dev_alloc(ctx, &ctx->d_part_first, 3 * n))) return rc;
-        CK(cudaMemsetAsync(ctx->d_part_first, 0xff, 3 * n * 4, ctx->s_main));
+    // tables allocated by this call join the context only once they are initialised
+    dbuf part, first;
+    if (!ctx->reg.part[which] && (rc = ensure(ctx, part, words * 4))) return rc;
+    if (!ctx->reg.part_first) {
+        if ((rc = ensure(ctx, first, 3 * n * 4))) return rc;
+        CK(cudaMemsetAsync(first, 0xff, 3 * n * 4, ctx->s_main));
     }
-    CK(cudaMemsetAsync(ctx->d_part[which], 0, words * 4, ctx->s_main));
-    CK(cudaMemcpyAsync(ctx->d_part[which], participation, n, cudaMemcpyHostToDevice, ctx->s_main));
+    void* dst = part ? part : ctx->reg.part[which];
+    CK(cudaMemsetAsync(dst, 0, words * 4, ctx->s_main));
+    CK(cudaMemcpyAsync(dst, participation, n, cudaMemcpyHostToDevice, ctx->s_main));
     CK(cudaStreamSynchronize(ctx->s_main));
+    if (part) ctx->reg.part[which] = std::move(part);
+    if (first) ctx->reg.part_first = std::move(first);
     return B2_OK;
 }
 int b2_participation_read(b2_ctx* ctx, int which, uint8_t* participation_out, uint64_t n) {
     B2_NVTX;
-    REQUIRE(ctx && (which == 0 || which == 1) && participation_out && n == ctx->n_val && ctx->d_part[which], "participation_read: not loaded / bad arguments");
+    REQUIRE(ctx && (which == 0 || which == 1) && participation_out && n == ctx->n_val && ctx->reg.part[which], "participation_read: not loaded / bad arguments");
     CK(cudaSetDevice(ctx->device));
-    CK(cudaMemcpyAsync(participation_out, ctx->d_part[which], n, cudaMemcpyDeviceToHost, ctx->s_main));
-    CK(cudaStreamSynchronize(ctx->s_main));
-    return B2_OK;
+    staging st(ctx);
+    st.out(participation_out, ctx->reg.part[which], n);
+    return st.finish();
 }
 int b2_participation_update(b2_ctx* ctx, int which, const uint32_t* members, const uint32_t* off, const uint8_t* bits, uint32_t bits_stride,
                             const uint8_t* flag_mask, const uint8_t* accept, uint32_t n_agg, uint64_t effective_balance_increment,
@@ -1121,27 +1098,28 @@ int b2_participation_update(b2_ctx* ctx, int which, const uint32_t* members, con
     B2_NVTX;
     REQUIRE(ctx && (which == 0 || which == 1) && members && off && bits && flag_mask && numerator_out && n_agg > 0 && bits_stride > 0 &&
                 effective_balance_increment > 0, "participation_update: bad arguments");
-    REQUIRE(ctx->n_val > 0 && ctx->d_part[which], "participation_update: registry / participation table not loaded");
+    REQUIRE(ctx->n_val > 0 && ctx->reg.part[which], "participation_update: registry / participation table not loaded");
     int rc;
     if ((rc = check_batch(ctx, members, off, bits_stride, n_agg, ctx->n_val))) return rc;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->s_main;
-    if ((rc = upload_batch(ctx, members, off, bits, bits_stride, n_agg, s))) return rc;
-    if ((rc = ensure(ctx, ctx->in_d, n_agg)) || (rc = ensure(ctx, ctx->in_f, n_agg)) || (rc = ensure(ctx, ctx->out_a, (size_t)n_agg * 8))) return rc;
-    CK(cudaMemcpyAsync(ctx->in_d.p, flag_mask, n_agg, cudaMemcpyHostToDevice, s));
-    if (accept) CK(cudaMemcpyAsync(ctx->in_f.p, accept, n_agg, cudaMemcpyHostToDevice, s));
-    const uint32_t *dm = (const uint32_t*)ctx->in_a.p, *dof = (const uint32_t*)ctx->in_b.p;
-    const uint8_t *db = (const uint8_t*)ctx->in_c.p, *dmask = (const uint8_t*)ctx->in_d.p, *dacc = accept ? (const uint8_t*)ctx->in_f.p : nullptr;
-    k_part_phase1<<<n_agg, 128, 0, s>>>(dm, dof, db, bits_stride, dmask, dacc, n_agg, (const uint8_t*)ctx->d_part[which], ctx->d_part_first);
+    staging st(ctx);
+    const uint32_t* dm = st.in(members, off[n_agg], 4);
+    const uint32_t* dof = st.in(off, (size_t)n_agg + 1);
+    const uint8_t* db = st.in(bits, (size_t)n_agg * bits_stride, 16);
+    const uint8_t* dmask = st.in(flag_mask, n_agg);
+    const uint8_t* dacc = accept ? st.in(accept, n_agg) : nullptr;
+    uint64_t* dnum = st.out(numerator_out, n_agg);
+    if (st.rc) return st.rc;
+    const registry_tables& R = ctx->reg;
+    k_part_phase1<<<n_agg, 128, 0, s>>>(dm, dof, db, bits_stride, dmask, dacc, n_agg, R.part[which], R.part_first);
     CKL(ctx);
-    k_part_phase2<<<n_agg, 128, 0, s>>>(dm, dof, db, bits_stride, dmask, dacc, n_agg, ctx->d_part_first, ctx->d_eff, effective_balance_increment,
-                                        base_reward_per_increment, (unsigned long long*)ctx->out_a.p);
+    k_part_phase2<<<n_agg, 128, 0, s>>>(dm, dof, db, bits_stride, dmask, dacc, n_agg, R.part_first, R.eff, effective_balance_increment,
+                                        base_reward_per_increment, (unsigned long long*)dnum);
     CKL(ctx);
-    k_part_phase3<<<n_agg, 128, 0, s>>>(dm, dof, db, bits_stride, dmask, dacc, n_agg, ctx->d_part_first, ctx->d_part[which]);
+    k_part_phase3<<<n_agg, 128, 0, s>>>(dm, dof, db, bits_stride, dmask, dacc, n_agg, R.part_first, R.part[which]);
     CKL(ctx);
-    CK(cudaMemcpyAsync(numerator_out, ctx->out_a.p, (size_t)n_agg * 8, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return B2_OK;
+    return st.finish();
 }
 
 // ------------------------------------------------------------------------------------------ FFG balance sums (:793-803)
@@ -1151,15 +1129,14 @@ int b2_ffg_balances(b2_ctx* ctx, uint32_t flag_index, uint64_t* out4) {
     REQUIRE(ctx->n_val > 0, "ffg_balances: registry not loaded");
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->s_main;
-    int rc;
-    if ((rc = ensure(ctx, ctx->out_b, 32))) return rc;
-    CK(cudaMemsetAsync(ctx->out_b.p, 0, 32, s));
-    k_ffg_balances<<<ctx->n_sm * 4, 256, 0, s>>>(ctx->n_val, (const unsigned long long*)ctx->d_eff, ctx->d_flags, (const uint8_t*)ctx->d_part[0],
-                                                 (const uint8_t*)ctx->d_part[1], flag_index, (unsigned long long*)ctx->out_b.p);
+    staging st(ctx);
+    uint64_t* d4 = st.out(out4, 4);
+    if (st.rc) return st.rc;
+    CK(cudaMemsetAsync(d4, 0, 32, s));
+    k_ffg_balances<<<ctx->n_sm * 4, 256, 0, s>>>(ctx->n_val, ctx->reg.eff, ctx->reg.flags, ctx->reg.part[0], ctx->reg.part[1], flag_index,
+                                                 (unsigned long long*)d4);
     CKL(ctx);
-    CK(cudaMemcpyAsync(out4, ctx->out_b.p, 32, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return B2_OK;
+    return st.finish();
 }
 
 // ------------------------------------------------------------------------------------------ fork-choice variants
@@ -1188,15 +1165,13 @@ int b2_on_attester_slashing(b2_ctx* ctx, const uint32_t* indices_1, uint32_t n1,
     for (uint32_t i = 1; i < n2; i++) REQUIRE(indices_2[i - 1] < indices_2[i], "on_attester_slashing: attesting_indices must be sorted and unique");
     if (n1 == 0 || n2 == 0) return B2_OK;
     CK(cudaSetDevice(ctx->device));
-    cudaStream_t s = ctx->s_main;
-    int rc;
-    if ((rc = ensure(ctx, ctx->in_a, (size_t)n1 * 4)) || (rc = ensure(ctx, ctx->in_b, (size_t)n2 * 4))) return rc;
-    CK(cudaMemcpyAsync(ctx->in_a.p, indices_1, (size_t)n1 * 4, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->in_b.p, indices_2, (size_t)n2 * 4, cudaMemcpyHostToDevice, s));
-    k_mark_equivocating<<<blocks_for(n1, 128), 128, 0, s>>>((const uint32_t*)ctx->in_a.p, n1, (const uint32_t*)ctx->in_b.p, n2, ctx->n_val, ctx->d_equiv);
+    staging st(ctx);
+    const uint32_t* d1 = st.in(indices_1, n1);
+    const uint32_t* d2 = st.in(indices_2, n2);
+    if (st.rc) return st.rc;
+    k_mark_equivocating<<<blocks_for(n1, 128), 128, 0, ctx->s_main>>>(d1, n1, d2, n2, ctx->n_val, ctx->reg.equiv);
     CKL(ctx);
-    CK(cudaStreamSynchronize(s));
-    return B2_OK;
+    return st.finish();
 }
 
 // ------------------------------------------------------------------------------------------ block tree
@@ -1246,28 +1221,32 @@ int b2_tree_load(b2_ctx* ctx, const uint32_t* parent, const uint64_t* slot, cons
         rank_p[p] = rank[b];
         packed[p] = (size[b] & 0x7fffu) | ((rank[b] & 0x7fffu) << 15) | (keep[b] ? 0x80000000u : 0u);
     }
-    if ((rc = dev_alloc(ctx, &ctx->d_pre, n)) || (rc = dev_alloc(ctx, &ctx->d_inv, n)) || (rc = dev_alloc(ctx, &ctx->d_size_keep, n)) ||
-        (rc = dev_alloc(ctx, &ctx->d_rank, n)) || (rc = dev_alloc(ctx, &ctx->d_next, (size_t)n + 1)) || (rc = dev_alloc(ctx, &ctx->d_gsize, n)) ||
-        (rc = dev_alloc(ctx, &ctx->d_votes, n)) || (rc = dev_alloc(ctx, &ctx->d_prefix, (size_t)n + 1)) || (rc = dev_alloc(ctx, &ctx->d_w2, n)) ||
-        (rc = dev_alloc(ctx, &ctx->d_weight, n)) || (rc = dev_alloc(ctx, &ctx->d_head, 1)) || (rc = dev_alloc(ctx, &ctx->d_packed, n)))
+    // the new tables replace the old ones only once complete, so a failed load leaves the tree as it was
+    tree_tables t;
+    if ((rc = ensure(ctx, t.pre, (size_t)n * 4)) || (rc = ensure(ctx, t.inv, (size_t)n * 4)) || (rc = ensure(ctx, t.size_keep, (size_t)n * 4)) ||
+        (rc = ensure(ctx, t.rank, (size_t)n * 4)) || (rc = ensure(ctx, t.next, ((size_t)n + 1) * 4)) || (rc = ensure(ctx, t.gsize, (size_t)n * 4)) ||
+        (rc = ensure(ctx, t.votes, (size_t)n * 8)) || (rc = ensure(ctx, t.prefix, ((size_t)n + 1) * 8)) || (rc = ensure(ctx, t.w2, (size_t)n * 8)) ||
+        (rc = ensure(ctx, t.weight, (size_t)n * 8)) || (rc = ensure(ctx, t.head, 4)) || (rc = ensure(ctx, t.packed, (size_t)n * 4)))
         return rc;
     cudaStream_t s = ctx->s_main;
-    CK(cudaMemcpyAsync(ctx->d_packed, packed.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    ctx->packed_ok = n < 32768;
-    CK(cudaMemcpyAsync(ctx->d_pre, pre.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->d_inv, inv.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->d_size_keep, size_keep.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(ctx->d_rank, rank_p.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    CK(cudaMemsetAsync(ctx->d_votes, 0, (size_t)n * 8, s));
+    CK(cudaMemcpyAsync(t.packed, packed.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(t.pre, pre.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(t.inv, inv.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(t.size_keep, size_keep.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(t.rank, rank_p.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
+    CK(cudaMemsetAsync(t.votes, 0, (size_t)n * 8, s));
     CK(cudaStreamSynchronize(s));
+    ctx->tree = std::move(t);
+    ctx->packed_ok = n < 32768;
     ctx->n_blocks = n;
     return B2_OK;
 }
 
 // the vote scatter's view of the validators [v_begin, v_end) under the context's fork-choice variant
 static ghost_votes_args votes_args(const b2_ctx* ctx, uint64_t v_begin, uint64_t v_end) {
-    return {v_end - v_begin, ctx->d_lmd_key + v_begin, ctx->d_lmd_block + v_begin, ctx->d_equiv + v_begin, ctx->d_flags + v_begin, ctx->d_eff + v_begin,
-            ctx->fc_min_key, 1u, ctx->fc_exclude_slashed ? 3u : 1u};
+    const registry_tables& R = ctx->reg;
+    return {v_end - v_begin, (unsigned long long*)R.lmd_key + v_begin, (uint32_t*)R.lmd_block + v_begin, (uint8_t*)R.equiv + v_begin,
+            (uint8_t*)R.flags + v_begin, (uint64_t*)R.eff + v_begin, ctx->fc_min_key, 1u, ctx->fc_exclude_slashed ? 3u : 1u};
 }
 
 // Arguments of the tree phase (K9); returns the dynamic shared memory to launch it with.  The shared-memory form (use_smem) holds
@@ -1276,17 +1255,18 @@ static ghost_votes_args votes_args(const b2_ctx* ctx, uint64_t v_begin, uint64_t
 // (hard_list).  Trees that do not fit run the generic form on global scratch (0 bytes).
 static size_t fill_tree_args(b2_ctx* ctx, ghost_tree_args& A, uint64_t* d_votes_preorder, uint32_t justified_idx, int32_t boost_idx, uint64_t boost_score,
                              uint64_t* d_weight_out, uint32_t* d_head_idx_out) {
+    const tree_tables& T = ctx->tree;
     A.n = ctx->n_blocks;
-    A.pre = ctx->d_pre;
-    A.inv = ctx->d_inv;
-    A.size_keep = ctx->d_size_keep;
-    A.rank = ctx->d_rank;
-    A.packed = ctx->packed_ok ? ctx->d_packed : nullptr;
+    A.pre = T.pre;
+    A.inv = T.inv;
+    A.size_keep = T.size_keep;
+    A.rank = T.rank;
+    A.packed = ctx->packed_ok ? (const uint32_t*)T.packed : nullptr;
     A.votes = (unsigned long long*)d_votes_preorder;
-    A.g_w = ctx->d_prefix;
-    A.g_w2 = ctx->d_w2;
-    A.g_size = ctx->d_gsize;
-    A.g_next = ctx->d_next;
+    A.g_w = T.prefix;
+    A.g_w2 = T.w2;
+    A.g_size = T.gsize;
+    A.g_next = T.next;
     A.weight_out = (unsigned long long*)d_weight_out;
     A.head_out = d_head_idx_out;
     A.justified = justified_idx;
@@ -1311,7 +1291,7 @@ static int wait_head(b2_ctx* ctx, uint32_t seq, cudaStream_t s, const char* what
             if (q != cudaErrorNotReady && q != cudaSuccess) return fail_cuda(ctx, q, what);
             if (q == cudaSuccess && (uint32_t)(*slot64 >> 32) != seq) {
                 uint32_t h = 0;
-                CK(cudaMemcpy(&h, ctx->d_head, 4, cudaMemcpyDeviceToHost));
+                CK(cudaMemcpy(&h, ctx->tree.head, 4, cudaMemcpyDeviceToHost));
                 *head_idx_out = h;
                 return B2_OK;
             }
@@ -1335,7 +1315,7 @@ int b2_vote_weights_range_dev(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, uin
         const bool smem = bins_bytes <= 200 * 1024;
         const unsigned grid = smem ? (unsigned)std::min<uint64_t>((uint64_t)ctx->n_sm, (V.n + 1023) / 1024) : blocks_for(V.n, 256);
         (smem ? k_ghost_votes_smem : k_ghost_votes)<<<grid, smem ? 1024 : 256, smem ? bins_bytes : 0, s>>>(
-            V.n, V.lmd_key, V.lmd_block, V.equiv, V.flags, V.eff, ctx->d_pre, ctx->n_blocks, (unsigned long long*)d_votes_preorder, V.min_key, V.flag_need,
+            V.n, V.lmd_key, V.lmd_block, V.equiv, V.flags, V.eff, ctx->tree.pre, ctx->n_blocks, (unsigned long long*)d_votes_preorder, V.min_key, V.flag_need,
             V.flag_mask);
         CKL(ctx);
     }
@@ -1369,11 +1349,11 @@ int b2_get_weights(b2_ctx* ctx, int32_t boost_idx, uint64_t boost_score, uint64_
     REQUIRE(ctx->n_val > 0 && ctx->n_blocks > 0, "get_weights: registry or tree not loaded");
     int rc;
     cudaStream_t s = ctx->s_main;
-    if ((rc = b2_vote_weights_dev(ctx, (uint64_t*)ctx->d_votes, s))) return rc;
-    if ((rc = b2_head_from_votes_dev(ctx, (uint64_t*)ctx->d_votes, 0, boost_idx, boost_score, (uint64_t*)ctx->d_weight, ctx->d_head, s))) return rc;
-    CK(cudaMemcpyAsync(weight_out, ctx->d_weight, (size_t)ctx->n_blocks * 8, cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    return B2_OK;
+    const tree_tables& T = ctx->tree;
+    if ((rc = b2_vote_weights_dev(ctx, T.votes, s)) || (rc = b2_head_from_votes_dev(ctx, T.votes, 0, boost_idx, boost_score, T.weight, T.head, s))) return rc;
+    staging st(ctx);
+    st.out(weight_out, T.weight, ctx->n_blocks);
+    return st.finish();
 }
 
 // ---- multi-GPU get_head with the all-reduce fused in over NVLink peer memory (k_get_head_fused_nvl)
@@ -1389,13 +1369,13 @@ int b2_fc_exchange_export(b2_ctx* ctx, uint8_t* handle64_out) {
         if (ctx->fc_peer[r] && r != ctx->fc_rank) CK(cudaIpcCloseMemHandle(ctx->fc_peer[r]));
         ctx->fc_peer[r] = nullptr;
     }
-    if (ctx->fc_block) CK(cudaFree(ctx->fc_block));
-    ctx->fc_block = nullptr;
+    ctx->fc_block = dbuf();
     ctx->fc_rank = -1;
     ctx->fc_world = 0;
-    ctx->fc_block_bytes = fc_acc_bytes(ctx->n_blocks) + 2 * B2_MAX_PEERS * sizeof(unsigned int);
-    CK(cudaMalloc(&ctx->fc_block, ctx->fc_block_bytes));
-    CK(cudaMemset(ctx->fc_block, 0, ctx->fc_block_bytes));
+    const size_t bytes = fc_acc_bytes(ctx->n_blocks) + 2 * B2_MAX_PEERS * sizeof(unsigned int);
+    int rc;
+    if ((rc = ensure(ctx, ctx->fc_block, bytes))) return rc;
+    CK(cudaMemset(ctx->fc_block, 0, bytes));
     ctx->fc_blocks_cap = ctx->n_blocks;
     ctx->fc_seq = 0;
     cudaIpcMemHandle_t h;
@@ -1431,7 +1411,7 @@ int b2_get_head_multi(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, uint32_t ju
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->s_main;
     ghost_tree_args A;
-    const size_t smem = fill_tree_args(ctx, A, (uint64_t*)ctx->d_votes, justified_idx, boost_idx, boost_score, nullptr, ctx->d_head);
+    const size_t smem = fill_tree_args(ctx, A, ctx->tree.votes, justified_idx, boost_idx, boost_score, nullptr, ctx->tree.head);
     REQUIRE(A.use_smem && A.packed, "get_head_multi: the tree does not fit the shared-memory form (< ~14 500 blocks)");
     const ghost_votes_args V = votes_args(ctx, v_begin, v_end);
     ghost_peer_args P;
@@ -1445,7 +1425,7 @@ int b2_get_head_multi(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, uint32_t ju
     P.world = (uint32_t)ctx->fc_world;
     P.seq = seq;
     const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)ctx->n_sm, (V.n + 1023) / 1024));
-    k_get_head_fused_nvl<<<grid, 1024, smem, s>>>(V, A, P, ctx->d_ticket, (unsigned long long*)ctx->d_votes, ctx->d_head_host, hseq);
+    k_get_head_fused_nvl<<<grid, 1024, smem, s>>>(V, A, P, ctx->d_ticket, ctx->tree.votes, ctx->d_head_host, hseq);
     CKL(ctx);
     CK(cudaEventRecord(ctx->ev_votes_done, s));
     return wait_head(ctx, hseq, s, "get_head_multi kernel", head_idx_out);
@@ -1460,9 +1440,12 @@ int b2_debug_head_clocks(b2_ctx* ctx, uint64_t* out32) {
     REQUIRE(ctx && out32, "debug_head_clocks: bad arguments");
     CK(cudaSetDevice(ctx->device));
     CK(cudaDeviceSynchronize());
-    CK(cudaMemcpy(out32, ctx->d_dbg, 32 * 8, cudaMemcpyDeviceToHost));
-    CK(cudaMemset(ctx->d_dbg, 0, 32 * 8));
-    return B2_OK;
+    staging st(ctx);
+    uint64_t* d = st.out(out32, 32);
+    if (st.rc) return st.rc;
+    CK(cudaMemcpyAsync(d, ctx->d_dbg, 32 * 8, cudaMemcpyDeviceToDevice, ctx->s_main));
+    CK(cudaMemsetAsync(ctx->d_dbg, 0, 32 * 8, ctx->s_main));
+    return st.finish();
 }
 
 int b2_get_head(b2_ctx* ctx, uint32_t justified_idx, int32_t boost_idx, uint64_t boost_score, uint32_t* head_idx_out) {
@@ -1473,7 +1456,7 @@ int b2_get_head(b2_ctx* ctx, uint32_t justified_idx, int32_t boost_idx, uint64_t
     int rc;
     cudaStream_t s = ctx->s_main;
     ghost_tree_args A;
-    const size_t smem = fill_tree_args(ctx, A, (uint64_t*)ctx->d_votes, justified_idx, boost_idx, boost_score, nullptr, ctx->d_head);
+    const size_t smem = fill_tree_args(ctx, A, ctx->tree.votes, justified_idx, boost_idx, boost_score, nullptr, ctx->tree.head);
     if (ctx->head_fused && A.use_smem && A.packed) {
         // one launch; the kernel writes (head, sequence) into mapped pinned memory and the host spins on the sequence number
         CK(cudaSetDevice(ctx->device));
@@ -1485,10 +1468,10 @@ int b2_get_head(b2_ctx* ctx, uint32_t justified_idx, int32_t boost_idx, uint64_t
         CK(cudaEventRecord(ctx->ev_votes_done, s));
         return wait_head(ctx, seq, s, "get_head kernel", head_idx_out);
     }
-    if ((rc = b2_vote_weights_dev(ctx, (uint64_t*)ctx->d_votes, s))) return rc;
-    if ((rc = b2_head_from_votes_dev(ctx, (uint64_t*)ctx->d_votes, justified_idx, boost_idx, boost_score, nullptr, ctx->d_head, s))) return rc;
+    if ((rc = b2_vote_weights_dev(ctx, ctx->tree.votes, s))) return rc;
+    if ((rc = b2_head_from_votes_dev(ctx, ctx->tree.votes, justified_idx, boost_idx, boost_score, nullptr, ctx->tree.head, s))) return rc;
     uint32_t h = 0;
-    CK(cudaMemcpyAsync(&h, ctx->d_head, 4, cudaMemcpyDeviceToHost, s));
+    CK(cudaMemcpyAsync(&h, ctx->tree.head, 4, cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     *head_idx_out = h;
     return B2_OK;
