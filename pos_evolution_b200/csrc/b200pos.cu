@@ -42,12 +42,34 @@ struct registry_tables {
     dbuf lmd_key, lmd_block, equiv;           // u64 epoch << 32 | 0xffffffff (0 = no message), u32 block, u8 equivocating
     dbuf part[2], part_first;                 // epoch participation flags (0 = current, 1 = previous), per-(validator, flag) election table
 };
-// block tree (b2_tree_load): everything the tree kernel reads is stored in pre-order
+// The shared-memory budgets of fork choice: the tree phase (227 KB per block minus the tree kernels' static shared memory) and the vote
+// scatter's per-CTA bins
+constexpr int TREE_SMEM_BYTES = 226 * 1024;
+constexpr int BINS_SMEM_BYTES = 200 * 1024;
+
+// The kernels a tree runs, a function of its size alone (tree_form_of)
+struct tree_form {
+    bool smem_tree;         // the tree phase in shared memory (ghost_tree_smem), else the generic form on global memory
+    bool work_list;         // ... with the work list of the marking phase
+    size_t tree_smem;       // dynamic shared memory of the tree phase
+    bool smem_bins;         // the vote scatter's bins in shared memory (k_ghost_votes_smem), else global atomics (k_ghost_votes)
+};
+// The shared-memory tree phase holds votes/prefix/weights u64[n+1], the packed word u32[n] and marks u32[n+1] in TREE_SMEM_BYTES, at most
+// 15 elements per thread; when it still fits, the launch also reserves the work list u32[n].  The bins are u64[n].
+static tree_form tree_form_of(uint32_t n) {
+    const size_t base = ((size_t)n + 1) * 8 + (size_t)n * 8 + 8, with_list = base + (size_t)n * 4;
+    const bool smem = base <= TREE_SMEM_BYTES && n <= 15 * 1024, list = smem && with_list <= TREE_SMEM_BYTES;
+    return {smem, list, !smem ? 0 : list ? with_list : base, (size_t)n * 8 <= BINS_SMEM_BYTES};
+}
+
+// block tree (b2_tree_load): its form and the tables that form reads, in pre-order
 struct tree_tables {
-    dbuf pre, inv, size_keep, rank, next, gsize;      // u32
-    dbuf packed;                                      // u32 size | rank << 15 | keep << 31 (used for trees of < 32 768 blocks)
-    dbuf votes, prefix, weight, w2;                   // u64
-    dbuf head;                                        // u32
+    tree_form form = {};
+    dbuf pre, inv, head;                              // u32
+    dbuf votes, weight;                               // u64
+    dbuf packed;                                      // shared-memory form: u32 size | rank << 15 | keep << 31
+    dbuf size_keep, rank, next;                       // generic form: u32 size | keep << 31, u32 root rank, u32[n+1] marks
+    dbuf prefix, w2;                                  // generic form: u64[n+1] prefix sums, u64 weights
 };
 
 struct vslot {
@@ -117,7 +139,6 @@ struct b2_ctx {
     int fc_exclude_slashed = 0;
     // block tree
     uint32_t n_blocks = 0;
-    bool packed_ok = false;                           // tree.packed is read only when set
     tree_tables tree;
     // scratch
     dbuf sc_pkjac, sc_pkst, sc_haff, sc_hflag, sc_g2aff, sc_g2st, sc_rec, sc_val, sc_shuf, sc_pivot;
@@ -274,8 +295,8 @@ int b2_init(int device, b2_ctx** out) {
                                &ctx->slot[i].ev_in};
         for (int k = 0; k < 6 && e == cudaSuccess; k++) e = cudaEventCreateWithFlags(evs[k], cudaEventDisableTiming);
     }
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_ghost_tree, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_ghost_votes_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_ghost_tree, cudaFuncAttributeMaxDynamicSharedMemorySize, TREE_SMEM_BYTES);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_ghost_votes_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, BINS_SMEM_BYTES);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_g1_gather_tma<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * (int)sizeof(gather_ws));
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_g1_gather_tma<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * (int)sizeof(gather_ws));
     ctx->n_sm = prop.multiProcessorCount;
@@ -288,8 +309,8 @@ int b2_init(int device, b2_ctx** out) {
         memset((void*)ctx->h_head, 0, 64);
         e = cudaHostGetDevicePointer((void**)&ctx->d_head_host, (void*)ctx->h_head, 0);
     }
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_get_head_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_get_head_fused_nvl, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_get_head_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, TREE_SMEM_BYTES);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_get_head_fused_nvl, cudaFuncAttributeMaxDynamicSharedMemorySize, TREE_SMEM_BYTES);
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_rlc_seed.p, 32);
     if (e == cudaSuccess) e = cudaMemset(ctx->d_rlc_seed, 0, 32);
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_guard.p, 256);
@@ -1212,32 +1233,42 @@ int b2_tree_load(b2_ctx* ctx, const uint32_t* parent, const uint64_t* slot, cons
     for (uint32_t i = 0; i < n; i++) rank[order[i]] = i;
     CK(cudaSetDevice(ctx->device));
     int rc;
-    // everything the tree kernel reads is stored in pre-order
-    std::vector<uint32_t> inv(n), size_keep(n), rank_p(n), packed(n);
-    for (uint32_t b = 0; b < n; b++) {
-        const uint32_t p = pre[b];
-        inv[p] = b;
-        size_keep[p] = size[b] | (keep[b] ? 0x80000000u : 0u);
-        rank_p[p] = rank[b];
-        packed[p] = (size[b] & 0x7fffu) | ((rank[b] & 0x7fffu) << 15) | (keep[b] ? 0x80000000u : 0u);
-    }
-    // the new tables replace the old ones only once complete, so a failed load leaves the tree as it was
+    // the new form and tables replace the old ones only once complete, so a failed load leaves the tree as it was
     tree_tables t;
-    if ((rc = ensure(ctx, t.pre, (size_t)n * 4)) || (rc = ensure(ctx, t.inv, (size_t)n * 4)) || (rc = ensure(ctx, t.size_keep, (size_t)n * 4)) ||
-        (rc = ensure(ctx, t.rank, (size_t)n * 4)) || (rc = ensure(ctx, t.next, ((size_t)n + 1) * 4)) || (rc = ensure(ctx, t.gsize, (size_t)n * 4)) ||
-        (rc = ensure(ctx, t.votes, (size_t)n * 8)) || (rc = ensure(ctx, t.prefix, ((size_t)n + 1) * 8)) || (rc = ensure(ctx, t.w2, (size_t)n * 8)) ||
-        (rc = ensure(ctx, t.weight, (size_t)n * 8)) || (rc = ensure(ctx, t.head, 4)) || (rc = ensure(ctx, t.packed, (size_t)n * 4)))
+    t.form = tree_form_of(n);
+    const bool smem = t.form.smem_tree;
+    // the tables of the tree's form, in pre-order.  A shared-memory tree has at most 15 * 1024 blocks: size and rank fit 15 bits.
+    std::vector<uint32_t> inv(n), packed(smem ? n : 0), size_keep(smem ? 0 : n), rank_p(smem ? 0 : n);
+    for (uint32_t b = 0; b < n; b++) {
+        const uint32_t p = pre[b], k = keep[b] ? 0x80000000u : 0u;
+        inv[p] = b;
+        if (smem) {
+            packed[p] = size[b] | (rank[b] << 15) | k;
+        } else {
+            size_keep[p] = size[b] | k;
+            rank_p[p] = rank[b];
+        }
+    }
+    const size_t n4 = (size_t)n * 4, n8 = (size_t)n * 8;
+    if ((rc = ensure(ctx, t.pre, n4)) || (rc = ensure(ctx, t.inv, n4)) || (rc = ensure(ctx, t.head, 4)) || (rc = ensure(ctx, t.votes, n8)) ||
+        (rc = ensure(ctx, t.weight, n8)))
+        return rc;
+    if (smem && (rc = ensure(ctx, t.packed, n4))) return rc;
+    if (!smem && ((rc = ensure(ctx, t.size_keep, n4)) || (rc = ensure(ctx, t.rank, n4)) || (rc = ensure(ctx, t.next, n4 + 4)) ||
+                  (rc = ensure(ctx, t.prefix, n8 + 8)) || (rc = ensure(ctx, t.w2, n8))))
         return rc;
     cudaStream_t s = ctx->s_main;
-    CK(cudaMemcpyAsync(t.packed, packed.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(t.pre, pre.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(t.inv, inv.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(t.size_keep, size_keep.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(t.rank, rank_p.data(), (size_t)n * 4, cudaMemcpyHostToDevice, s));
-    CK(cudaMemsetAsync(t.votes, 0, (size_t)n * 8, s));
+    CK(cudaMemcpyAsync(t.pre, pre.data(), n4, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(t.inv, inv.data(), n4, cudaMemcpyHostToDevice, s));
+    if (smem) {
+        CK(cudaMemcpyAsync(t.packed, packed.data(), n4, cudaMemcpyHostToDevice, s));
+    } else {
+        CK(cudaMemcpyAsync(t.size_keep, size_keep.data(), n4, cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(t.rank, rank_p.data(), n4, cudaMemcpyHostToDevice, s));
+    }
+    CK(cudaMemsetAsync(t.votes, 0, n8, s));
     CK(cudaStreamSynchronize(s));
     ctx->tree = std::move(t);
-    ctx->packed_ok = n < 32768;
     ctx->n_blocks = n;
     return B2_OK;
 }
@@ -1249,35 +1280,14 @@ static ghost_votes_args votes_args(const b2_ctx* ctx, uint64_t v_begin, uint64_t
             (uint8_t*)R.flags + v_begin, (uint64_t*)R.eff + v_begin, ctx->fc_min_key, 1u, ctx->fc_exclude_slashed ? 3u : 1u};
 }
 
-// Arguments of the tree phase (K9); returns the dynamic shared memory to launch it with.  The shared-memory form (use_smem) holds
-// votes/prefix/weights u64[n+1], packed word u32[n] and marks u32[n+1] in 226 KB (227 KB per block minus the kernel's static shared
-// memory) and at most 15 elements per thread; when it still fits, the launch also reserves the work list u32[n] of the marking phase
-// (hard_list).  Trees that do not fit run the generic form on global scratch (0 bytes).
-static size_t fill_tree_args(b2_ctx* ctx, ghost_tree_args& A, uint64_t* d_votes_preorder, uint32_t justified_idx, int32_t boost_idx, uint64_t boost_score,
-                             uint64_t* d_weight_out, uint32_t* d_head_idx_out) {
+// the tree phase's (K9) view of the tree in its form, without host publication; it is launched with ctx->tree.form.tree_smem bytes of
+// dynamic shared memory
+static ghost_tree_args tree_args(const b2_ctx* ctx, uint64_t* d_votes_preorder, uint32_t justified_idx, int32_t boost_idx, uint64_t boost_score,
+                                 uint64_t* d_weight_out, uint32_t* d_head_idx_out) {
     const tree_tables& T = ctx->tree;
-    A.n = ctx->n_blocks;
-    A.pre = T.pre;
-    A.inv = T.inv;
-    A.size_keep = T.size_keep;
-    A.rank = T.rank;
-    A.packed = ctx->packed_ok ? (const uint32_t*)T.packed : nullptr;
-    A.votes = (unsigned long long*)d_votes_preorder;
-    A.g_w = T.prefix;
-    A.g_w2 = T.w2;
-    A.g_size = T.gsize;
-    A.g_next = T.next;
-    A.weight_out = (unsigned long long*)d_weight_out;
-    A.head_out = d_head_idx_out;
-    A.justified = justified_idx;
-    A.boost_idx = boost_idx;
-    A.boost_score = boost_score;
-    A.dbg = ctx->d_dbg;
-    const size_t base = ((size_t)A.n + 1) * 8 + (size_t)A.n * 8 + 8;
-    const size_t with_list = base + (size_t)A.n * 4;
-    A.use_smem = base <= 226 * 1024 && A.n <= 15 * 1024;
-    A.hard_list = A.use_smem && A.packed && with_list <= 226 * 1024;
-    return !A.use_smem ? 0 : A.hard_list ? with_list : base;
+    return {ctx->n_blocks, T.pre, T.inv, T.size_keep, T.rank, T.packed, (unsigned long long*)d_votes_preorder, T.prefix, T.w2, T.next,
+            (unsigned long long*)d_weight_out, d_head_idx_out, nullptr, 0, justified_idx, boost_idx, boost_score, T.form.smem_tree,
+            T.form.work_list, ctx->d_dbg};
 }
 
 // Spins on the mapped (head, sequence) slot until the get_head kernel on `s` has published call `seq`.  Every 2^20 polls it checks that
@@ -1312,7 +1322,7 @@ int b2_vote_weights_range_dev(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, uin
     const size_t bins_bytes = (size_t)ctx->n_blocks * 8;
     if (V.n > 0) {          // else nothing to scatter; the accumulator is clean by contract
         // the bins in shared memory when they fit (a persistent grid of at most one CTA per SM), else the global-atomic form
-        const bool smem = bins_bytes <= 200 * 1024;
+        const bool smem = ctx->tree.form.smem_bins;
         const unsigned grid = smem ? (unsigned)std::min<uint64_t>((uint64_t)ctx->n_sm, (V.n + 1023) / 1024) : blocks_for(V.n, 256);
         (smem ? k_ghost_votes_smem : k_ghost_votes)<<<grid, smem ? 1024 : 256, smem ? bins_bytes : 0, s>>>(
             V.n, V.lmd_key, V.lmd_block, V.equiv, V.flags, V.eff, ctx->tree.pre, ctx->n_blocks, (unsigned long long*)d_votes_preorder, V.min_key, V.flag_need,
@@ -1336,9 +1346,7 @@ int b2_head_from_votes_dev(b2_ctx* ctx, uint64_t* d_votes_preorder, uint32_t jus
     REQUIRE(justified_idx < ctx->n_blocks && boost_idx < (int32_t)ctx->n_blocks, "head_from_votes: block index out of range");
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
-    ghost_tree_args A;
-    const size_t smem = fill_tree_args(ctx, A, d_votes_preorder, justified_idx, boost_idx, boost_score, d_weight_out, d_head_idx_out);
-    k_ghost_tree<<<1, 1024, smem, s>>>(A);
+    k_ghost_tree<<<1, 1024, ctx->tree.form.tree_smem, s>>>(tree_args(ctx, d_votes_preorder, justified_idx, boost_idx, boost_score, d_weight_out, d_head_idx_out));
     CKL(ctx);
     return B2_OK;
 }
@@ -1410,9 +1418,8 @@ int b2_get_head_multi(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, uint32_t ju
     REQUIRE(justified_idx < ctx->n_blocks && boost_idx < (int32_t)ctx->n_blocks, "get_head_multi: block index out of range");
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->s_main;
-    ghost_tree_args A;
-    const size_t smem = fill_tree_args(ctx, A, ctx->tree.votes, justified_idx, boost_idx, boost_score, nullptr, ctx->tree.head);
-    REQUIRE(A.use_smem && A.packed, "get_head_multi: the tree does not fit the shared-memory form (< ~14 500 blocks)");
+    REQUIRE(ctx->tree.form.smem_tree, "get_head_multi: the tree does not fit the shared-memory form (<= 14 463 blocks)");
+    ghost_tree_args A = tree_args(ctx, ctx->tree.votes, justified_idx, boost_idx, boost_score, nullptr, ctx->tree.head);
     const ghost_votes_args V = votes_args(ctx, v_begin, v_end);
     ghost_peer_args P;
     const uint32_t seq = ++ctx->fc_seq ? ctx->fc_seq : ++ctx->fc_seq;                  // the collective call number (same on every rank)
@@ -1424,8 +1431,10 @@ int b2_get_head_multi(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, uint32_t ju
     P.rank = (uint32_t)ctx->fc_rank;
     P.world = (uint32_t)ctx->fc_world;
     P.seq = seq;
+    A.host_out = ctx->d_head_host;
+    A.host_seq = hseq;
     const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)ctx->n_sm, (V.n + 1023) / 1024));
-    k_get_head_fused_nvl<<<grid, 1024, smem, s>>>(V, A, P, ctx->d_ticket, ctx->tree.votes, ctx->d_head_host, hseq);
+    k_get_head_fused_nvl<<<grid, 1024, ctx->tree.form.tree_smem, s>>>(V, A, P, ctx->d_ticket, ctx->tree.votes);
     CKL(ctx);
     CK(cudaEventRecord(ctx->ev_votes_done, s));
     return wait_head(ctx, hseq, s, "get_head_multi kernel", head_idx_out);
@@ -1455,15 +1464,16 @@ int b2_get_head(b2_ctx* ctx, uint32_t justified_idx, int32_t boost_idx, uint64_t
     REQUIRE(justified_idx < ctx->n_blocks && boost_idx < (int32_t)ctx->n_blocks, "get_head: block index out of range");
     int rc;
     cudaStream_t s = ctx->s_main;
-    ghost_tree_args A;
-    const size_t smem = fill_tree_args(ctx, A, ctx->tree.votes, justified_idx, boost_idx, boost_score, nullptr, ctx->tree.head);
-    if (ctx->head_fused && A.use_smem && A.packed) {
+    if (ctx->head_fused && ctx->tree.form.smem_tree) {
         // one launch; the kernel writes (head, sequence) into mapped pinned memory and the host spins on the sequence number
         CK(cudaSetDevice(ctx->device));
+        ghost_tree_args A = tree_args(ctx, ctx->tree.votes, justified_idx, boost_idx, boost_score, nullptr, ctx->tree.head);
         const ghost_votes_args V = votes_args(ctx, 0, ctx->n_val);
         const uint32_t seq = ++ctx->head_seq ? ctx->head_seq : ++ctx->head_seq;       // never 0
+        A.host_out = ctx->d_head_host;
+        A.host_seq = seq;
         const unsigned grid = (unsigned)std::min<uint64_t>((uint64_t)ctx->n_sm, (V.n + 1023) / 1024);
-        k_get_head_fused<<<grid, 1024, smem, s>>>(V, A, ctx->d_ticket, ctx->d_head_host, seq);
+        k_get_head_fused<<<grid, 1024, ctx->tree.form.tree_smem, s>>>(V, A, ctx->d_ticket);
         CKL(ctx);
         CK(cudaEventRecord(ctx->ev_votes_done, s));
         return wait_head(ctx, seq, s, "get_head kernel", head_idx_out);

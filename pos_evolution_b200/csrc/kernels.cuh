@@ -451,6 +451,14 @@ __global__ void __launch_bounds__(128) k_lmd_phase2(const uint32_t* __restrict__
 }
 
 // ------------------------------------------------------------------------------------------ K8: vote scatter
+// Whether a validator's latest message counts towards get_latest_attesting_balance, in both vote scatters: it exists (key != 0), has not
+// expired (key >= min_key, the fork-choice variant's vote expiry), the validator does not equivocate, its flags pass the variant's test
+// (flags & flag_mask == flag_need: active, and not slashed when the variant excludes slashed validators), and it names a loaded block.
+// The callers have loaded every operand, so the tests are combined without branches.
+__device__ __forceinline__ bool latest_message_counts(unsigned long long key, uint32_t block, uint32_t equiv, uint32_t flags, unsigned long long min_key,
+                                                      uint32_t flag_need, uint32_t flag_mask, uint32_t n_blocks) {
+    return (key != 0) & (key >= min_key) & (equiv == 0) & ((flags & flag_mask) == flag_need) & (block < n_blocks);
+}
 // One thread per validator: coalesced reads of the latest-message table (u64 key + u32 block), the
 // effective-balance table (u64) and two byte masks; votes are combined inside the warp (lanes voting
 // for the same block elect a leader) and the leader issues one 64-bit atomic add into the pre-order
@@ -460,18 +468,15 @@ __global__ void __launch_bounds__(256) k_ghost_votes(uint64_t n, const unsigned 
                                                       const uint8_t* __restrict__ flags, const uint64_t* __restrict__ eff,
                                                       const uint32_t* __restrict__ pre, uint32_t n_blocks, unsigned long long* votes, unsigned long long min_key, uint32_t flag_need, uint32_t flag_mask) {
     uint64_t v = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    bool on = v < n;
+    bool on = false;
     uint32_t b = 0xffffffffu;
     unsigned long long bal = 0;
-    if (on) {
-        on = lmd_key[v] != 0 && lmd_key[v] >= min_key && !equiv[v] && ((flags[v] & flag_mask) == flag_need);
+    if (v < n) {
+        const uint32_t blk = lmd_block[v];
+        on = latest_message_counts(lmd_key[v], blk, equiv[v], flags[v], min_key, flag_need, flag_mask, n_blocks);
         if (on) {
-            uint32_t blk = lmd_block[v];
-            on = blk < n_blocks;
-            if (on) {
-                b = pre[blk];
-                bal = eff[v];
-            }
+            b = pre[blk];
+            bal = eff[v];
         }
     }
     const int lane = threadIdx.x & 31;
@@ -533,7 +538,7 @@ __device__ __forceinline__ void ghost_votes_body(unsigned long long* bins, const
         bool on[U];
 #pragma unroll
         for (int u = 0; u < U; u++) {
-            on[u] = key[u] != 0 && key[u] >= V.min_key && !eq[u] && ((fl[u] & V.flag_mask) == V.flag_need) && blk[u] < n_blocks;
+            on[u] = latest_message_counts(key[u], blk[u], eq[u], fl[u], V.min_key, V.flag_need, V.flag_mask, n_blocks);
             b[u] = on[u] ? pre[blk[u]] : 0xffffffffu;
         }
 #pragma unroll
@@ -583,28 +588,31 @@ __global__ void __launch_bounds__(1024) k_ghost_votes_smem(uint64_t n, const uns
 // mark every block that is NOT the best child of its parent; a block lies on the head path iff no block on its root path is
 // marked, i.e. iff the number of marked ancestors-or-self is zero.  That count is a second prefix sum (+1 at the marked block,
 // -1 past its subtree), and the head is the last pre-order position with count zero -- two scans and a max-reduction
-// instead of log2(n) rounds over all blocks.  Trees too large for shared memory use the same code on global scratch.
+// instead of log2(n) rounds over all blocks.  Trees too large for shared memory run the same algorithm on global memory (the generic
+// form, ghost_tree_body).  b2_tree_load chooses the form and builds only the tables it reads; the others are null.
 struct ghost_tree_args {
     uint32_t n;
     const uint32_t* pre;         // block -> pre-order position
     const uint32_t* inv;         // pre-order position -> block
-    const uint32_t* size_keep;   // pre-order: subtree size | (get_filtered_block_tree membership << 31)
-    const uint32_t* rank;        // pre-order: lexicographic rank of the 32-byte root (tie-break of :1114-1116)
-    const uint32_t* packed;      // pre-order, trees of < 32 768 blocks: size | rank << 15 | keep << 31 (one word: the shared-memory form)
+    const uint32_t* size_keep;   // generic form, pre-order: subtree size | (get_filtered_block_tree membership << 31)
+    const uint32_t* rank;        // generic form, pre-order: lexicographic rank of the 32-byte root (tie-break of :1114-1116)
+    const uint32_t* packed;      // shared-memory form, pre-order: size | rank << 15 | keep << 31 (one word per block)
     unsigned long long* votes;   // in: direct votes in pre-order; zeroed on exit
-    unsigned long long* g_w;     // global fallback scratch n+1 (prefix sums)
-    unsigned long long* g_w2;    // global fallback scratch n (weights)
-    uint32_t* g_size;            // global fallback scratch n
-    uint32_t* g_next;            // global fallback scratch n+1 (marks / counts)
+    unsigned long long* g_w;     // generic form scratch n+1 (prefix sums)
+    unsigned long long* g_w2;    // generic form scratch n (weights)
+    uint32_t* g_next;            // generic form scratch n+1 (marks / counts)
     unsigned long long* weight_out;  // optional, per block (original numbering)
     uint32_t* head_out;
+    uint32_t* host_out;          // optional: mapped pinned host memory that receives (head, host_seq) in one 64-bit store
+    uint32_t host_seq;
     uint32_t justified;
     int32_t boost_idx;
     unsigned long long boost_score;
-    int use_smem;
+    int use_smem;                // the shared-memory form (ghost_tree_smem) on packed; else the generic form
     int hard_list;               // shared-memory form: the launch reserved u32[n] more for the work list of the marking phase
     unsigned long long* dbg;     // optional: thread 0 of the tree phase stores clock64() at its phase boundaries (b2_debug_head_clocks)
 };
+#define B2_TREE_STAMP(k) do { if (A.dbg && threadIdx.x == 0) A.dbg[k] = clock64(); } while (0)
 
 // exclusive prefix sum of x[0..n) in place, x[n] = total; every thread of the block must call it
 template <class T> __device__ __forceinline__ void block_exclusive_scan(T* x, uint32_t n, T* warp_tot) {
@@ -643,25 +651,58 @@ template <class T> __device__ __forceinline__ void block_exclusive_scan(T* x, ui
     __syncthreads();
 }
 
-__device__ __forceinline__ void ghost_tree_body(const ghost_tree_args& A, unsigned long long* smem_u64, uint32_t* host_out, uint32_t host_seq) {
+// get_weight of every block, in the original numbering, from the weights w[] in pre-order
+__device__ __forceinline__ void store_weights(const ghost_tree_args& A, const unsigned long long* w) {
+    if (A.weight_out)
+        for (uint32_t b = threadIdx.x; b < A.n; b += blockDim.x) A.weight_out[b] = w[A.pre[b]];
+}
+// The end of the tree phase in both forms.  After the second scan mark[p+1] is the inclusive count at p = number of marked blocks among
+// p and its ancestors.  The head path below the justified block (at pre-order position jp) = the positions of its subtree whose count
+// equals the justified block's own count (nothing marked in between); the head is the last of them in pre-order.  The subtree sizes are
+// the size_mask bits of the form's per-block words size[].  Thread 0 stores the head to A.head_out and, if A.host_out is set, publishes
+// it there with A.host_seq.
+__device__ __forceinline__ void ghost_tree_head(const ghost_tree_args& A, const uint32_t* mark, const uint32_t* size, uint32_t size_mask, uint32_t jp,
+                                                uint32_t& head_pos) {
+    const uint32_t base = mark[jp + 1];
+    const uint32_t jend = jp + (size[jp] & size_mask);
+    uint32_t best_pos = 0;
+    bool have = false;
+    for (uint32_t p = jp + threadIdx.x; p < jend; p += blockDim.x) {
+        if (mark[p + 1] == base) {
+            best_pos = p;
+            have = true;
+        }
+    }
+    if (have) atomicMax(&head_pos, best_pos);
+    __syncthreads();
+    B2_TREE_STAMP(7);
+    if (threadIdx.x == 0) {
+        const uint32_t h = (A.justified < A.n) ? A.inv[max(head_pos, jp)] : 0xffffffffu;
+        *A.head_out = h;
+        if (A.host_out)                         // zero-copy result: (head, sequence number) in one 64-bit store to mapped pinned memory
+            *reinterpret_cast<volatile unsigned long long*>(A.host_out) = (unsigned long long)h | ((unsigned long long)A.host_seq << 32);
+    }
+    B2_TREE_STAMP(15);
+}
+
+// The generic form of the tree phase, for trees too large for shared memory: the tables and scratch of b2_tree_load in global memory.
+__device__ __forceinline__ void ghost_tree_body(const ghost_tree_args& A) {
     __shared__ unsigned long long warp_tot[32];
     __shared__ uint32_t warp_tot32[32];
     __shared__ uint32_t head_pos;
     const uint32_t n = A.n, tid = threadIdx.x, T = blockDim.x;
-#define B2_TREE_STAMP(k) do { if (A.dbg && tid == 0) A.dbg[k] = clock64(); } while (0)
     B2_TREE_STAMP(0);
-    unsigned long long* W = A.use_smem ? smem_u64 : A.g_w;                                     // n+1: votes -> prefix -> weights
-    uint32_t* size = A.use_smem ? reinterpret_cast<uint32_t*>(smem_u64 + (n + 1)) : A.g_size;   // n
-    uint32_t* mark = A.use_smem ? size + n : A.g_next;                                          // n+1: marks -> counts
+    unsigned long long* W = A.g_w;                                          // n+1: votes -> prefix sums
+    const uint32_t* size = A.size_keep;                                     // n
+    uint32_t* mark = A.g_next;                                              // n+1: marks -> counts
     const uint32_t boost_p = A.boost_idx >= 0 ? A.pre[A.boost_idx] : 0xffffffffu;
     if (tid == 0) head_pos = 0;
-    // stage votes (+ boost) and sizes, coalesced; leave the global accumulator clean for the next call
+    // stage votes (+ boost), coalesced; leave the global accumulator clean for the next call
     for (uint32_t p = tid; p < n; p += T) {
-        unsigned long long v = __ldcg(&A.votes[p]);      // L2: in the fused kernel other CTAs' atomics produced these values
+        unsigned long long v = __ldcg(&A.votes[p]);
         A.votes[p] = 0;
         if (p == boost_p) v += A.boost_score;
         W[p] = v;
-        size[p] = A.size_keep[p];
         mark[p] = 0;
     }
     if (tid == 0) mark[n] = 0;
@@ -669,31 +710,12 @@ __device__ __forceinline__ void ghost_tree_body(const ghost_tree_args& A, unsign
     B2_TREE_STAMP(1);
     block_exclusive_scan(W, n, warp_tot);
     B2_TREE_STAMP(2);
-    // weights: w[p] = S[p + size] - S[p].  Shared-memory mode overwrites S in place (through registers: the smem budget
-    // caps n at ~14 500 = 15 per thread); global mode writes a separate array.
-    unsigned long long* Wt = A.use_smem ? W : A.g_w2;
-    if (A.use_smem) {
-        constexpr int MAXPT = 15;
-        unsigned long long wreg[MAXPT];
-#pragma unroll
-        for (int j = 0; j < MAXPT; j++) {
-            uint32_t p = tid + j * T;
-            if (p < n) wreg[j] = W[p + (size[p] & 0x7fffffffu)] - W[p];
-        }
-        __syncthreads();
-    B2_TREE_STAMP(3);
-#pragma unroll
-        for (int j = 0; j < MAXPT; j++) {
-            uint32_t p = tid + j * T;
-            if (p < n) W[p] = wreg[j];
-        }
-    } else {
-        for (uint32_t p = tid; p < n; p += T) Wt[p] = W[p + (size[p] & 0x7fffffffu)] - W[p];
-    }
+    // weights: w[p] = S[p + size] - S[p]
+    unsigned long long* Wt = A.g_w2;
+    for (uint32_t p = tid; p < n; p += T) Wt[p] = W[p + (size[p] & 0x7fffffffu)] - W[p];
     __syncthreads();
     B2_TREE_STAMP(4);
-    if (A.weight_out)
-        for (uint32_t b = tid; b < n; b += T) A.weight_out[b] = Wt[A.pre[b]];
+    store_weights(A, Wt);
     // every child that is not its parent's best child gets +1 at its position and -1 just past its subtree
     const uint32_t jp = A.justified < n ? A.pre[A.justified] : 0;
     for (uint32_t p = tid; p < n; p += T) {
@@ -722,31 +744,10 @@ __device__ __forceinline__ void ghost_tree_body(const ghost_tree_args& A, unsign
     B2_TREE_STAMP(5);
     block_exclusive_scan(mark, n, warp_tot32);          // mark[p] = number of marked proper ancestors ... of positions < p
     B2_TREE_STAMP(6);
-    // after the scan mark[p+1] is the inclusive count at p = number of marked blocks among p and its ancestors.  The head path
-    // below the justified block = the positions of its subtree whose count equals the justified block's own count
-    // (nothing marked in between); the head is the last of them in pre-order.
-    const uint32_t base = mark[jp + 1];
-    const uint32_t jend = jp + (size[jp] & 0x7fffffffu);
-    uint32_t best_pos = 0;
-    bool have = false;
-    for (uint32_t p = jp + tid; p < jend; p += T) {
-        if (mark[p + 1] == base) {
-            best_pos = p;
-            have = true;
-        }
-    }
-    if (have) atomicMax(&head_pos, best_pos);
-    __syncthreads();
-    B2_TREE_STAMP(7);
-    if (tid == 0) {
-        const uint32_t h = (A.justified < n) ? A.inv[max(head_pos, jp)] : 0xffffffffu;
-        *A.head_out = h;
-        if (host_out) *reinterpret_cast<volatile unsigned long long*>(host_out) = (unsigned long long)h | ((unsigned long long)host_seq << 32);
-    }
-    B2_TREE_STAMP(15);
+    ghost_tree_head(A, mark, size, 0x7fffffffu, jp, head_pos);
 }
-// ---- the shared-memory form of the tree phase (every tree that fits: < ~14 500 blocks), specialised after the phase clocks of the
-// generic body (tools/head_clocks.py on an earlier GPU: 44 900 SM clocks = 23.6 us, of which marking 17 800, staging 8 700, first scan
+// ---- the shared-memory form of the tree phase (every tree that fits: <= 14 463 blocks), specialised after the phase clocks of the
+// generic body run on shared memory (tools/head_clocks.py on an earlier GPU: 44 900 SM clocks = 23.6 us, of which marking 17 800, staging 8 700, first scan
 // 6 100): (1) all arrays are __shared__ pointers -- LDS/STS instead of generic LD/ST whose address space is resolved at run time;
 // (2) the per-block word packs subtree size, root rank and the filter bit, so a tie between equal-weight siblings costs no global
 // load (the generic body reads A.rank[] from global memory inside the child loop); (3) the staging loop issues all of a thread's
@@ -806,8 +807,8 @@ template <class T, int MAXPT> __device__ __forceinline__ void smem_exclusive_sca
 // slots, so the phase times are instruction counts: the 15-trip form spends a third of its instructions on predicated-off trips
 // when n = 10 000 needs 10 (11 in the scans), hence the two instantiations behind ghost_tree_smem().
 template <int MAXPT>
-__device__ __forceinline__ void ghost_tree_smem_t(const ghost_tree_args& A, unsigned long long* smem_u64, uint32_t* host_out, uint32_t host_seq,
-                                               unsigned long long* warp_tot, uint32_t* warp_tot32, uint32_t* cells) {
+__device__ __forceinline__ void ghost_tree_smem_t(const ghost_tree_args& A, unsigned long long* smem_u64, unsigned long long* warp_tot, uint32_t* warp_tot32,
+                                                  uint32_t* cells) {
     uint32_t& head_pos = cells[0];
     uint32_t& n_hard = cells[1];
     const uint32_t n = A.n, tid = threadIdx.x, T = blockDim.x;
@@ -860,8 +861,7 @@ __device__ __forceinline__ void ghost_tree_smem_t(const ghost_tree_args& A, unsi
     }
     __syncthreads();
     B2_TREE_STAMP(4);
-    if (A.weight_out)
-        for (uint32_t b = tid; b < n; b += T) A.weight_out[b] = W[A.pre[b]];
+    store_weights(A, W);
     // every child that is not its parent's best child gets +1 at its position and -1 just past its subtree.
     // Most parents of a block tree have ONE child (the chain); it is trivially the best child and nothing is marked.  Looping over
     // parents thread by thread makes every warp wait for its lane with the most children in each of its ~10 trips (13 800 clocks).
@@ -943,41 +943,22 @@ __device__ __forceinline__ void ghost_tree_smem_t(const ghost_tree_args& A, unsi
     B2_TREE_STAMP(5);
     smem_exclusive_scan<uint32_t, MAXPT>(mark, n, warp_tot32);
     B2_TREE_STAMP(6);
-    const uint32_t base = mark[jp + 1];
-    const uint32_t jend = jp + B2_SZ(sz[jp]);
-    uint32_t best_pos = 0;
-    bool have = false;
-    for (uint32_t p = jp + tid; p < jend; p += T) {
-        if (mark[p + 1] == base) {
-            best_pos = p;
-            have = true;
-        }
-    }
-    if (have) atomicMax(&head_pos, best_pos);
-    __syncthreads();
-    B2_TREE_STAMP(7);
-    if (tid == 0) {
-        const uint32_t h = (A.justified < n) ? A.inv[max(head_pos, jp)] : 0xffffffffu;
-        *A.head_out = h;
-        if (host_out)                           // zero-copy result: (head, sequence number) in one 64-bit store to mapped pinned memory
-            *reinterpret_cast<volatile unsigned long long*>(host_out) = (unsigned long long)h | ((unsigned long long)host_seq << 32);
-    }
-    B2_TREE_STAMP(15);
+    ghost_tree_head(A, mark, sz, 0x7fffu, jp, head_pos);             // the B2_SZ field
 }
-__device__ __forceinline__ void ghost_tree_smem(const ghost_tree_args& A, unsigned long long* smem_u64, uint32_t* host_out, uint32_t host_seq) {
+__device__ __forceinline__ void ghost_tree_smem(const ghost_tree_args& A, unsigned long long* smem_u64) {
     __shared__ unsigned long long warp_tot[32];
     __shared__ uint32_t warp_tot32[32];
     __shared__ uint32_t cells[2];                                           // head position, length of the work list
-    if (A.n <= 11u * blockDim.x) ghost_tree_smem_t<11>(A, smem_u64, host_out, host_seq, warp_tot, warp_tot32, cells);
-    else ghost_tree_smem_t<15>(A, smem_u64, host_out, host_seq, warp_tot, warp_tot32, cells);      // n <= 15 * 1024: fill_tree_args's use_smem test
+    if (A.n <= 11u * blockDim.x) ghost_tree_smem_t<11>(A, smem_u64, warp_tot, warp_tot32, cells);
+    else ghost_tree_smem_t<15>(A, smem_u64, warp_tot, warp_tot32, cells);      // n <= 15 * 1024: tree_form_of's smem_tree test
 }
 
 __global__ void __launch_bounds__(1024) k_ghost_tree(ghost_tree_args A) {
     extern __shared__ unsigned long long smem_u64[];
-    if (A.use_smem && A.packed)
-        ghost_tree_smem(A, smem_u64, nullptr, 0);
+    if (A.use_smem)
+        ghost_tree_smem(A, smem_u64);
     else
-        ghost_tree_body(A, smem_u64, nullptr, 0);
+        ghost_tree_body(A);
 }
 // get_head in ONE launch (b2_get_head): every CTA scatters its share of the votes (K8), the CTA that finishes last -- elected by a
 // ticket counter -- runs the tree phase (K9) on the completed vote array and writes the head straight into mapped pinned host memory
@@ -996,12 +977,12 @@ __device__ __forceinline__ bool last_cta(unsigned int* ticket, bool& is_last) {
     if (threadIdx.x == 0) *ticket = 0;                 // re-armed for the next call
     return true;
 }
-__global__ void __launch_bounds__(1024) k_get_head_fused(ghost_votes_args V, ghost_tree_args A, unsigned int* ticket, uint32_t* host_out, uint32_t host_seq) {
+__global__ void __launch_bounds__(1024) k_get_head_fused(ghost_votes_args V, ghost_tree_args A, unsigned int* ticket) {
     extern __shared__ unsigned long long smem_u64[];
     __shared__ bool is_last;
     ghost_votes_body(smem_u64, V, A.pre, A.n, A.votes, A.dbg);
     if (!last_cta(ticket, is_last)) return;
-    ghost_tree_smem(A, smem_u64, host_out, host_seq);  // (the fused kernel is only launched for trees in the shared-memory form)
+    ghost_tree_smem(A, smem_u64);                      // (the fused kernel is only launched for trees in the shared-memory form)
 }
 
 // get_head over ONE validator set spread over the GPUs of a box (BASELINE.json config 4: N/8 validators per GPU) as one kernel per rank,
@@ -1021,7 +1002,7 @@ struct ghost_peer_args {
     uint32_t rank, world, seq;
 };
 __global__ void __launch_bounds__(1024) k_get_head_fused_nvl(ghost_votes_args V, ghost_tree_args A, ghost_peer_args P, unsigned int* ticket,
-                                                              unsigned long long* local_votes, uint32_t* host_out, uint32_t host_seq) {
+                                                              unsigned long long* local_votes) {
     extern __shared__ unsigned long long smem_u64[];
     __shared__ bool is_last;
     ghost_votes_body(smem_u64, V, A.pre, A.n, local_votes, A.dbg);
@@ -1048,7 +1029,7 @@ __global__ void __launch_bounds__(1024) k_get_head_fused_nvl(ghost_votes_args V,
     __threadfence_system();
     __syncthreads();
     A.votes = P.acc[P.rank] + (size_t)par * n;         // the tree phase reads (ld.cg) and zeroes the complete accumulator
-    ghost_tree_smem(A, smem_u64, host_out, host_seq);
+    ghost_tree_smem(A, smem_u64);
 }
 
 }  // namespace b2

@@ -12,7 +12,7 @@ from oracle import fast
 
 gpu = pytest.mark.gpu
 
-# the shared-memory budgets of the host code: fill_tree_args (tree phase: 226 KB per block) and b2_vote_weights_range_dev (vote bins)
+# the shared-memory budgets of the host code's tree_form_of: the tree phase (226 KB per block) and the vote bins
 TREE_SMEM_BYTES = 226 * 1024
 BINS_SMEM_BYTES = 200 * 1024
 
