@@ -83,6 +83,20 @@ int b2_fast_aggregate_verify(b2_ctx* ctx, const uint32_t* members, const uint32_
 int b2_fast_aggregate_verify_pks(b2_ctx* ctx, const uint8_t* pk48, const uint32_t* pk_off, const uint8_t* msg32,
                                  const uint8_t* sig96, uint32_t n_agg, uint8_t* ok_out);
 
+/* bls.AggregateVerify (IETF POP scheme: messages need NOT be distinct), batched.  Set s = pairs [pair_off[s], pair_off[s+1]):
+ * (pk48[i], msg32[i]) for each pair, and one signature sig96[s].  ok_out[s] = 1 iff the set is non-empty, every key passes
+ * KeyValidate, the signature decodes and lies in G2, and  prod_i e(pk_i, H(m_i)) * e(-g1, S) == 1: n + 1 Miller loops and ONE final
+ * exponentiation per set.  Not affected by b2_set_verify_mode (always the exact per-set equation). */
+int b2_aggregate_verify_pks(b2_ctx* ctx, const uint8_t* pk48, const uint8_t* msg32, const uint32_t* pair_off, const uint8_t* sig96,
+                            uint32_t n_sets, uint8_t* ok_out);
+/* the same with the signers taken from the registry by index (keys validated once at b2_registry_load); a signer index
+ * >= n_validators is B2_EINVAL */
+int b2_aggregate_verify(b2_ctx* ctx, const uint32_t* signer, const uint8_t* msg32, const uint32_t* pair_off, const uint8_t* sig96,
+                        uint32_t n_sets, uint8_t* ok_out);
+/* bls.AggregatePKs (py_ecc _AggregatePKs), batched: segment s = pk48[off[s] .. off[s+1]) -> compressed sum (the infinity encoding
+ * when the keys cancel); status = B2_PK_* bits of b2_g1_aggregate (B2_PK_INVALID_KEY, B2_PK_EMPTY; B2_PK_INFINITY alone is a valid result) */
+int b2_aggregate_pks(b2_ctx* ctx, const uint8_t* pk48, const uint32_t* off, uint32_t n_seg, uint8_t* out48, uint8_t* status);
+
 /* bls.SkToPk / bls.Sign, batched (sk = 8 little-endian u32 limbs, 0 < sk < r).  Signature i = sk[i] * H(msg[msg_idx[i]]). */
 int b2_sk_to_pk(b2_ctx* ctx, const uint32_t* sk8, uint64_t n, uint8_t* pk48_out);
 int b2_sign(b2_ctx* ctx, const uint32_t* sk8, const uint32_t* msg_idx, uint64_t n, const uint8_t* msg32, uint32_t n_msg,
@@ -190,6 +204,11 @@ int b2_aggregate_dev(b2_ctx* ctx, const uint8_t* d_sig96, const uint32_t* d_seg_
 int b2_fast_aggregate_verify_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_off, const uint8_t* d_bits,
                                  uint32_t bits_stride, const uint8_t* d_msg32, const uint8_t* d_sig96, uint32_t n_agg,
                                  uint8_t* d_ok_out, void* stream);
+/* b2_aggregate_verify on device arrays: d_signer / d_msg32 hold n_pairs entries.  A signer index >= n_validators fails only its own set
+ * (B2_GUARD_BAD_INDEX).  Malformed offsets -- d_pair_off[0] != 0, a decreasing pair, or d_pair_off[n_sets] > n_pairs -- fail EVERY set
+ * of the call (the item -> set mapping needs monotone offsets) and set B2_GUARD_BAD_ROW; nothing is read out of bounds either way. */
+int b2_aggregate_verify_dev(b2_ctx* ctx, const uint32_t* d_signer, const uint8_t* d_msg32, const uint32_t* d_pair_off, uint64_t n_pairs,
+                            const uint8_t* d_sig96, uint32_t n_sets, uint8_t* d_ok_out, void* stream);
 /* The gather stage of K2 alone, for measurement (north_star: ">= 60 % of HBM-read roofline on the pubkey gather"): for every aggregate
  * the XOR of the 24 record words of each selected member's pubkey record (get_attesting_indices + the pubkey list of
  * is_valid_indexed_attestation, pos-evolution.md:736/:745, without the additions).  form 1 = TMA-staged (cp.async.bulk -> shared

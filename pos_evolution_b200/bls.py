@@ -3,7 +3,8 @@
 Same names, argument meaning and error behaviour as the module the reference calls
 (pos-evolution.md:165 ``bls.Verify``; BASELINE.json names ``bls.Aggregate`` and
 ``bls.FastAggregateVerify``): verification functions never raise and return False for any
-malformed input; ``Aggregate`` raises ValueError on an empty list or an undecodable signature.
+malformed input; ``Aggregate`` raises ValueError on an empty list or an undecodable signature, ``AggregatePKs`` on an empty list or
+a key that fails KeyValidate.
 Every call goes through the C ABI (include/b200pos.h) to hand-written sm_90a kernels; there is
 no CPU path.  These per-call functions move a few hundred bytes over PCIe each -- for throughput
 use the batch API (pos_evolution_b200.engine.Engine / spec.EpochProcessor).
@@ -72,6 +73,45 @@ def FastAggregateVerify(pubkeys: Sequence[bytes], message: bytes, signature: byt
 
 def Verify(PK: bytes, message: bytes, signature: bytes) -> bool:
     return FastAggregateVerify([PK], message, signature)
+
+
+def AggregateVerify(pubkeys: Sequence[bytes], messages: Sequence[bytes], signature: bytes) -> bool:
+    """One signature over (pubkeys[i], messages[i]) pairs; messages need not be distinct (proof-of-possession scheme)."""
+    try:
+        msgs = list(messages)
+    except TypeError:
+        return False
+    ms = [_msg(m) for m in msgs]
+    try:
+        pks = [bytes(p) for p in pubkeys]
+        sig = bytes(signature)
+        if len(pks) < 1 or len(pks) != len(ms) or len(sig) != 96 or any(len(p) != 48 for p in pks):
+            return False
+        ok = engine().aggregate_verify_pks(np.frombuffer(b"".join(pks), dtype=np.uint8), [0, len(pks)],
+                                           np.frombuffer(b"".join(ms), dtype=np.uint8), np.frombuffer(sig, dtype=np.uint8))
+        return bool(ok[0])
+    except (TypeError, ValueError):
+        return False
+
+
+B2_PK_INVALID_KEY, B2_PK_EMPTY = 1, 2
+
+
+def AggregatePKs(pubkeys: Sequence[bytes]) -> bytes:
+    """Sum of the keys, compressed (the infinity encoding when they cancel); ValueError on an empty list or a key that fails
+    KeyValidate."""
+    pks = [bytes(p) for p in pubkeys]
+    if len(pks) < 1:
+        raise ValueError("AggregatePKs: empty list")
+    if any(len(p) != 48 for p in pks):
+        raise ValueError("AggregatePKs: key is not 48 bytes")
+    out, status = engine().aggregate_pks(np.frombuffer(b"".join(pks), dtype=np.uint8), [0, len(pks)])
+    if status[0] & (B2_PK_INVALID_KEY | B2_PK_EMPTY):
+        raise ValueError("AggregatePKs: invalid key")
+    return bytes(out[0])
+
+
+_AggregatePKs = AggregatePKs          # the name pyspec's wrapper calls on its backend
 
 
 def KeyValidate(pubkey: bytes) -> bool:

@@ -14,6 +14,7 @@
 #include "kernels.cuh"
 #include "gather.cuh"
 #include "rlc.cuh"
+#include "aggverify.cuh"
 
 using namespace b2;
 
@@ -142,6 +143,11 @@ struct b2_ctx {
     tree_tables tree;
     // scratch
     dbuf sc_pkjac, sc_pkst, sc_haff, sc_hflag, sc_g2aff, sc_g2st, sc_rec, sc_val, sc_shuf, sc_pivot;
+    // bls.AggregateVerify: signature points / flags, partial products and status words of the (block, set) runs, offsets-malformed
+    // word; and its own side streams and events, so that it never re-records an event an epoch in flight waits on
+    dbuf sc_av_saff, sc_av_sflag, sc_av_f, sc_av_st, sc_av_bad;
+    cudaStream_t s_av[2] = {nullptr, nullptr};
+    cudaEvent_t ev_av[3] = {nullptr, nullptr, nullptr};
     std::vector<dbuf> stage;                          // the synchronous entry points' host inputs and outputs (struct staging)
 };
 
@@ -288,6 +294,8 @@ int b2_init(int device, b2_ctx** out) {
         e = cudaStreamCreateWithPriority(&ctx->slot[i].s_tail, cudaStreamNonBlocking, prio_hi);
         for (int k = 0; k < 2 && e == cudaSuccess; k++) e = cudaStreamCreateWithPriority(&ctx->slot[i].s_aux[k], cudaStreamNonBlocking, prio_hi);
     }
+    for (int k = 0; k < 2 && e == cudaSuccess; k++) e = cudaStreamCreateWithPriority(&ctx->s_av[k], cudaStreamNonBlocking, prio_hi);
+    for (int k = 0; k < 3 && e == cudaSuccess; k++) e = cudaEventCreateWithFlags(&ctx->ev_av[k], cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_lmd_done, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_votes_done, cudaEventDisableTiming);
     for (int i = 0; i < B2_EPOCH_SLOTS && e == cudaSuccess; i++) {
@@ -352,6 +360,10 @@ void b2_destroy(b2_ctx* ctx) {
     if (ctx->s_main) cudaStreamDestroy(ctx->s_main);
     for (int i = 0; i < 4; i++)
         if (ctx->s_dec[i]) cudaStreamDestroy(ctx->s_dec[i]);
+    for (int k = 0; k < 2; k++)
+        if (ctx->s_av[k]) cudaStreamDestroy(ctx->s_av[k]);
+    for (int k = 0; k < 3; k++)
+        if (ctx->ev_av[k]) cudaEventDestroy(ctx->ev_av[k]);
     if (ctx->ev_lmd_done) cudaEventDestroy(ctx->ev_lmd_done);
     if (ctx->ev_votes_done) cudaEventDestroy(ctx->ev_votes_done);
     if (ctx->h_head) cudaFreeHost((void*)ctx->h_head);
@@ -857,6 +869,136 @@ int b2_fast_aggregate_verify_pks(b2_ctx* ctx, const uint8_t* pk48, const uint32_
     uint8_t* dok = st.out(ok_out, n_agg);
     pk_source P = {nullptr, dof, nullptr, 0, dpk, n_pk};
     if ((rc = st.rc) || (rc = verify_fork(ctx, ctx->slot[0], P, dmsg, n_agg, s)) || (rc = verify_main(ctx, ctx->slot[0], dsig, n_agg, dok, s))) return rc;
+    return st.finish();
+}
+
+// ------------------------------------------------------------------------------------------ AggregateVerify / AggregatePKs
+// Keys by registry index (d_signer) or explicit (d_pk48, decoded + KeyValidated here).  Hashing and key decoding fork onto the
+// context's AggregateVerify side streams; signature preparation, the per-item Miller loops and the per-set final exponentiations
+// run on `s`.  The grid covers n_pairs + n_sets items whatever the offsets say; k_av_check makes the kernels that follow skip the
+// whole batch when the offsets are malformed.
+static int aggregate_verify_enqueue(b2_ctx* ctx, const uint32_t* d_signer, const uint8_t* d_pk48, const uint8_t* d_msg32, const uint32_t* d_pair_off,
+                                    uint64_t n_pairs, const uint8_t* d_sig96, uint32_t n_sets, uint8_t* d_ok, cudaStream_t s) {
+    const unsigned n_blocks = blocks_for(n_pairs + n_sets, B2_AV_BLOCK);
+    const size_t n_slots = (size_t)n_sets + n_blocks;
+    int rc;
+    if ((rc = ensure(ctx, ctx->sc_haff, n_pairs * 192 + 16)) || (rc = ensure(ctx, ctx->sc_hflag, n_pairs + 16)) ||
+        (rc = ensure(ctx, ctx->sc_av_saff, (size_t)n_sets * 192)) || (rc = ensure(ctx, ctx->sc_av_sflag, n_sets)) ||
+        (rc = ensure(ctx, ctx->sc_av_f, n_slots * 576)) || (rc = ensure(ctx, ctx->sc_av_st, n_slots * 4)) || (rc = ensure(ctx, ctx->sc_av_bad, 4)))
+        return rc;
+    if (d_pk48 && ((rc = ensure(ctx, ctx->sc_rec, n_pairs * 96 + 16)) || (rc = ensure(ctx, ctx->sc_val, n_pairs + 16)))) return rc;
+    uint32_t* bad_row = ctx->sc_av_bad;
+    CK(cudaMemsetAsync(bad_row, 0, 4, s));
+    k_av_check<<<blocks_for(n_sets, 128), 128, 0, s>>>(d_pair_off, n_sets, n_pairs, bad_row, ctx->d_guard);
+    CKL(ctx);
+    if (n_pairs) {
+        CK(cudaEventRecord(ctx->ev_av[0], s));
+        CK(cudaStreamWaitEvent(ctx->s_av[0], ctx->ev_av[0], 0));
+        k_hash_to_g2<<<blocks_for(2 * n_pairs, 32), 32, 0, ctx->s_av[0]>>>(d_msg32, (uint32_t)n_pairs, ctx->sc_haff, ctx->sc_hflag);
+        CKL(ctx);
+        CK(cudaEventRecord(ctx->ev_av[1], ctx->s_av[0]));
+        if (d_pk48) {
+            CK(cudaStreamWaitEvent(ctx->s_av[1], ctx->ev_av[0], 0));
+            k_g1_decompress_validate<<<blocks_for(n_pairs, 128), 128, 0, ctx->s_av[1]>>>(d_pk48, n_pairs, ctx->sc_rec, ctx->sc_val);
+            CKL(ctx);
+            CK(cudaEventRecord(ctx->ev_av[2], ctx->s_av[1]));
+        }
+    }
+    k_sig_prepare<<<blocks_for(n_sets, 32), 32, 0, s>>>(d_sig96, n_sets, ctx->sc_av_saff, ctx->sc_av_sflag);
+    CKL(ctx);
+    if (n_pairs) {
+        CK(cudaStreamWaitEvent(s, ctx->ev_av[1], 0));
+        if (d_pk48) CK(cudaStreamWaitEvent(s, ctx->ev_av[2], 0));
+    }
+    const uint32_t* records = d_pk48 ? (const uint32_t*)ctx->sc_rec : (const uint32_t*)ctx->reg.records;
+    const uint8_t* valid = d_pk48 ? (const uint8_t*)ctx->sc_val : (const uint8_t*)ctx->reg.valid;
+    k_av_miller<<<n_blocks, B2_AV_BLOCK, 0, s>>>(d_pair_off, n_sets, d_signer, records, valid, d_pk48 ? n_pairs : ctx->n_val,
+                                                 ctx->sc_haff, ctx->sc_hflag, ctx->sc_av_saff, ctx->sc_av_sflag, bad_row, ctx->sc_av_f, ctx->sc_av_st,
+                                                 ctx->d_guard);
+    CKL(ctx);
+    k_av_final<<<blocks_for(n_sets, 32), 32, 0, s>>>(d_pair_off, n_sets, bad_row, ctx->sc_av_f, ctx->sc_av_st, d_ok);
+    CKL(ctx);
+    return B2_OK;
+}
+
+int b2_aggregate_verify_dev(b2_ctx* ctx, const uint32_t* d_signer, const uint8_t* d_msg32, const uint32_t* d_pair_off, uint64_t n_pairs, const uint8_t* d_sig96,
+                            uint32_t n_sets, uint8_t* d_ok_out, void* stream) {
+    B2_NVTX;
+    REQUIRE(ctx && d_pair_off && d_sig96 && d_ok_out && n_sets > 0 && (n_pairs == 0 || (d_signer && d_msg32)) && n_pairs + n_sets < (1ull << 32),
+            "aggregate_verify_dev: bad arguments");
+    REQUIRE(ctx->n_val > 0, "aggregate_verify: registry not loaded");
+    CK(cudaSetDevice(ctx->device));
+    return aggregate_verify_enqueue(ctx, d_signer, nullptr, d_msg32, d_pair_off, n_pairs, d_sig96, n_sets, d_ok_out, (cudaStream_t)stream);
+}
+
+int b2_aggregate_verify(b2_ctx* ctx, const uint32_t* signer, const uint8_t* msg32, const uint32_t* pair_off, const uint8_t* sig96, uint32_t n_sets,
+                        uint8_t* ok_out) {
+    B2_NVTX;
+    REQUIRE(ctx && pair_off && sig96 && ok_out && n_sets > 0, "aggregate_verify: bad arguments");
+    REQUIRE(ctx->n_val > 0, "aggregate_verify: registry not loaded");
+    int rc;
+    if ((rc = check_offsets(ctx, pair_off, n_sets, "aggregate_verify: pair_off"))) return rc;
+    const uint64_t n_pairs = pair_off[n_sets];
+    REQUIRE(n_pairs == 0 || (signer && msg32), "aggregate_verify: null signers or messages");
+    REQUIRE(n_pairs + n_sets < (1ull << 32), "aggregate_verify: too many pairs");
+    for (uint64_t i = 0; i < n_pairs; i++) REQUIRE(signer[i] < ctx->n_val, "aggregate_verify: signer index outside the registry");
+    CK(cudaSetDevice(ctx->device));
+    staging st(ctx);
+    const uint32_t* dsigner = st.in(signer, n_pairs, 4);
+    const uint8_t* dmsg = st.in(msg32, n_pairs * 32, 16);
+    const uint32_t* doff = st.in(pair_off, (size_t)n_sets + 1);
+    const uint8_t* dsig = st.in(sig96, (size_t)n_sets * 96);
+    uint8_t* dok = st.out(ok_out, n_sets);
+    if ((rc = st.rc) || (rc = aggregate_verify_enqueue(ctx, dsigner, nullptr, dmsg, doff, n_pairs, dsig, n_sets, dok, ctx->s_main))) return rc;
+    return st.finish();
+}
+
+int b2_aggregate_verify_pks(b2_ctx* ctx, const uint8_t* pk48, const uint8_t* msg32, const uint32_t* pair_off, const uint8_t* sig96, uint32_t n_sets,
+                            uint8_t* ok_out) {
+    B2_NVTX;
+    REQUIRE(ctx && pair_off && sig96 && ok_out && n_sets > 0, "aggregate_verify_pks: bad arguments");
+    int rc;
+    if ((rc = check_offsets(ctx, pair_off, n_sets, "aggregate_verify_pks: pair_off"))) return rc;
+    const uint64_t n_pairs = pair_off[n_sets];
+    REQUIRE(n_pairs == 0 || (pk48 && msg32), "aggregate_verify_pks: null pubkeys or messages");
+    REQUIRE(n_pairs + n_sets < (1ull << 32), "aggregate_verify_pks: too many pairs");
+    CK(cudaSetDevice(ctx->device));
+    staging st(ctx);
+    const uint8_t* dpk = st.in(pk48, n_pairs * 48, 16);
+    const uint8_t* dmsg = st.in(msg32, n_pairs * 32, 16);
+    const uint32_t* doff = st.in(pair_off, (size_t)n_sets + 1);
+    const uint8_t* dsig = st.in(sig96, (size_t)n_sets * 96);
+    uint8_t* dok = st.out(ok_out, n_sets);
+    if ((rc = st.rc) || (rc = aggregate_verify_enqueue(ctx, nullptr, dpk, dmsg, doff, n_pairs, dsig, n_sets, dok, ctx->s_main))) return rc;
+    return st.finish();
+}
+
+// py_ecc _AggregatePKs, batched: decode + KeyValidate every key, per-segment sums (the status bits of b2_g1_aggregate), compress
+int b2_aggregate_pks(b2_ctx* ctx, const uint8_t* pk48, const uint32_t* off, uint32_t n_seg, uint8_t* out48, uint8_t* status) {
+    B2_NVTX;
+    REQUIRE(ctx && off && out48 && status && n_seg > 0, "aggregate_pks: bad arguments");
+    int rc;
+    if ((rc = check_offsets(ctx, off, n_seg, "aggregate_pks: off"))) return rc;
+    const uint64_t n_pk = off[n_seg];
+    REQUIRE(n_pk == 0 || pk48, "aggregate_pks: null pubkeys");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = ctx->s_main;
+    staging st(ctx);
+    const uint8_t* dpk = st.in(pk48, n_pk * 48, 16);
+    const uint32_t* doff = st.in(off, (size_t)n_seg + 1);
+    uint8_t* d48 = st.out(out48, (size_t)n_seg * 48);
+    if ((rc = st.rc) || (rc = ensure(ctx, ctx->sc_rec, n_pk * 96 + 16)) || (rc = ensure(ctx, ctx->sc_val, n_pk + 16)) ||
+        (rc = ensure(ctx, ctx->sc_pkjac, (size_t)n_seg * 144)) || (rc = ensure(ctx, ctx->sc_pkst, n_seg)))
+        return rc;
+    if (n_pk) {
+        k_g1_decompress_validate<<<blocks_for(n_pk, 128), 128, 0, s>>>(dpk, n_pk, ctx->sc_rec, ctx->sc_val);
+        CKL(ctx);
+    }
+    k_g1_segment_sum<<<n_seg, 128, 0, s>>>(ctx->sc_rec, ctx->sc_val, doff, n_seg, ctx->sc_pkjac, ctx->sc_pkst);
+    CKL(ctx);
+    k_g1_compress<<<blocks_for(n_seg, 64), 64, 0, s>>>(ctx->sc_pkjac, n_seg, d48);
+    CKL(ctx);
+    st.out(status, ctx->sc_pkst, n_seg);
     return st.finish();
 }
 

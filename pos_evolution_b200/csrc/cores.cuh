@@ -163,6 +163,55 @@ HD uint8_t core_final_verdict(const fp12& f0, const fp12& f1, uint8_t pk_status,
     return fp12_is_one(final_exponentiation(fp12_mul(f0, f1))) ? 1 : 0;
 }
 
+// ---- bls.AggregateVerify, batched (kernels in aggverify.cuh).  Set s owns the items [pair_off[s] + s, pair_off[s+1] + s + 1): one per
+// (key, message) pair, then one for its signature.  Every item is one Miller loop; the set's product of them takes ONE final
+// exponentiation:  prod_i e(pk_i, H(m_i)) * e(-g1, S) == 1.  An item also yields the status bits that reject its set outright.
+enum AvStatus : uint32_t { AV_BAD_KEY = 1, AV_BAD_INDEX = 2 /* signer index outside the registry */, AV_BAD_SIG = 4 };
+// the set of item i: the last s whose first item pair_off[s] + s is <= i (first items strictly increase when pair_off is monotone)
+HD uint32_t av_set_of(const uint32_t* pair_off, uint32_t n_sets, uint32_t i) {
+    uint32_t lo = 0, hi = n_sets - 1;
+#pragma unroll 1
+    while (lo < hi) {
+        const uint32_t mid = lo + (hi - lo + 1) / 2;
+        if (pair_off[mid] + mid <= i) {
+            lo = mid;
+        } else {
+            hi = mid - 1;
+        }
+    }
+    return lo;
+}
+// The Miller-loop arguments of an item, so that pair and signature items of one warp share ONE call of miller_loop.
+// Pair item: (pk, H(m)) with pk = key record idx of a table of n_keys; an index outside the table or a key that failed KeyValidate
+// rejects the set and leaves P at infinity (the loop then returns 1 at once).
+HD void core_av_pair(const uint32_t* records, const uint8_t* valid, uint32_t idx, uint64_t n_keys, const g2_aff& h, uint8_t hflag, g1_jac& p,
+                     g2_aff& q, bool& q_inf, uint32_t& bad) {
+    q = h;
+    q_inf = hflag != 0;
+    p = pt_inf<fp>();
+    if (idx >= n_keys) {
+        bad |= AV_BAD_INDEX;
+    } else if (!valid[idx]) {
+        bad |= AV_BAD_KEY;
+    } else {
+        p = pt_from_affine(load_record(records, idx));
+    }
+}
+// Signature item: (-g1, S); an undecodable or non-G2 signature rejects the set
+HD void core_av_sig(const g2_aff& s, uint8_t sflag, g1_jac& p, g2_aff& q, bool& q_inf, uint32_t& bad) {
+    p.x = fp_load_const(C_G1X);
+    p.y = fp_load_const(C_G1Y_NEG);
+    p.z = fp_one();
+    q = s;
+    q_inf = sflag != SIG_OK;
+    if (sflag == SIG_INVALID) bad |= AV_BAD_SIG;
+}
+// F = the product of the set's Miller values, bad = the OR of its items' status bits
+HD uint8_t core_av_verdict(const fp12& F, uint32_t bad, bool nonempty) {
+    if (!nonempty || bad) return 0;
+    return fp12_is_one(final_exponentiation(F)) ? 1 : 0;
+}
+
 // ---- random-linear-combination batch verification (SURVEY.md section 8(f)-4, section 2 K6 "optional RLC batch mode")
 // Instead of n independent checks e(PK_i, H_i) * e(-g1, S_i) == 1, one check per group of aggregates:
 //     prod_i e([r_i] PK_i, H_i)  *  e(-g1, sum_i [r_i] S_i)  ==  1

@@ -126,6 +126,41 @@ class Engine:
         self._ck(self.lib.b2_fast_aggregate_verify_pks(self.h, _p(pks), _p(pk_off), _p(msgs), _p(sigs), n_agg, _p(ok)))
         return ok
 
+    def aggregate_verify_pks(self, pks48, pair_off, msgs32, sigs96):
+        """bls.AggregateVerify per set: set s = (pks48[i], msgs32[i]) for i in [pair_off[s], pair_off[s+1]), signature sigs96[s] -> uint8[n_sets]"""
+        pair_off = _c(pair_off, np.uint32)
+        n_sets = pair_off.shape[0] - 1
+        pks = _c(pks48, np.uint8).reshape(-1, 48)
+        msgs = _c(msgs32, np.uint8).reshape(-1, 32)
+        assert int(pair_off[-1]) == pks.shape[0] == msgs.shape[0]
+        sigs = _c(sigs96, np.uint8).reshape(n_sets, 96)
+        ok = np.zeros(n_sets, dtype=np.uint8)
+        self._ck(self.lib.b2_aggregate_verify_pks(self.h, _p(pks), _p(msgs), _p(pair_off), _p(sigs), n_sets, _p(ok)))
+        return ok
+
+    def aggregate_verify(self, signers, pair_off, msgs32, sigs96):
+        """bls.AggregateVerify with the keys taken from the registry: pair i is (registry key signers[i], msgs32[i])"""
+        pair_off = _c(pair_off, np.uint32)
+        n_sets = pair_off.shape[0] - 1
+        signers = _c(signers, np.uint32)
+        msgs = _c(msgs32, np.uint8).reshape(-1, 32)
+        assert int(pair_off[-1]) == signers.shape[0] == msgs.shape[0]
+        sigs = _c(sigs96, np.uint8).reshape(n_sets, 96)
+        ok = np.zeros(n_sets, dtype=np.uint8)
+        self._ck(self.lib.b2_aggregate_verify(self.h, _p(signers), _p(msgs), _p(pair_off), _p(sigs), n_sets, _p(ok)))
+        return ok
+
+    def aggregate_pks(self, pks48, off):
+        """bls.AggregatePKs per segment s = pks48[off[s] .. off[s+1]) -> (uint8[n_seg,48] compressed sums, uint8[n_seg] B2_PK_* status bits)"""
+        off = _c(off, np.uint32)
+        n_seg = off.shape[0] - 1
+        pks = _c(pks48, np.uint8).reshape(-1, 48)
+        assert int(off[-1]) == pks.shape[0]
+        out = np.zeros((n_seg, 48), dtype=np.uint8)
+        status = np.zeros(n_seg, dtype=np.uint8)
+        self._ck(self.lib.b2_aggregate_pks(self.h, _p(pks), _p(off), n_seg, _p(out), _p(status)))
+        return out, status
+
     @staticmethod
     def _sk_limbs(sks):
         out = np.zeros((len(sks), 8), dtype=np.uint32)
@@ -324,6 +359,12 @@ class Engine:
         stride = d_bits.shape[1]
         self._ck(self.lib.b2_fast_aggregate_verify_dev(self.h, d_members.data_ptr(), d_off.data_ptr(), d_bits.data_ptr(), stride,
                                                        d_msgs.data_ptr(), d_sigs.data_ptr(), n_agg, d_ok.data_ptr(), self._stream()))
+
+    def aggregate_verify_dev(self, d_signer, d_msgs, d_pair_off, d_sigs, d_ok):
+        """b2_aggregate_verify_dev: d_signer uint32[n_pairs], d_msgs uint8[n_pairs,32], d_pair_off uint32[n_sets+1], d_sigs uint8[n_sets,96]"""
+        n_sets = d_pair_off.numel() - 1
+        self._ck(self.lib.b2_aggregate_verify_dev(self.h, d_signer.data_ptr(), d_msgs.data_ptr(), d_pair_off.data_ptr(), d_signer.numel(),
+                                                  d_sigs.data_ptr(), n_sets, d_ok.data_ptr(), self._stream()))
 
     def latest_messages_update_dev(self, d_members, d_off, d_bits, d_target_epoch, d_block_idx, d_accept):
         n_agg = d_off.numel() - 1
