@@ -1,5 +1,6 @@
 // fp.cuh -- arithmetic in Fp (p = BLS12-381 base field, 381 bits), 12 x 32-bit limbs held in
-// registers, Montgomery form with R = 2^384, values always fully reduced to [0, p).
+// registers, Montgomery form with R = 2^384, values fully reduced to [0, p).  The one exception is the
+// inside of a fixed-exponent chain (fp_pow_prog_t), whose values stay in [0, 2p) (fp_mul_lazy / fp_sqr_lazy).
 //
 // This is kernel K1 of SURVEY.md section 2 (no counterpart in the reference: the reference
 // reaches field arithmetic only through its bls.* call sites, pos-evolution.md:165/:736/:976).
@@ -113,7 +114,7 @@ HD void mont_reduce_row(uint32_t* E, uint32_t* O) {
     mad_wide_cc(O[0], O[1], P_LIMB(1), m);
 #pragma unroll
     for (int k = 2; k < 12; k += 2) madc_wide_cc(O[k], O[k + 1], P_LIMB(k + 1), m);
-    // no carry out of O: the running total is < 2^416 (see header)
+    // no carry out of O: the running total is < 2^416 (see fp_mul_lazy)
     mad_wide_cc(E[0], E[1], P_LIMB(0), m);
 #pragma unroll
     for (int j = 2; j < 12; j += 2) madc_wide_cc(E[j], E[j + 1], P_LIMB(j), m);
@@ -134,7 +135,10 @@ HD void mont_mul_row(uint32_t* E, uint32_t* X, const uint32_t* a, uint32_t bi) {
     X[11] = addc(X[11], 0);
 }
 
-HD fp fp_mul(const fp& a, const fp& b) {
+// a*b/R mod p in [0, 2p) for a, b in [0, 2p), without the final subtraction.  With S the running value after a row and its
+// division by 2^32, S < a + p by induction (S' < (a + p + (a + p)(2^32 - 1)) / 2^32), so before the division a row holds
+// < 3p * 2^32 < 2^416: the 13 limbs of (ev, od) never carry out.  The result is (ab + Mp)/R < 4p^2/R + p < 1.5p (p < R/8).
+HD fp fp_mul_lazy(const fp& a, const fp& b) {
     uint32_t ev[12], od[12];
     const uint32_t b0 = b.l[0];
 #pragma unroll
@@ -158,26 +162,23 @@ HD fp fp_mul(const fp& a, const fp& b) {
 #pragma unroll
     for (int k = 1; k < 11; k++) r.l[k] = addc_cc(ev[k], od[k + 1]);
     r.l[11] = addc(ev[11], 0);
+    return r;
+}
+HD fp fp_mul(const fp& a, const fp& b) {
+    fp r = fp_mul_lazy(a, b);
     fp_final_sub(r.l);
     return r;
 }
 
 // Dedicated squaring (separated operand scanning): 66 off-diagonal + 12 diagonal wide products for the 768-bit
-// square, then a product-free Montgomery reduction of its low half (144 wide products) -- 222 IMAD.WIDE instead of
-// the 288 of fp_mul(a, a).  The extra carry bookkeeping is IADD3 work on the otherwise idle ALU pipe.
+// square, then a Montgomery reduction of the whole square in place (144 wide products) -- 222 IMAD.WIDE instead of
+// the 288 of fp_mul(a, a).
 //
 // Off-diagonal terms a_i*a_j (i < j) land on limbs (s, s+1), s = i+j.  For a fixed i the terms with j = i+1, i+3, ...
 // sit on consecutive ODD-aligned limb pairs and those with j = i+2, i+4, ... on consecutive EVEN-aligned pairs: each is
 // one carry chain, into the accumulator of its alignment (uo / ue, indexed by absolute limb).  Rows are processed in
 // increasing i; a chain's carry-out is absorbed by the limb just above it, which at that moment holds nothing but
 // earlier absorbed carries (every product that lands there belongs to a later row), so it cannot overflow.
-HD void mont_shift_row(uint32_t* E, uint32_t* X) {            // mont_mul_row without products: divide by 2^32
-    E[0] = add_cc(E[0], X[1]);
-#pragma unroll
-    for (int k = 0; k < 10; k++) X[k] = addc_cc(X[k + 2], 0u);
-    X[10] = addc(0u, 0u);
-    X[11] = 0u;
-}
 
 // 2N-limb square of an N-limb number (N even), separated operand scanning as described above: N(N-1)/2 + N wide products.
 template <int N>
@@ -267,34 +268,53 @@ HD void sqr_product(const uint32_t* a, uint32_t* t) {
 #endif
 }
 
-HD fp fp_sqr(const fp& a) {
-    uint32_t t[24];
+// Montgomery reduction of the 24-limb square in place (separated operand scanning, indexed by absolute limb): row i takes
+// m = t[i]*(-p^-1) and adds m*p at limb i as the two alignment chains of mont_reduce_row, the even-j products onto the limb pairs
+// that start at i's parity, the odd-j ones onto the pairs of the other parity.  Afterwards limb i is zero, so the division by
+// 2^32 is only the next row starting one limb higher.  A 64-bit IMAD.WIDE operand is an aligned register pair, so each
+// alignment keeps its own accumulator: A holds the pairs that start at even limbs, B those that start at odd limbs (one array
+// for both would put every limb in a low and a high half within one row, and ptxas then spends a MOV per product).  Row i first
+// folds limb i of the other accumulator into its own (the carry enters the odd-j chain, which starts at limb i+1).
+// Carries: the even-j chain carries out at limb i+12, the odd-j chain at limb i+13, each into the LOW limb of a pair of its
+// accumulator.  The high half of the square therefore sits on the HIGH limbs of the pairs only (odd limbs 13..23 in A, even
+// limbs 12..22 in B), so a carry never lands on product data: before row i, limb i+12 of its accumulator holds at most the
+// previous row's one-bit carry and limb i+13 nothing, and neither can overflow.
+// Bound: for a < 2p, a^2 + M*p < 4p^2 + R*p with M < R; as p < R/8 that is < R * 1.5p < R^2, so the carry out of limb 23
+// (last row) is zero, and (A + B)[12..23] = (a^2 + M*p)/R < 1.5p.  For a < p the result is < 1.125p.
+HD fp fp_sqr_lazy(const fp& a) {
+    uint32_t t[24], A[24], B[24];
     sqr_product(a.l, t);
-    // Montgomery-reduce the low half (result <= p), add the high half (< p/8): the sum is < 2p
-    uint32_t ev[12], od[12];
 #pragma unroll
-    for (int k = 0; k < 12; k++) {
-        ev[k] = t[k];
-        od[k] = 0u;
+    for (int k = 0; k < 24; k++) {
+        const bool in_b = k >= 12 && !(k & 1);
+        A[k] = in_b ? 0u : t[k];
+        B[k] = in_b ? t[k] : 0u;
     }
-    mont_reduce_row(ev, od);
 #pragma unroll
-    for (int i = 1; i < 12; i += 2) {
-        mont_shift_row(od, ev);
-        mont_reduce_row(od, ev);
-        if (i + 1 < 12) {
-            mont_shift_row(ev, od);
-            mont_reduce_row(ev, od);
-        }
+    for (int i = 0; i < 12; i++) {
+        uint32_t* X = (i & 1) ? B : A;          // pairs (i, i+1), (i+2, i+3), ...
+        uint32_t* Y = (i & 1) ? A : B;          // pairs (i+1, i+2), ...
+        if (i > 0) X[i] = add_cc(X[i], Y[i]);
+        const uint32_t m = X[i] * B2_MONT_INV;
+        if (i > 0) madc_wide_cc(Y[i + 1], Y[i + 2], P_LIMB(1), m);
+        else mad_wide_cc(Y[i + 1], Y[i + 2], P_LIMB(1), m);
+#pragma unroll
+        for (int j = 3; j < 12; j += 2) madc_wide_cc(Y[i + j], Y[i + j + 1], P_LIMB(j), m);
+        if (i + 13 < 24) Y[i + 13] = addc(Y[i + 13], 0u);
+        mad_wide_cc(X[i], X[i + 1], P_LIMB(0), m);
+#pragma unroll
+        for (int j = 2; j < 12; j += 2) madc_wide_cc(X[i + j], X[i + j + 1], P_LIMB(j), m);
+        X[i + 12] = addc(X[i + 12], 0u);
     }
     fp r;
-    r.l[0] = add_cc(ev[0], od[1]);
+    r.l[0] = add_cc(A[12], B[12]);
 #pragma unroll
-    for (int k = 1; k < 11; k++) r.l[k] = addc_cc(ev[k], od[k + 1]);
-    r.l[11] = addc(ev[11], 0u);
-    r.l[0] = add_cc(r.l[0], t[12]);
-#pragma unroll
-    for (int k = 1; k < 12; k++) r.l[k] = addc_cc(r.l[k], t[12 + k]);
+    for (int k = 1; k < 11; k++) r.l[k] = addc_cc(A[12 + k], B[12 + k]);
+    r.l[11] = addc(A[23], B[23]);
+    return r;
+}
+HD fp fp_sqr(const fp& a) {
+    fp r = fp_sqr_lazy(a);
     fp_final_sub(r.l);
     return r;
 }
@@ -328,14 +348,16 @@ struct pow_tbl_local {
     HD void set(int i, const fp& v) { t[i] = v; }
     HD fp get(uint32_t i) const { return t[i]; }
 };
+// Inside the chain nothing is compared or encoded, so the table and every step stay in [0, 2p) (the lazy forms take and return
+// values there); only the result is reduced.  `a` may itself lie anywhere in [0, 2p).
 template <class TBL> HDN fp fp_pow_prog_t(const fp& a, int off, TBL& tbl) {
     const uint32_t* prog = const_table() + off;
-    fp a2 = fp_sqr(a);
+    fp a2 = fp_sqr_lazy(a);
     fp cur = a;
     tbl.set(0, cur);
 #pragma unroll 1
     for (int i = 1; i < 8; i++) {
-        cur = fp_mul(cur, a2);
+        cur = fp_mul_lazy(cur, a2);
         tbl.set(i, cur);
     }
     // entry 8 = a^255 = (a^15)^16 * a^15: the run token of tools/gen_consts.py:token_program (one multiplication per EIGHT
@@ -343,8 +365,8 @@ template <class TBL> HDN fp fp_pow_prog_t(const fp& a, int off, TBL& tbl) {
     {
         fp t = cur;
 #pragma unroll 1
-        for (int i = 0; i < 4; i++) t = fp_sqr(t);
-        tbl.set(8, fp_mul(t, cur));
+        for (int i = 0; i < 4; i++) t = fp_sqr_lazy(t);
+        tbl.set(8, fp_mul_lazy(t, cur));
     }
     const uint32_t n = prog[0];
     fp r = tbl.get(prog[1] & 0xffu);
@@ -352,10 +374,11 @@ template <class TBL> HDN fp fp_pow_prog_t(const fp& a, int off, TBL& tbl) {
     for (uint32_t k = 2; k <= n; k++) {
         const uint32_t op = prog[k];
 #pragma unroll 1
-        for (uint32_t s = op >> 8; s; s--) r = fp_sqr(r);
+        for (uint32_t s = op >> 8; s; s--) r = fp_sqr_lazy(r);
         const uint32_t idx = op & 0xffu;
-        if (idx != 0xffu) r = fp_mul(r, tbl.get(idx));
+        if (idx != 0xffu) r = fp_mul_lazy(r, tbl.get(idx));
     }
+    fp_final_sub(r.l);
     return r;
 }
 HD fp fp_pow_prog(const fp& a, int off) {

@@ -40,8 +40,10 @@ DEV uint32_t madc_hi_cc(uint32_t a, uint32_t b, uint32_t c) { uint32_t r; asm vo
 DEV uint32_t madc_hi(uint32_t a, uint32_t b, uint32_t c) { uint32_t r; asm volatile("madc.hi.u32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(c)); return r; }
 // 64-bit-wide multiply-accumulate steps.  The lo/hi halves MUST sit in one asm statement: ptxas only
 // fuses adjacent mad.lo.cc + madc.hi.cc into a single IMAD.WIDE.U32(.X) (checked with cuobjdump).
+// The plain product is one mul.wide.u32 into a 64-bit register, which is one IMAD.WIDE.U32 by definition; a mul.lo / mul.hi
+// pair is one only when ptxas pairs the two (CUDA 12.9 does; otherwise it is an IMAD plus an IMAD.HI.U32, 6 pipe cycles, not 4).
 DEV void mul_wide(uint32_t& lo, uint32_t& hi, uint32_t a, uint32_t b) {
-    asm volatile("mul.lo.u32 %0, %2, %3; mul.hi.u32 %1, %2, %3;" : "=r"(lo), "=r"(hi) : "r"(a), "r"(b));
+    asm("{ .reg .b64 t; mul.wide.u32 t, %2, %3; mov.b64 {%0, %1}, t; }" : "=r"(lo), "=r"(hi) : "r"(a), "r"(b));
 }
 DEV void mad_wide_cc(uint32_t& lo, uint32_t& hi, uint32_t a, uint32_t b) {          // (hi:lo) += a*b ; CF out
     asm volatile("mad.lo.cc.u32 %0, %2, %3, %0; madc.hi.cc.u32 %1, %2, %3, %1;" : "+r"(lo), "+r"(hi) : "r"(a), "r"(b));
