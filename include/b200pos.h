@@ -97,6 +97,23 @@ int b2_aggregate_verify(b2_ctx* ctx, const uint32_t* signer, const uint8_t* msg3
  * when the keys cancel); status = B2_PK_* bits of b2_g1_aggregate (B2_PK_INVALID_KEY, B2_PK_EMPTY; B2_PK_INFINITY alone is a valid result) */
 int b2_aggregate_pks(b2_ctx* ctx, const uint8_t* pk48, const uint32_t* off, uint32_t n_seg, uint8_t* out48, uint8_t* status);
 
+/* ---- sync committees (pos-evolution.md:371-372, :540-590; Altair process_sync_aggregate): n_committees tables of committee_size keys
+ * (1 <= committee_size <= 1024), pk48 = committee after committee.  Decodes + KeyValidates every key and sums each committee's valid
+ * keys ONCE; valid_out (may be NULL): 1 = KeyValidate passed, per key.  Replaces the previously loaded committees only on success. */
+int b2_sync_committee_load(b2_ctx* ctx, const uint8_t* pk48, uint32_t committee_size, uint32_t n_committees, uint8_t* valid_out);
+/* eth_fast_aggregate_verify (Altair bls helper) of block i: participants = the keys of committee committee_idx[i] whose bit is set in
+ * bits[i * ceil(committee_size/8) ...] (SSZ Bitvector order; bits past committee_size are ignored); msg32 = signing root.  ok_out[i] in
+ * {0,1}: FastAggregateVerify over the participants' keys, except that no participant accepts exactly the G2 infinity signature
+ * (0xc0 then 95 zero bytes).  The aggregate key is the sum of the participants or the committee sum minus the non-participants,
+ * whichever needs fewer additions.  pk48_out (may be NULL): the compressed sum of the participants' valid keys per block.
+ * Needs no registry; a committee index >= n_committees, or no loaded committee, is B2_EINVAL.  b2_set_verify_mode applies. */
+int b2_sync_aggregate_verify(b2_ctx* ctx, const uint32_t* committee_idx, const uint8_t* bits, const uint8_t* msg32, const uint8_t* sig96,
+                             uint32_t n, uint8_t* ok_out, uint8_t* pk48_out);
+/* the same on device arrays (asynchronous on `stream`): a committee index >= n_committees fails only its own block and sets
+ * B2_GUARD_BAD_INDEX */
+int b2_sync_aggregate_verify_dev(b2_ctx* ctx, const uint32_t* d_committee_idx, const uint8_t* d_bits, const uint8_t* d_msg32,
+                                 const uint8_t* d_sig96, uint32_t n, uint8_t* d_ok_out, uint8_t* d_pk48_out, void* stream);
+
 /* bls.SkToPk / bls.Sign, batched (sk = 8 little-endian u32 limbs, 0 < sk < r).  Signature i = sk[i] * H(msg[msg_idx[i]]). */
 int b2_sk_to_pk(b2_ctx* ctx, const uint32_t* sk8, uint64_t n, uint8_t* pk48_out);
 int b2_sign(b2_ctx* ctx, const uint32_t* sk8, const uint32_t* msg_idx, uint64_t n, const uint8_t* msg32, uint32_t n_msg,

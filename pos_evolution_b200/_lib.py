@@ -40,6 +40,9 @@ SIGNATURES = {
     "b2_aggregate_verify": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p]),
     "b2_aggregate_verify_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p]),
     "b2_aggregate_pks": (c_int, [c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p]),
+    "b2_sync_committee_load": (c_int, [c_void_p, c_void_p, c_uint32, c_uint32, c_void_p]),
+    "b2_sync_aggregate_verify": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p]),
+    "b2_sync_aggregate_verify_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p]),
     "b2_sk_to_pk": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p]),
     "b2_sign": (c_int, [c_void_p, c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p]),
     "b2_hash_to_g2": (c_int, [c_void_p, c_void_p, c_uint32, c_void_p]),

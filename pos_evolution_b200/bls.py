@@ -4,7 +4,8 @@ Same names, argument meaning and error behaviour as the module the reference cal
 (pos-evolution.md:165 ``bls.Verify``; BASELINE.json names ``bls.Aggregate`` and
 ``bls.FastAggregateVerify``): verification functions never raise and return False for any
 malformed input; ``Aggregate`` raises ValueError on an empty list or an undecodable signature, ``AggregatePKs`` on an empty list or
-a key that fails KeyValidate.
+a key that fails KeyValidate.  The Altair helpers ``eth_fast_aggregate_verify`` and ``eth_aggregate_pubkeys`` (what
+process_sync_aggregate calls) are here too; the second raises AssertionError, as upstream.
 Every call goes through the C ABI (include/b200pos.h) to hand-written sm_90a kernels; there is
 no CPU path.  These per-call functions move a few hundred bytes over PCIe each -- for throughput
 use the batch API (pos_evolution_b200.engine.Engine / spec.EpochProcessor).
@@ -138,3 +139,27 @@ def Aggregate(signatures: Sequence[bytes]) -> bytes:
 def AggregateBatch(signatures96: np.ndarray, seg_off):
     """Batched bls.Aggregate: segment s = rows [seg_off[s], seg_off[s+1]).  -> (uint8[n_seg,96], int32[n_seg] status)."""
     return engine().aggregate(signatures96, seg_off)
+
+
+# ---- Altair bls helpers (restated from the upstream consensus specs, specs/altair/bls.md; not part of the reference's text)
+G2_POINT_AT_INFINITY = bytes([0xC0]) + bytes(95)
+
+
+def eth_aggregate_pubkeys(pubkeys: Sequence[bytes]) -> bytes:
+    """Sum of the keys, compressed; AssertionError on an empty list or a key that fails KeyValidate."""
+    pks = [bytes(p) for p in pubkeys]
+    assert len(pks) > 0, "eth_aggregate_pubkeys: empty list"
+    assert all(len(p) == 48 for p in pks), "eth_aggregate_pubkeys: key is not 48 bytes"
+    out, status = engine().aggregate_pks(np.frombuffer(b"".join(pks), dtype=np.uint8), [0, len(pks)])
+    assert not status[0] & (B2_PK_INVALID_KEY | B2_PK_EMPTY), "eth_aggregate_pubkeys: invalid key"
+    return bytes(out[0])
+
+
+def eth_fast_aggregate_verify(pubkeys: Sequence[bytes], message: bytes, signature: bytes) -> bool:
+    """FastAggregateVerify, except that an empty key list verifies exactly the G2 infinity signature."""
+    try:
+        if len(pubkeys) == 0 and bytes(signature) == G2_POINT_AT_INFINITY:
+            return True
+    except TypeError:
+        return False
+    return FastAggregateVerify(pubkeys, message, signature)

@@ -15,6 +15,7 @@
 #include "gather.cuh"
 #include "rlc.cuh"
 #include "aggverify.cuh"
+#include "syncagg.cuh"
 
 using namespace b2;
 
@@ -71,6 +72,13 @@ struct tree_tables {
     dbuf packed;                                      // shared-memory form: u32 size | rank << 15 | keep << 31
     dbuf size_keep, rank, next;                       // generic form: u32 size | keep << 31, u32 root rank, u32[n+1] marks
     dbuf prefix, w2;                                  // generic form: u64[n+1] prefix sums, u64 weights
+};
+
+// sync committees (b2_sync_committee_load): n committees of `size` keys, replaced together
+struct sync_tables {
+    dbuf records, valid;       // u32[24] affine record and u8 KeyValidate per position, committee after committee
+    dbuf sum, sum_status;      // per committee: Jacobian sum of its valid keys (u32[36]), k_g1_segment_sum's status byte
+    uint32_t size = 0, n = 0;
 };
 
 struct vslot {
@@ -149,6 +157,7 @@ struct b2_ctx {
     cudaStream_t s_av[2] = {nullptr, nullptr};
     cudaEvent_t ev_av[3] = {nullptr, nullptr, nullptr};
     std::vector<dbuf> stage;                          // the synchronous entry points' host inputs and outputs (struct staging)
+    sync_tables sync;
 };
 
 struct nvtx_scope {
@@ -598,6 +607,8 @@ struct pk_source {
     uint32_t bits_stride;
     const uint8_t* d_pk48;      // explicit-key form when non-null (d_off = pk offsets)
     uint64_t n_pk;
+    const uint32_t* d_committee;      // sync-committee form when non-null: block i = committee d_committee[i] of ctx->sync, bit row d_bits + i * ceil(size / 8)
+    uint8_t* d_pk48_out;              // sync-committee form: compressed aggregate key per block (may be null)
 };
 // Two forms of K5/K6.  `team`: three lanes per pairing -- shortest critical path, used when the caller waits for the result
 // (synchronous entry points).  Thread-per-item: 2.7x longer, but ~40 % fewer warp instructions in total -- used by the pipelined
@@ -650,6 +661,15 @@ static int verify_fork(b2_ctx* ctx, vslot& V, const pk_source& P, const uint8_t*
         k_g1_segment_sum<<<n_agg, 128, 0, V.s_aux[1]>>>((const uint32_t*)ctx->sc_rec.p, (const uint8_t*)ctx->sc_val.p, P.d_off, n_agg,
                                                           (uint32_t*)V.pkjac.p, (uint8_t*)V.pkst.p);
         CKL(ctx);
+    } else if (P.d_committee) {
+        const sync_tables& T = ctx->sync;
+        k_sync_aggregate_pk<<<blocks_for(n_agg, B2_SYNC_WARPS), 32 * B2_SYNC_WARPS, 0, V.s_aux[1]>>>(T.records, T.valid, T.sum, T.size, T.n, P.d_committee,
+                                                                                                    P.d_bits, n_agg, V.pkjac, V.pkst, ctx->d_guard);
+        CKL(ctx);
+        if (P.d_pk48_out) {
+            k_g1_compress<<<blocks_for(n_agg, 64), 64, 0, V.s_aux[1]>>>(V.pkjac, n_agg, P.d_pk48_out);
+            CKL(ctx);
+        }
     } else {
         // one block per aggregate.  128 threads when the caller waits; ONE WARP under the epoch pipeline: the 5-round shuffle tree costs
         // every warp 80 Fp multiplications whatever its share of the 512 records, so 4 warps spend 2.1x the multiply-pipe time of one
@@ -999,6 +1019,78 @@ int b2_aggregate_pks(b2_ctx* ctx, const uint8_t* pk48, const uint32_t* off, uint
     k_g1_compress<<<blocks_for(n_seg, 64), 64, 0, s>>>(ctx->sc_pkjac, n_seg, d48);
     CKL(ctx);
     st.out(status, ctx->sc_pkst, n_seg);
+    return st.finish();
+}
+
+// ------------------------------------------------------------------------------------------ sync committees (syncagg.cuh)
+// Decode + KeyValidate every key and sum each committee's valid keys, into tables built aside: the loaded committees are replaced
+// only once the new ones are complete.
+int b2_sync_committee_load(b2_ctx* ctx, const uint8_t* pk48, uint32_t committee_size, uint32_t n_committees, uint8_t* valid_out) {
+    B2_NVTX;
+    REQUIRE(ctx && pk48 && committee_size > 0 && n_committees > 0, "sync_committee_load: bad arguments");
+    REQUIRE(committee_size <= B2_SYNC_MAX_SIZE, "sync_committee_load: committee_size above the kernel's limit (1024)");
+    const uint64_t n_pk = (uint64_t)committee_size * n_committees;
+    REQUIRE(n_pk < (1ull << 32), "sync_committee_load: too many keys");
+    CK(cudaSetDevice(ctx->device));
+    sync_tables t;
+    int rc;
+    if ((rc = ensure(ctx, t.records, n_pk * 96)) || (rc = ensure(ctx, t.valid, n_pk)) || (rc = ensure(ctx, t.sum, (size_t)n_committees * 144)) ||
+        (rc = ensure(ctx, t.sum_status, n_committees)))
+        return rc;
+    std::vector<uint32_t> off(n_committees + 1);
+    for (uint32_t c = 0; c <= n_committees; c++) off[c] = c * committee_size;
+    staging st(ctx);
+    const uint8_t* dpk = st.in(pk48, n_pk * 48);
+    const uint32_t* doff = st.in(off.data(), off.size());
+    if (st.rc) return st.rc;
+    cudaStream_t s = ctx->s_main;
+    k_g1_decompress_validate<<<blocks_for(n_pk, 128), 128, 0, s>>>(dpk, n_pk, t.records, t.valid);
+    CKL(ctx);
+    k_g1_segment_sum<<<n_committees, 128, 0, s>>>(t.records, t.valid, doff, n_committees, t.sum, t.sum_status);
+    CKL(ctx);
+    if (valid_out) st.out(valid_out, t.valid, n_pk);
+    if ((rc = st.finish())) return rc;
+    t.size = committee_size;
+    t.n = n_committees;
+    ctx->sync = std::move(t);
+    return B2_OK;
+}
+
+// eth_fast_aggregate_verify per block: the committee form of verify_fork (k_sync_aggregate_pk), the unchanged pairing half, then the
+// empty-participation rule on the verdicts
+int b2_sync_aggregate_verify_dev(b2_ctx* ctx, const uint32_t* d_committee_idx, const uint8_t* d_bits, const uint8_t* d_msg32, const uint8_t* d_sig96,
+                                 uint32_t n, uint8_t* d_ok_out, uint8_t* d_pk48_out, void* stream) {
+    B2_NVTX;
+    REQUIRE(ctx && d_committee_idx && d_bits && d_msg32 && d_sig96 && d_ok_out && n > 0, "sync_aggregate_verify_dev: bad arguments");
+    REQUIRE(ctx->sync.n > 0, "sync_aggregate_verify: no sync committee loaded");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    vslot& V = ctx->slot[0];
+    int rc;
+    pk_source P = {nullptr, nullptr, d_bits, 0, nullptr, 0, d_committee_idx, d_pk48_out};
+    if ((rc = verify_fork(ctx, V, P, d_msg32, n, s)) || (rc = verify_main(ctx, V, d_sig96, n, d_ok_out, s))) return rc;
+    k_sync_empty_verdict<<<blocks_for(n, 128), 128, 0, s>>>(V.pkst, d_sig96, n, d_ok_out);
+    CKL(ctx);
+    return B2_OK;
+}
+
+int b2_sync_aggregate_verify(b2_ctx* ctx, const uint32_t* committee_idx, const uint8_t* bits, const uint8_t* msg32, const uint8_t* sig96, uint32_t n,
+                             uint8_t* ok_out, uint8_t* pk48_out) {
+    B2_NVTX;
+    REQUIRE(ctx && committee_idx && bits && msg32 && sig96 && ok_out && n > 0, "sync_aggregate_verify: bad arguments");
+    REQUIRE(ctx->sync.n > 0, "sync_aggregate_verify: no sync committee loaded");
+    for (uint32_t i = 0; i < n; i++) REQUIRE(committee_idx[i] < ctx->sync.n, "sync_aggregate_verify: committee index out of range");
+    CK(cudaSetDevice(ctx->device));
+    const size_t stride = (ctx->sync.size + 7) / 8;
+    staging st(ctx);
+    const uint32_t* dc = st.in(committee_idx, n);
+    const uint8_t* db = st.in(bits, n * stride, 16);
+    const uint8_t* dmsg = st.in(msg32, (size_t)n * 32);
+    const uint8_t* dsig = st.in(sig96, (size_t)n * 96);
+    uint8_t* dok = st.out(ok_out, n);
+    uint8_t* d48 = pk48_out ? st.out(pk48_out, (size_t)n * 48) : nullptr;
+    int rc;
+    if ((rc = st.rc) || (rc = b2_sync_aggregate_verify_dev(ctx, dc, db, dmsg, dsig, n, dok, d48, ctx->s_main))) return rc;
     return st.finish();
 }
 

@@ -161,6 +161,33 @@ class Engine:
         self._ck(self.lib.b2_aggregate_pks(self.h, _p(pks), _p(off), n_seg, _p(out), _p(status)))
         return out, status
 
+    # ------------------------------------------------------------------ sync committees (Altair process_sync_aggregate)
+    def sync_committee_load(self, pubkeys48, committee_size: int):
+        """n committees of committee_size keys, uint8[n * committee_size, 48] committee after committee: decoded, KeyValidated and
+        summed once on the device (they replace the previously loaded committees).  Returns uint8[n * committee_size]: 1 where
+        KeyValidate passed."""
+        pk = _c(pubkeys48, np.uint8).reshape(-1, 48)
+        size = int(committee_size)
+        assert size > 0 and pk.shape[0] % size == 0
+        valid = np.zeros(pk.shape[0], dtype=np.uint8)
+        self._ck(self.lib.b2_sync_committee_load(self.h, _p(pk), size, pk.shape[0] // size, _p(valid)))
+        self.sync_committee_size = size
+        return valid
+
+    def sync_aggregate_verify(self, committee_idx, bits, msgs32, sigs96, want_pubkeys: bool = False):
+        """eth_fast_aggregate_verify per block: block i = participants of committee committee_idx[i] selected by its Bitvector row
+        bits[i] (uint8[n, ceil(committee_size / 8)]), signing root msgs32[i], signature sigs96[i] -> uint8[n] verdicts, and with
+        want_pubkeys also uint8[n, 48]: the compressed aggregate key of the participants."""
+        cidx = _c(committee_idx, np.uint32)
+        n = cidx.shape[0]
+        b = _c(bits, np.uint8).reshape(n, -1)
+        msgs = _c(msgs32, np.uint8).reshape(n, 32)
+        sigs = _c(sigs96, np.uint8).reshape(n, 96)
+        ok = np.zeros(n, dtype=np.uint8)
+        pk = np.zeros((n, 48), dtype=np.uint8) if want_pubkeys else None
+        self._ck(self.lib.b2_sync_aggregate_verify(self.h, _p(cidx), _p(b), _p(msgs), _p(sigs), n, _p(ok), _p(pk)))
+        return (ok, pk) if want_pubkeys else ok
+
     @staticmethod
     def _sk_limbs(sks):
         out = np.zeros((len(sks), 8), dtype=np.uint32)
@@ -365,6 +392,13 @@ class Engine:
         n_sets = d_pair_off.numel() - 1
         self._ck(self.lib.b2_aggregate_verify_dev(self.h, d_signer.data_ptr(), d_msgs.data_ptr(), d_pair_off.data_ptr(), d_signer.numel(),
                                                   d_sigs.data_ptr(), n_sets, d_ok.data_ptr(), self._stream()))
+
+    def sync_aggregate_verify_dev(self, d_committee_idx, d_bits, d_msgs, d_sigs, d_ok, d_pk48=None):
+        """b2_sync_aggregate_verify_dev: d_committee_idx uint32[n], d_bits uint8[n, ceil(committee_size / 8)], d_msgs uint8[n,32],
+        d_sigs uint8[n,96], d_ok uint8[n], d_pk48 uint8[n,48] or None"""
+        n = d_committee_idx.numel()
+        self._ck(self.lib.b2_sync_aggregate_verify_dev(self.h, d_committee_idx.data_ptr(), d_bits.data_ptr(), d_msgs.data_ptr(), d_sigs.data_ptr(), n,
+                                                       d_ok.data_ptr(), d_pk48.data_ptr() if d_pk48 is not None else None, self._stream()))
 
     def latest_messages_update_dev(self, d_members, d_off, d_bits, d_target_epoch, d_block_idx, d_accept):
         n_agg = d_off.numel() - 1

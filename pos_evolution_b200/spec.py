@@ -12,7 +12,7 @@ This module never imports oracle/.
 """
 import hashlib
 from dataclasses import dataclass, field
-from typing import Dict, List, Sequence, Set
+from typing import Dict, List, Optional, Sequence, Set
 
 import numpy as np
 
@@ -23,6 +23,8 @@ GENESIS_EPOCH = 0
 ZERO32 = bytes(32)
 DOMAIN_BEACON_PROPOSER = bytes.fromhex("00000000")
 DOMAIN_BEACON_ATTESTER = bytes.fromhex("01000000")
+DOMAIN_SYNC_COMMITTEE = bytes.fromhex("07000000")
+SYNC_REWARD_WEIGHT = 2
 TIMELY_SOURCE_FLAG_INDEX, TIMELY_TARGET_FLAG_INDEX, TIMELY_HEAD_FLAG_INDEX = 0, 1, 2
 PARTICIPATION_FLAG_WEIGHTS = [14, 26, 14]
 PROPOSER_WEIGHT = 8
@@ -46,10 +48,12 @@ class Preset:
     MAX_EFFECTIVE_BALANCE: int = 32 * 10**9
     EFFECTIVE_BALANCE_INCREMENT: int = 10**9
     PROPOSER_SCORE_BOOST: int = 40
+    SYNC_COMMITTEE_SIZE: int = 512
+    EPOCHS_PER_SYNC_COMMITTEE_PERIOD: int = 256
 
 
 MAINNET = Preset("mainnet", 32, 64, 128, 90, 65536, 8192)
-MINIMAL = Preset("minimal", 8, 4, 4, 10, 64, 64)
+MINIMAL = Preset("minimal", 8, 4, 4, 10, 64, 64, SYNC_COMMITTEE_SIZE=32, EPOCHS_PER_SYNC_COMMITTEE_PERIOD=8)
 
 
 # ----------------------------------------------------------------------------- containers
@@ -117,6 +121,18 @@ class BeaconBlock:                     # :671-676 (fields fork choice reads)
 
 
 @dataclass
+class SyncCommittee:                   # BeaconState.current_sync_committee / next_sync_committee (:371-372); Altair container
+    pubkeys: List[bytes]               # SYNC_COMMITTEE_SIZE keys; a validator may appear more than once
+    aggregate_pubkey: bytes
+
+
+@dataclass
+class SyncAggregate:                   # Altair BeaconBlockBody.sync_aggregate
+    sync_committee_bits: List[bool]    # Bitvector[SYNC_COMMITTEE_SIZE]
+    sync_committee_signature: bytes
+
+
+@dataclass
 class BeaconState:                     # :338-374 (fields the path reads/writes)
     slot: int
     fork: Fork
@@ -131,6 +147,8 @@ class BeaconState:                     # :338-374 (fields the path reads/writes)
     current_justified_checkpoint: Checkpoint = Checkpoint()
     finalized_checkpoint: Checkpoint = Checkpoint()
     justification_bits: List[int] = field(default_factory=lambda: [0] * JUSTIFICATION_BITS_LENGTH)
+    current_sync_committee: Optional[SyncCommittee] = None          # :371
+    next_sync_committee: Optional[SyncCommittee] = None             # :372
 
 
 @dataclass
@@ -250,7 +268,9 @@ class Spec:
         self._committee_cache = {}
         self._mirror = None                # device mirror of a Store (block tree + latest messages), see _sync_store
         self.registry_valid = None         # KeyValidate verdict per validator of the registry on the device (uint8[n])
-        self.stats = {"registry_uploads": 0, "balance_refreshes": 0, "store_uploads": 0, "lmd_device_updates": 0}
+        self._sync_key = None              # (length, hash of the pubkey bytes) of the sync committee on the device
+        self.sync_committee_valid = None   # KeyValidate verdict per position of that committee (uint8[SYNC_COMMITTEE_SIZE])
+        self.stats = {"registry_uploads": 0, "balance_refreshes": 0, "store_uploads": 0, "lmd_device_updates": 0, "sync_committee_uploads": 0}
         # full: fingerprint = hash of ALL pubkeys on every call (O(n) host work, catches any in-place replacement);
         # sampled: first / last / 62 strided pubkeys (O(1)); auto: full up to 65 536 validators, sampled above
         self.registry_check = "auto"
@@ -646,6 +666,83 @@ class Spec:
             tables[which][:] = eng.participation_read(which).tolist()
             for v in num:
                 state.balances[proposer] += int(v) // denominator
+
+    # ------------------------------------------------------------------ sync committee (:371-372, :540-590; Altair)
+    def compute_sync_committee_period(self, epoch):                            # :586-587
+        return epoch // self.p.EPOCHS_PER_SYNC_COMMITTEE_PERIOD
+
+    def is_assigned_to_sync_committee(self, state, epoch, validator_index):    # :564-577
+        sync_committee_period = self.compute_sync_committee_period(epoch)
+        current_sync_committee_period = self.compute_sync_committee_period(self.get_current_epoch(state))
+        next_sync_committee_period = current_sync_committee_period + 1
+        assert sync_committee_period in (current_sync_committee_period, next_sync_committee_period)
+        pubkey = state.validators[validator_index].pubkey
+        if sync_committee_period == current_sync_committee_period:
+            return pubkey in state.current_sync_committee.pubkeys
+        return pubkey in state.next_sync_committee.pubkeys
+
+    def sync_committee_on_device(self, state):
+        """state.current_sync_committee.pubkeys on the device, decoded, KeyValidated and summed ONCE per committee CONTENT (the cache key
+        is the length and a hash of all the pubkey bytes, as sync_pubkeys keys the registry).  Returns True when it uploaded."""
+        pubkeys = [bytes(pk) for pk in state.current_sync_committee.pubkeys]
+        key = (len(pubkeys), hashlib.blake2b(b"".join(pubkeys), digest_size=16).digest())
+        if key == self._sync_key:
+            return False
+        self._sync_key = None                  # a failed load below leaves nothing cached
+        self.sync_committee_valid = self.engine.sync_committee_load(np.frombuffer(b"".join(pubkeys), dtype=np.uint8), len(pubkeys))
+        self._sync_key = key
+        self.stats["sync_committee_uploads"] += 1
+        return True
+
+    def verify_sync_aggregates(self, state, items):
+        """eth_fast_aggregate_verify of state.current_sync_committee for a batch of (slot, block_root, SyncAggregate): signing root
+        sha256(block_root || get_domain(state, DOMAIN_SYNC_COMMITTEE, compute_epoch_at_slot(slot))) -- one b2_sha256_batch call --
+        and every verdict in one b2_sync_aggregate_verify call.  A bit vector of the wrong length or a signature that is not 96 bytes
+        is False.  -> uint8[len(items)]"""
+        if not items:
+            return np.zeros(0, dtype=np.uint8)
+        self.sync_committee_on_device(state)
+        size = len(state.current_sync_committee.pubkeys)
+        roots, rows, sigs, shape_ok = [], [], [], []
+        for slot, block_root, agg in items:
+            bits, sig = list(agg.sync_committee_bits), bytes(agg.sync_committee_signature)
+            good = len(bits) == size and len(sig) == 96 and len(bytes(block_root)) == 32
+            shape_ok.append(good)
+            roots.append((bytes(block_root) if good else ZERO32) + self.get_domain(state, DOMAIN_SYNC_COMMITTEE, self.compute_epoch_at_slot(slot)))
+            rows.append(bits if good else [])
+            sigs.append(sig if good else bytes(96))
+        msgs = self.engine.sha256_batch(np.frombuffer(b"".join(roots), dtype=np.uint8), 64)
+        ok = self.engine.sync_aggregate_verify(np.zeros(len(items), dtype=np.uint32), pack_bits(rows, (size + 7) // 8), msgs,
+                                               np.frombuffer(b"".join(sigs), dtype=np.uint8))
+        return ok & np.asarray(shape_ok, dtype=np.uint8)
+
+    def process_sync_aggregate(self, state, sync_aggregate):
+        """Altair process_sync_aggregate, restated from the upstream consensus specs (specs/altair/beacon-chain.md; the reference
+        names the sync committee but does not contain this function).  The signature check runs on the GPU against the cached
+        committee (verify_sync_aggregates); the committee_size balance updates stay on the host."""
+        previous_slot = max(state.slot, 1) - 1
+        root = self.get_block_root_at_slot(state, previous_slot)
+        assert self.verify_sync_aggregates(state, [(previous_slot, root, sync_aggregate)])[0]
+        total_active_increments = self.get_total_active_balance(state) // self.p.EFFECTIVE_BALANCE_INCREMENT
+        total_base_rewards = self.get_base_reward_per_increment(state) * total_active_increments
+        max_participant_rewards = total_base_rewards * SYNC_REWARD_WEIGHT // WEIGHT_DENOMINATOR // self.p.SLOTS_PER_EPOCH
+        participant_reward = max_participant_rewards // self.p.SYNC_COMMITTEE_SIZE
+        proposer_reward = participant_reward * PROPOSER_WEIGHT // (WEIGHT_DENOMINATOR - PROPOSER_WEIGHT)
+        first = {}
+        for i, v in enumerate(state.validators):                # all_pubkeys.index(pubkey): the FIRST registry index of a key
+            first.setdefault(bytes(v.pubkey), i)
+        committee_indices = []
+        for pk in state.current_sync_committee.pubkeys:
+            if bytes(pk) not in first:
+                raise ValueError("sync committee pubkey is not in the registry")
+            committee_indices.append(first[bytes(pk)])
+        proposer = self.get_beacon_proposer_index(state)
+        for participant_index, participation_bit in zip(committee_indices, sync_aggregate.sync_committee_bits):
+            if participation_bit:
+                state.balances[participant_index] += participant_reward
+                state.balances[proposer] += proposer_reward
+            else:
+                state.balances[participant_index] = max(0, state.balances[participant_index] - participant_reward)
 
     # ------------------------------------------------------------------ fork choice
     def update_latest_messages(self, store, attesting_indices, attestation):   # :1435-1441
