@@ -197,6 +197,43 @@ int b2_set_fork_choice_params(b2_ctx* ctx, uint64_t min_vote_epoch, int exclude_
 int b2_set_verify_mode(b2_ctx* ctx, int mode, const uint8_t* seed32);
 int b2_on_attester_slashing(b2_ctx* ctx, const uint32_t* indices_1, uint32_t n1, const uint32_t* indices_2, uint32_t n2);
 
+/* ---- slasher: FIND the slashable attestations (is_slashable_attestation_data, pos-evolution.md:1128-1143: double vote, surround vote)
+ * among everything that streams through, so that an AttesterSlashing (:1160-1162, on_attester_slashing :1447-1461) can be produced.
+ * A slasher is a device-resident history of n_validators validators over a ring of history_epochs (H) epochs with a current epoch `cur`
+ * that only moves forward; the window is low = max(0, cur - H + 1) .. cur.  It is independent of the registry; a context that never
+ * calls b2_slasher_init allocates nothing.  Memory: 6 * n_validators * H + 32 * H * max_attestations_per_target bytes; the byte count
+ * is compared with the free device memory first, and B2_ENOMEM is returned without trying the allocation when it does not fit.  A
+ * failed init leaves the context, and a previously initialised slasher, as they were.  H, max_attestations_per_target <= 65535. */
+int b2_slasher_init(b2_ctx* ctx, uint64_t n_validators, uint32_t history_epochs, uint32_t max_attestations_per_target, uint64_t current_epoch);
+int b2_slasher_free(b2_ctx* ctx); /* also done by b2_destroy */
+/* move the current epoch forward (a lower one is B2_EINVAL); the columns of the new epochs start empty.  Synchronises the device. */
+int b2_slasher_advance(b2_ctx* ctx, uint64_t current_epoch);
+/* Offer n_agg aggregates (members / off / bits as above; source_epoch, target_epoch = data.source.epoch, data.target.epoch;
+ * data_root32 = hash_tree_root(AttestationData)).  Aggregate a is ACCEPTED iff accept[a] != 0 (or accept == NULL), s <= t <= cur,
+ * s >= low and fewer than max_attestations_per_target aggregates with target t have been accepted; otherwise att_status_out[a] =
+ * B2_SLASHER_* says why and it neither checks nor records anything.  For every selected member v of an accepted aggregate (s, t),
+ * kind_out (u8[off[n_agg]], parallel to members; 0 for clear bits and unaccepted rows) is evaluated against EVERY attestation by v
+ * accepted so far, the other aggregates of this call included, whatever their position (:1128-1143):
+ *   B2_SLASHABLE_DOUBLE      the first accepted attestation by v with target t (earliest call, then lowest position) has another root;
+ *   B2_SLASHABLE_SURROUNDS   some accepted attestation by v has source > s and target < t; conflict_target_out[i][0] = the smallest such target;
+ *   B2_SLASHABLE_SURROUNDED  some accepted attestation by v has source < s and target > t; conflict_target_out[i][1] = the largest such target
+ * (conflict_target_out u32[off[n_agg]][2], may be NULL; 0xffffffff where the bit is clear).  Detection is exact against everything ever
+ * accepted, not only what is still inside the window.  n_flagged_out = number of member slots with kind != 0. */
+enum { B2_SLASHER_OK = 0, B2_SLASHER_NOT_ACCEPTED = 1, B2_SLASHER_SOURCE_AFTER_TARGET = 2, B2_SLASHER_TARGET_AHEAD = 3,
+       B2_SLASHER_SOURCE_EXPIRED = 4, B2_SLASHER_COLUMN_FULL = 5, B2_SLASHER_BAD_ROW = 6 /* device form only */ };
+enum { B2_SLASHABLE_DOUBLE = 1, B2_SLASHABLE_SURROUNDS = 2, B2_SLASHABLE_SURROUNDED = 4 };
+int b2_slasher_update(b2_ctx* ctx, const uint32_t* members, const uint32_t* off, const uint8_t* bits, uint32_t bits_stride,
+                      const uint64_t* source_epoch, const uint64_t* target_epoch, const uint8_t* data_root32, const uint8_t* accept, uint32_t n_agg,
+                      int32_t* att_status_out, uint8_t* kind_out, uint32_t* conflict_target_out, uint32_t* n_flagged_out);
+/* the same on device arrays (asynchronous on `stream`; the arrays b2_epoch_tail_dev / b2_latest_messages_update_dev take, with the
+ * verdict bytes as d_accept, so it chains after b2_epoch_wait_dev).  Self-guarding: a malformed offsets row is B2_SLASHER_BAD_ROW and
+ * its member slots are not written (B2_GUARD_BAD_ROW); a member index >= n_validators is skipped, its kind stays 0
+ * (B2_GUARD_BAD_INDEX); an epoch that does not fit 32 bits sets B2_GUARD_BAD_EPOCH and the row is refused by status 2 or 3. */
+int b2_slasher_update_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_off, const uint8_t* d_bits, uint32_t bits_stride,
+                          const uint64_t* d_source_epoch, const uint64_t* d_target_epoch, const uint8_t* d_data_root32, const uint8_t* d_accept,
+                          uint32_t n_agg, int32_t* d_att_status_out, uint8_t* d_kind_out, uint32_t* d_conflict_target_out,
+                          uint32_t* d_n_flagged_out, void* stream);
+
 /* Store.blocks (pos-evolution.md:898) as arrays in topological order (parent[b] < b, parent[0] ignored; block 0 =
  * store.justified_checkpoint.root).  leaf_viable[b]: the get_filtered_block_tree leaf test (:1104, prose :1121-1124). */
 int b2_tree_load(b2_ctx* ctx, const uint32_t* parent, const uint64_t* slot, const uint8_t* root32, const uint8_t* leaf_viable,

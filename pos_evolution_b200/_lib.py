@@ -63,6 +63,13 @@ SIGNATURES = {
     "b2_set_verify_mode": (c_int, [c_void_p, c_int, c_void_p]),
     "b2_epoch_set_pairing_form": (c_int, [c_void_p, c_int]),
     "b2_on_attester_slashing": (c_int, [c_void_p, c_void_p, c_uint32, c_void_p, c_uint32]),
+    "b2_slasher_init": (c_int, [c_void_p, c_uint64, c_uint32, c_uint32, c_uint64]),
+    "b2_slasher_free": (c_int, [c_void_p]),
+    "b2_slasher_advance": (c_int, [c_void_p, c_uint64]),
+    "b2_slasher_update": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32,
+                                  c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b2_slasher_update_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32,
+                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_tree_load": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32]),
     "b2_get_weights": (c_int, [c_void_p, c_int32, c_uint64, c_void_p]),
     "b2_get_head": (c_int, [c_void_p, c_uint32, c_int32, c_uint64, c_void_p]),

@@ -16,6 +16,7 @@
 #include "rlc.cuh"
 #include "aggverify.cuh"
 #include "syncagg.cuh"
+#include "slasher.cuh"
 
 using namespace b2;
 
@@ -79,6 +80,14 @@ struct sync_tables {
     dbuf records, valid;       // u32[24] affine record and u8 KeyValidate per position, committee after committee
     dbuf sum, sum_status;      // per committee: Jacobian sum of its valid keys (u32[36]), k_g1_segment_sum's status byte
     uint32_t size = 0, n = 0;
+};
+
+// slasher (b2_slasher_init): span tables and first-vote ids per (validator, epoch of the ring), per-column counts and root log
+// (slasher.cuh), and the ids of the aggregates of the update in flight
+struct slasher_tables {
+    dbuf min_span, max_span, first_id, count, root, agg_id;
+    uint64_t n_val = 0;
+    uint32_t H = 0, K = 0, cur = 0;      // H == 0: not initialised
 };
 
 struct vslot {
@@ -158,6 +167,7 @@ struct b2_ctx {
     cudaEvent_t ev_av[3] = {nullptr, nullptr, nullptr};
     std::vector<dbuf> stage;                          // the synchronous entry points' host inputs and outputs (struct staging)
     sync_tables sync;
+    slasher_tables sl;
 };
 
 struct nvtx_scope {
@@ -1426,6 +1436,138 @@ int b2_on_attester_slashing(b2_ctx* ctx, const uint32_t* indices_1, uint32_t n1,
     if (st.rc) return st.rc;
     k_mark_equivocating<<<blocks_for(n1, 128), 128, 0, ctx->s_main>>>(d1, n1, d2, n2, ctx->n_val, ctx->reg.equiv);
     CKL(ctx);
+    return st.finish();
+}
+
+// ------------------------------------------------------------------------------------------ slasher (is_slashable_attestation_data :1128-1143)
+static slasher_view slasher_view_of(const slasher_tables& t) {
+    return {t.min_span, t.max_span, t.first_id, t.count, t.root, t.n_val, t.H, t.K, t.cur, t.cur >= t.H - 1 ? t.cur - (t.H - 1) : 0};
+}
+// every column empty
+static int slasher_clear(b2_ctx* ctx, const slasher_tables& t, cudaStream_t s) {
+    const size_t table = (size_t)t.n_val * t.H * 2;
+    CK(cudaMemsetAsync(t.min_span, 0xff, table, s));
+    CK(cudaMemsetAsync(t.max_span, 0, table, s));
+    CK(cudaMemsetAsync(t.first_id, 0xff, table, s));
+    CK(cudaMemsetAsync(t.count, 0, (size_t)t.H * 4, s));
+    return B2_OK;
+}
+
+int b2_slasher_init(b2_ctx* ctx, uint64_t n_validators, uint32_t history_epochs, uint32_t max_attestations_per_target, uint64_t current_epoch) {
+    B2_NVTX;
+    // the bounds keep the byte count below 2^52: no 64-bit overflow
+    REQUIRE(ctx && n_validators > 0 && n_validators < (1ull << 32) && history_epochs > 0 && history_epochs <= 65535 &&
+                max_attestations_per_target > 0 && max_attestations_per_target <= 65535 && current_epoch < 0xffffffffull,
+            "slasher_init: bad arguments (validators < 2^32, 1 <= history_epochs, max_attestations_per_target <= 65535, epoch < 2^32 - 1)");
+    CK(cudaSetDevice(ctx->device));
+    const uint64_t table = n_validators * history_epochs * 2, log = (uint64_t)history_epochs * max_attestations_per_target * 32;
+    const uint64_t bytes = 3 * table + log + (uint64_t)history_epochs * 4;
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    if (bytes > free_b) {      // refused before any allocation is tried: the card may be shared
+        snprintf(ctx->err, sizeof(ctx->err), "slasher_init: %llu bytes needed, %llu free on the device", (unsigned long long)bytes, (unsigned long long)free_b);
+        return B2_ENOMEM;
+    }
+    slasher_tables t;      // built aside: a failed init leaves a previous slasher in place
+    int rc;
+    if ((rc = ensure(ctx, t.min_span, table)) || (rc = ensure(ctx, t.max_span, table)) || (rc = ensure(ctx, t.first_id, table)) ||
+        (rc = ensure(ctx, t.root, log)) || (rc = ensure(ctx, t.count, (size_t)history_epochs * 4)))
+        return rc;
+    t.n_val = n_validators;
+    t.H = history_epochs;
+    t.K = max_attestations_per_target;
+    t.cur = (uint32_t)current_epoch;
+    if ((rc = slasher_clear(ctx, t, ctx->s_main))) return rc;
+    CK(cudaStreamSynchronize(ctx->s_main));
+    ctx->sl = std::move(t);
+    return B2_OK;
+}
+
+int b2_slasher_free(b2_ctx* ctx) {
+    B2_NVTX;
+    REQUIRE(ctx, "null context");
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaDeviceSynchronize());
+    ctx->sl = slasher_tables();
+    return B2_OK;
+}
+
+int b2_slasher_advance(b2_ctx* ctx, uint64_t current_epoch) {
+    B2_NVTX;
+    REQUIRE(ctx && ctx->sl.H, "slasher_advance: no slasher (b2_slasher_init)");
+    slasher_tables& t = ctx->sl;
+    REQUIRE(current_epoch >= t.cur && current_epoch < 0xffffffffull, "slasher_advance: the current epoch only moves forward and fits 32 bits");
+    if (current_epoch == t.cur) return B2_OK;
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaDeviceSynchronize());      // updates enqueued on the caller's streams see the window they were enqueued with
+    const uint64_t n_cols = current_epoch - t.cur;
+    if (n_cols >= t.H) {
+        int rc;
+        if ((rc = slasher_clear(ctx, t, ctx->s_main))) return rc;
+    } else {
+        const unsigned blocks = (unsigned)std::min<uint64_t>((t.n_val * n_cols + 255) / 256, (uint64_t)ctx->n_sm * 16);
+        k_slasher_advance<<<blocks, 256, 0, ctx->s_main>>>(slasher_view_of(t), t.cur + 1, (uint32_t)n_cols);
+        CKL(ctx);
+    }
+    CK(cudaStreamSynchronize(ctx->s_main));
+    t.cur = (uint32_t)current_epoch;
+    return B2_OK;
+}
+
+int b2_slasher_update_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_off, const uint8_t* d_bits, uint32_t bits_stride,
+                          const uint64_t* d_source_epoch, const uint64_t* d_target_epoch, const uint8_t* d_data_root32, const uint8_t* d_accept,
+                          uint32_t n_agg, int32_t* d_att_status_out, uint8_t* d_kind_out, uint32_t* d_conflict_target_out, uint32_t* d_n_flagged_out,
+                          void* stream) {
+    B2_NVTX;
+    REQUIRE(ctx && d_members && d_off && d_bits && d_source_epoch && d_target_epoch && d_data_root32 && d_att_status_out && d_kind_out &&
+                d_n_flagged_out && n_agg > 0 && bits_stride > 0, "slasher_update_dev: bad arguments");
+    REQUIRE(ctx->sl.H, "slasher_update: no slasher (b2_slasher_init)");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    int rc;
+    if ((rc = ensure(ctx, ctx->sl.agg_id, (size_t)n_agg * 4))) return rc;
+    const slasher_view S = slasher_view_of(ctx->sl);
+    uint32_t* ids = ctx->sl.agg_id;
+    CK(cudaMemsetAsync(d_n_flagged_out, 0, 4, s));
+    k_slasher_rows<<<blocks_for(n_agg, 128), 128, 0, s>>>(S, d_off, bits_stride, d_source_epoch, d_target_epoch, d_data_root32, d_accept, n_agg,
+                                                          d_att_status_out, ids, ctx->d_guard);
+    CKL(ctx);
+    k_slasher_record<<<n_agg, 128, 0, s>>>(S, d_members, d_off, d_bits, bits_stride, d_source_epoch, d_target_epoch, ids, n_agg, ctx->d_guard);
+    CKL(ctx);
+    k_slasher_check<<<n_agg, 128, 0, s>>>(S, d_members, d_off, d_bits, bits_stride, d_source_epoch, d_target_epoch, ids, n_agg, d_kind_out,
+                                          d_conflict_target_out, d_n_flagged_out);
+    CKL(ctx);
+    return B2_OK;
+}
+
+int b2_slasher_update(b2_ctx* ctx, const uint32_t* members, const uint32_t* off, const uint8_t* bits, uint32_t bits_stride,
+                      const uint64_t* source_epoch, const uint64_t* target_epoch, const uint8_t* data_root32, const uint8_t* accept, uint32_t n_agg,
+                      int32_t* att_status_out, uint8_t* kind_out, uint32_t* conflict_target_out, uint32_t* n_flagged_out) {
+    B2_NVTX;
+    REQUIRE(ctx && members && off && bits && source_epoch && target_epoch && data_root32 && att_status_out && kind_out && n_flagged_out &&
+                n_agg > 0 && bits_stride > 0, "slasher_update: bad arguments");
+    REQUIRE(ctx->sl.H, "slasher_update: no slasher (b2_slasher_init)");
+    int rc;
+    if ((rc = check_batch(ctx, members, off, bits_stride, n_agg, ctx->sl.n_val))) return rc;
+    for (uint32_t a = 0; a < n_agg; a++)
+        REQUIRE(source_epoch[a] < 0xffffffffull && target_epoch[a] < 0xffffffffull, "slasher_update: epoch does not fit 32 bits");
+    CK(cudaSetDevice(ctx->device));
+    staging st(ctx);
+    const size_t total = off[n_agg];
+    const uint32_t* dm = st.in(members, total, 4);
+    const uint32_t* dof = st.in(off, (size_t)n_agg + 1);
+    const uint8_t* db = st.in(bits, (size_t)n_agg * bits_stride, 16);
+    const uint64_t* dse = st.in(source_epoch, n_agg);
+    const uint64_t* dte = st.in(target_epoch, n_agg);
+    const uint8_t* droot = st.in(data_root32, (size_t)n_agg * 32);
+    const uint8_t* dacc = accept ? st.in(accept, n_agg) : nullptr;
+    int32_t* dst = st.out(att_status_out, n_agg);
+    uint8_t* dkind = st.out(kind_out, total);
+    uint32_t* dconf = conflict_target_out ? st.out(conflict_target_out, 2 * total) : nullptr;
+    uint32_t* dflag = st.out(n_flagged_out, 1);
+    if ((rc = st.rc) ||
+        (rc = b2_slasher_update_dev(ctx, dm, dof, db, bits_stride, dse, dte, droot, dacc, n_agg, dst, dkind, dconf, dflag, ctx->s_main)))
+        return rc;
     return st.finish();
 }
 

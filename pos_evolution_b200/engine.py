@@ -323,6 +323,35 @@ class Engine:
         a, b = _c(indices_1, np.uint32), _c(indices_2, np.uint32)
         self._ck(self.lib.b2_on_attester_slashing(self.h, _p(a), a.shape[0], _p(b), b.shape[0]))
 
+    # ------------------------------------------------------------------ slasher (is_slashable_attestation_data, pos-evolution.md:1128-1143)
+    def slasher_init(self, n_validators: int, history_epochs: int, max_attestations_per_target: int, current_epoch: int = 0):
+        """Device-resident attestation history of n_validators over a ring of history_epochs epochs (6 * n * H + 32 * H * max bytes);
+        raises B2Error(B2_ENOMEM) without allocating when that exceeds the free device memory."""
+        self._ck(self.lib.b2_slasher_init(self.h, int(n_validators), int(history_epochs), int(max_attestations_per_target), int(current_epoch)))
+
+    def slasher_free(self):
+        self._ck(self.lib.b2_slasher_free(self.h))
+
+    def slasher_advance(self, current_epoch: int):
+        self._ck(self.lib.b2_slasher_advance(self.h, int(current_epoch)))
+
+    def slasher_update(self, members, off, bits, source_epoch, target_epoch, data_root32, accept=None):
+        """Offer a batch of aggregates -> (status int32[n_agg] B2_SLASHER_*, kind uint8[len(members)] B2_SLASHABLE_* bits per member
+        slot, conflict_target uint32[len(members), 2] (smallest surrounded / largest surrounding target, 0xffffffff = none), n_flagged)."""
+        members, off, bits, n_agg, stride = self._batch(members, off, bits)
+        se, te = _c(source_epoch, np.uint64), _c(target_epoch, np.uint64)
+        roots = _c(data_root32, np.uint8).reshape(n_agg, 32)
+        acc = _c(accept, np.uint8) if accept is not None else None
+        assert se.shape == (n_agg,) and te.shape == (n_agg,) and members.shape[0] >= int(off[-1])
+        total = int(off[-1])
+        status = np.zeros(n_agg, dtype=np.int32)
+        kind = np.zeros(total, dtype=np.uint8)
+        conflict = np.full((total, 2), 0xFFFFFFFF, dtype=np.uint32)
+        flagged = ctypes.c_uint32(0)
+        self._ck(self.lib.b2_slasher_update(self.h, _p(members), _p(off), _p(bits), stride, _p(se), _p(te), _p(roots), _p(acc), n_agg,
+                                            _p(status), _p(kind), _p(conflict), ctypes.byref(flagged)))
+        return status, kind, conflict, int(flagged.value)
+
     def tree_load(self, parent, slot, roots32, leaf_viable):
         parent, slot = _c(parent, np.uint32), _c(slot, np.uint64)
         roots = _c(roots32, np.uint8).reshape(-1, 32)
@@ -405,6 +434,17 @@ class Engine:
         self._ck(self.lib.b2_latest_messages_update_dev(self.h, d_members.data_ptr(), d_off.data_ptr(), d_bits.data_ptr(), d_bits.shape[1],
                                                         d_target_epoch.data_ptr(), d_block_idx.data_ptr(),
                                                         d_accept.data_ptr() if d_accept is not None else None, n_agg, self._stream()))
+
+    def slasher_update_dev(self, d_members, d_off, d_bits, d_source_epoch, d_target_epoch, d_roots, d_accept, d_status, d_kind, d_conflict,
+                           d_n_flagged):
+        """b2_slasher_update_dev: the arrays of latest_messages_update_dev plus uint64 source epochs and uint8[n_agg, 32] data roots;
+        outputs int32[n_agg], uint8[len(members)], uint32[len(members), 2] or None, uint32[1]"""
+        n_agg = d_off.numel() - 1
+        self._ck(self.lib.b2_slasher_update_dev(self.h, d_members.data_ptr(), d_off.data_ptr(), d_bits.data_ptr(), d_bits.shape[1],
+                                                d_source_epoch.data_ptr(), d_target_epoch.data_ptr(), d_roots.data_ptr(),
+                                                d_accept.data_ptr() if d_accept is not None else None, n_agg, d_status.data_ptr(),
+                                                d_kind.data_ptr(), d_conflict.data_ptr() if d_conflict is not None else None,
+                                                d_n_flagged.data_ptr(), self._stream()))
 
     def epoch_dev(self, d_sigs, d_members, d_off, d_bits, d_msgs, d_target_epoch, d_block_idx, d_agg_sig, d_agg_status, d_ok):
         n_agg = d_off.numel() - 1

@@ -270,6 +270,7 @@ class Spec:
         self.registry_valid = None         # KeyValidate verdict per validator of the registry on the device (uint8[n])
         self._sync_key = None              # (length, hash of the pubkey bytes) of the sync committee on the device
         self.sync_committee_valid = None   # KeyValidate verdict per position of that committee (uint8[SYNC_COMMITTEE_SIZE])
+        self._slasher = None               # slasher_start: size and current epoch of the device history, accepted attestations by target epoch
         self.stats = {"registry_uploads": 0, "balance_refreshes": 0, "store_uploads": 0, "lmd_device_updates": 0, "sync_committee_uploads": 0}
         # full: fingerprint = hash of ALL pubkeys on every call (O(n) host work, catches any in-place replacement);
         # sampled: first / last / 62 strided pubkeys (O(1)); auto: full up to 65 536 validators, sampled above
@@ -826,6 +827,76 @@ class Spec:
                 m["n_equiv"] = len(store.equivocating_indices)
             else:
                 self._mirror = None
+
+    # ------------------------------------------------------------------ slashing detection (:1128-1143 -> AttesterSlashing :1160-1162)
+    def slasher_start(self, state, history_epochs, max_attestations_per_target=None):
+        """Start a slasher (Engine.slasher_init) for the validators of `state` at its current epoch: a device-resident history of
+        history_epochs epochs that find_attester_slashings feeds.  max_attestations_per_target defaults to twice the committees of an epoch."""
+        per_target = max_attestations_per_target or 2 * self.p.MAX_COMMITTEES_PER_SLOT * self.p.SLOTS_PER_EPOCH
+        cur = self.get_current_epoch(state)
+        self.engine.slasher_init(len(state.validators), history_epochs, per_target, cur)
+        self._slasher = dict(n=len(state.validators), H=int(history_epochs), cur=cur, recorded={})
+
+    def find_attester_slashings(self, state, indexed_attestations, verify=True) -> List[AttesterSlashing]:
+        """Offer IndexedAttestations to the slasher and return the AttesterSlashings they complete, against everything offered before and
+        against each other.  verify: only attestations that pass is_valid_indexed_attestation(state, .) are recorded.  The double and
+        surround votes are found on the GPU (b2_slasher_update); the host keeps the accepted attestations by target epoch inside the
+        window and, only when something was flagged, looks up the partner at the reported target epoch, asserts
+        is_slashable_attestation_data on the pair and orders it as on_attester_slashing wants it (attestation_1 surrounds attestation_2)."""
+        sl = self._slasher
+        assert sl is not None, "slasher_start first"
+        atts = list(indexed_attestations)
+        if not atts:
+            return []
+        n = sl["n"]
+        accept = self.are_valid_indexed_attestations(state, atts) if verify else np.ones(len(atts), dtype=np.uint8)
+        accept = np.array(accept, dtype=np.uint8)
+        cur = self.get_current_epoch(state)
+        if cur > sl["cur"]:
+            self.engine.slasher_advance(cur)
+            sl["cur"] = cur
+            low = max(0, cur - sl["H"] + 1)
+            for t in [t for t in sl["recorded"] if t < low]:      # nothing the device still accepts can conflict with them
+                del sl["recorded"][t]
+        members, off, src, tgt, roots = [], [0], [], [], []
+        for a, ia in enumerate(atts):
+            idx = [int(i) for i in ia.attesting_indices]
+            s, t = int(ia.data.source.epoch), int(ia.data.target.epoch)
+            if not (idx and idx == sorted(set(idx)) and idx[-1] < n and max(s, t) < 0xFFFFFFFF):
+                accept[a], idx, s, t = 0, [], 0, 0              # what the device tables cannot hold is not offered
+            members += idx
+            off.append(len(members))
+            src.append(s)
+            tgt.append(t)
+            roots.append(hash_tree_root_attestation_data(ia.data))
+        sizes = np.diff(np.asarray(off, dtype=np.int64))
+        bits = np.zeros((len(atts), max(1, (int(sizes.max()) + 7) // 8)), dtype=np.uint8)
+        for a, k in enumerate(sizes):
+            bits[a] = np.packbits(np.arange(8 * bits.shape[1]) < k, bitorder="little")
+        status, kind, conflict, n_flagged = self.engine.slasher_update(
+            np.asarray(members, dtype=np.uint32), off, bits, src, tgt, np.frombuffer(b"".join(roots), dtype=np.uint8), accept)
+        for a in np.nonzero(status == 0)[0]:
+            sl["recorded"].setdefault(tgt[a], []).append(atts[a])
+        if n_flagged == 0:
+            return []
+        rules = {       # kind bit -> (partner's target epoch, ordered pair) of attestation `ia` with partner `c`
+            1: lambda ia, c: ia.data != c.data and (c, ia),
+            2: lambda ia, c: ia.data.source.epoch < c.data.source.epoch and (ia, c),
+            4: lambda ia, c: c.data.source.epoch < ia.data.source.epoch and (c, ia),
+        }
+        out, seen = [], set()
+        for i in np.nonzero(kind)[0]:
+            a = int(np.searchsorted(off, i, side="right")) - 1
+            ia, v = atts[a], members[i]
+            for bit, target in ((1, tgt[a]), (2, int(conflict[i, 0])), (4, int(conflict[i, 1]))):
+                if not kind[i] & bit:
+                    continue
+                pair = next(p for p in (rules[bit](ia, c) for c in sl["recorded"][target] if c is not ia and v in c.attesting_indices) if p)
+                assert self.is_slashable_attestation_data(pair[0].data, pair[1].data)
+                if (id(pair[0]), id(pair[1])) not in seen:
+                    seen.add((id(pair[0]), id(pair[1])))
+                    out.append(AttesterSlashing(pair[0], pair[1]))
+        return out
 
     def _store_arrays(self, store):
         """Store (dicts) -> the array form of include/b200pos.h: blocks below the justified root in topological order."""
