@@ -205,9 +205,22 @@ int b2_on_attester_slashing(b2_ctx* ctx, const uint32_t* indices_1, uint32_t n1,
  * is compared with the free device memory first, and B2_ENOMEM is returned without trying the allocation when it does not fit.  A
  * failed init leaves the context, and a previously initialised slasher, as they were.  H, max_attestations_per_target <= 65535. */
 int b2_slasher_init(b2_ctx* ctx, uint64_t n_validators, uint32_t history_epochs, uint32_t max_attestations_per_target, uint64_t current_epoch);
+/* The same for the validators [v_begin, v_end) of n_validators only (0 <= v_begin < v_end <= n_validators, else B2_EINVAL): one rank's
+ * share of a registry sharded by validator range.  Memory 6 * (v_end - v_begin) * H + 32 * H * max_attestations_per_target + 4 * H bytes,
+ * compared with the free device memory as above.  Updates take the whole batch: a member index >= n_validators still sets
+ * B2_GUARD_BAD_INDEX (device form) or is B2_EINVAL (host form); a valid member outside [v_begin, v_end) is skipped silently (kind 0,
+ * conflict targets 0xffffffff, not counted in n_flagged).  Statuses, ids, column counts and the root log do not depend on the range, so
+ * slashers over the ranges of a partition fed the same batches stay consistent, and the union of their kind vectors is the vector of
+ * one slasher over all validators.  b2_slasher_init is b2_slasher_init_range(0, n_validators). */
+int b2_slasher_init_range(b2_ctx* ctx, uint64_t n_validators, uint64_t v_begin, uint64_t v_end, uint32_t history_epochs,
+                          uint32_t max_attestations_per_target, uint64_t current_epoch);
 int b2_slasher_free(b2_ctx* ctx); /* also done by b2_destroy */
-/* move the current epoch forward (a lower one is B2_EINVAL); the columns of the new epochs start empty.  Synchronises the device. */
+/* move the current epoch forward (a lower one, or one that does not fit 32 bits, is B2_EINVAL and changes nothing); the columns of the
+ * new epochs start empty.  Synchronises the device. */
 int b2_slasher_advance(b2_ctx* ctx, uint64_t current_epoch);
+/* The same without synchronising: the column reset is enqueued on `stream` and the window moves at enqueue time, so every update
+ * enqueued after this call sees the new window and must be stream-ordered after the reset by the caller (same stream, or an event). */
+int b2_slasher_advance_dev(b2_ctx* ctx, uint64_t current_epoch, void* stream);
 /* Offer n_agg aggregates (members / off / bits as above; source_epoch, target_epoch = data.source.epoch, data.target.epoch;
  * data_root32 = hash_tree_root(AttestationData)).  Aggregate a is ACCEPTED iff accept[a] != 0 (or accept == NULL), s <= t <= cur,
  * s >= low and fewer than max_attestations_per_target aggregates with target t have been accepted; otherwise att_status_out[a] =

@@ -65,7 +65,9 @@ SIGNATURES = {
     "b2_on_attester_slashing": (c_int, [c_void_p, c_void_p, c_uint32, c_void_p, c_uint32]),
     "b2_slasher_init": (c_int, [c_void_p, c_uint64, c_uint32, c_uint32, c_uint64]),
     "b2_slasher_free": (c_int, [c_void_p]),
+    "b2_slasher_init_range": (c_int, [c_void_p, c_uint64, c_uint64, c_uint64, c_uint32, c_uint32, c_uint64]),
     "b2_slasher_advance": (c_int, [c_void_p, c_uint64]),
+    "b2_slasher_advance_dev": (c_int, [c_void_p, c_uint64, c_void_p]),
     "b2_slasher_update": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32,
                                   c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_slasher_update_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32,

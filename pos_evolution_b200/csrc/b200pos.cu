@@ -86,7 +86,8 @@ struct sync_tables {
 // (slasher.cuh), and the ids of the aggregates of the update in flight
 struct slasher_tables {
     dbuf min_span, max_span, first_id, count, root, agg_id;
-    uint64_t n_val = 0;
+    uint64_t n_val = 0, n_rows = 0;      // validators of the registry; rows held, for validators v_begin .. v_begin + n_rows - 1
+    uint32_t v_begin = 0;
     uint32_t H = 0, K = 0, cur = 0;      // H == 0: not initialised
 };
 
@@ -1441,11 +1442,11 @@ int b2_on_attester_slashing(b2_ctx* ctx, const uint32_t* indices_1, uint32_t n1,
 
 // ------------------------------------------------------------------------------------------ slasher (is_slashable_attestation_data :1128-1143)
 static slasher_view slasher_view_of(const slasher_tables& t) {
-    return {t.min_span, t.max_span, t.first_id, t.count, t.root, t.n_val, t.H, t.K, t.cur, t.cur >= t.H - 1 ? t.cur - (t.H - 1) : 0};
+    return {t.min_span, t.max_span, t.first_id, t.count, t.root, t.n_val, t.n_rows, t.v_begin, t.H, t.K, t.cur, t.cur >= t.H - 1 ? t.cur - (t.H - 1) : 0};
 }
 // every column empty
 static int slasher_clear(b2_ctx* ctx, const slasher_tables& t, cudaStream_t s) {
-    const size_t table = (size_t)t.n_val * t.H * 2;
+    const size_t table = (size_t)t.n_rows * t.H * 2;
     CK(cudaMemsetAsync(t.min_span, 0xff, table, s));
     CK(cudaMemsetAsync(t.max_span, 0, table, s));
     CK(cudaMemsetAsync(t.first_id, 0xff, table, s));
@@ -1453,14 +1454,17 @@ static int slasher_clear(b2_ctx* ctx, const slasher_tables& t, cudaStream_t s) {
     return B2_OK;
 }
 
-int b2_slasher_init(b2_ctx* ctx, uint64_t n_validators, uint32_t history_epochs, uint32_t max_attestations_per_target, uint64_t current_epoch) {
+int b2_slasher_init_range(b2_ctx* ctx, uint64_t n_validators, uint64_t v_begin, uint64_t v_end, uint32_t history_epochs,
+                          uint32_t max_attestations_per_target, uint64_t current_epoch) {
     B2_NVTX;
     // the bounds keep the byte count below 2^52: no 64-bit overflow
-    REQUIRE(ctx && n_validators > 0 && n_validators < (1ull << 32) && history_epochs > 0 && history_epochs <= 65535 &&
-                max_attestations_per_target > 0 && max_attestations_per_target <= 65535 && current_epoch < 0xffffffffull,
-            "slasher_init: bad arguments (validators < 2^32, 1 <= history_epochs, max_attestations_per_target <= 65535, epoch < 2^32 - 1)");
+    REQUIRE(ctx && n_validators > 0 && n_validators < (1ull << 32) && v_begin < v_end && v_end <= n_validators && history_epochs > 0 &&
+                history_epochs <= 65535 && max_attestations_per_target > 0 && max_attestations_per_target <= 65535 && current_epoch < 0xffffffffull,
+            "slasher_init: bad arguments (validators < 2^32, 0 <= v_begin < v_end <= validators, 1 <= history_epochs, "
+            "max_attestations_per_target <= 65535, epoch < 2^32 - 1)");
     CK(cudaSetDevice(ctx->device));
-    const uint64_t table = n_validators * history_epochs * 2, log = (uint64_t)history_epochs * max_attestations_per_target * 32;
+    const uint64_t rows = v_end - v_begin;
+    const uint64_t table = rows * history_epochs * 2, log = (uint64_t)history_epochs * max_attestations_per_target * 32;
     const uint64_t bytes = 3 * table + log + (uint64_t)history_epochs * 4;
     size_t free_b = 0, total_b = 0;
     CK(cudaMemGetInfo(&free_b, &total_b));
@@ -1474,6 +1478,8 @@ int b2_slasher_init(b2_ctx* ctx, uint64_t n_validators, uint32_t history_epochs,
         (rc = ensure(ctx, t.root, log)) || (rc = ensure(ctx, t.count, (size_t)history_epochs * 4)))
         return rc;
     t.n_val = n_validators;
+    t.n_rows = rows;
+    t.v_begin = (uint32_t)v_begin;
     t.H = history_epochs;
     t.K = max_attestations_per_target;
     t.cur = (uint32_t)current_epoch;
@@ -1481,6 +1487,10 @@ int b2_slasher_init(b2_ctx* ctx, uint64_t n_validators, uint32_t history_epochs,
     CK(cudaStreamSynchronize(ctx->s_main));
     ctx->sl = std::move(t);
     return B2_OK;
+}
+
+int b2_slasher_init(b2_ctx* ctx, uint64_t n_validators, uint32_t history_epochs, uint32_t max_attestations_per_target, uint64_t current_epoch) {
+    return b2_slasher_init_range(ctx, n_validators, 0, n_validators, history_epochs, max_attestations_per_target, current_epoch);
 }
 
 int b2_slasher_free(b2_ctx* ctx) {
@@ -1492,25 +1502,37 @@ int b2_slasher_free(b2_ctx* ctx) {
     return B2_OK;
 }
 
-int b2_slasher_advance(b2_ctx* ctx, uint64_t current_epoch) {
+int b2_slasher_advance_dev(b2_ctx* ctx, uint64_t current_epoch, void* stream) {
     B2_NVTX;
     REQUIRE(ctx && ctx->sl.H, "slasher_advance: no slasher (b2_slasher_init)");
     slasher_tables& t = ctx->sl;
     REQUIRE(current_epoch >= t.cur && current_epoch < 0xffffffffull, "slasher_advance: the current epoch only moves forward and fits 32 bits");
     if (current_epoch == t.cur) return B2_OK;
     CK(cudaSetDevice(ctx->device));
-    CK(cudaDeviceSynchronize());      // updates enqueued on the caller's streams see the window they were enqueued with
+    cudaStream_t s = (cudaStream_t)stream;
     const uint64_t n_cols = current_epoch - t.cur;
     if (n_cols >= t.H) {
         int rc;
-        if ((rc = slasher_clear(ctx, t, ctx->s_main))) return rc;
+        if ((rc = slasher_clear(ctx, t, s))) return rc;
     } else {
-        const unsigned blocks = (unsigned)std::min<uint64_t>((t.n_val * n_cols + 255) / 256, (uint64_t)ctx->n_sm * 16);
-        k_slasher_advance<<<blocks, 256, 0, ctx->s_main>>>(slasher_view_of(t), t.cur + 1, (uint32_t)n_cols);
+        const unsigned blocks = (unsigned)std::min<uint64_t>((t.n_rows * n_cols + 255) / 256, (uint64_t)ctx->n_sm * 16);
+        k_slasher_advance<<<blocks, 256, 0, s>>>(slasher_view_of(t), t.cur + 1, (uint32_t)n_cols);
         CKL(ctx);
     }
+    t.cur = (uint32_t)current_epoch;      // the window of every update enqueued from now on; they are ordered after the reset by the caller
+    return B2_OK;
+}
+
+int b2_slasher_advance(b2_ctx* ctx, uint64_t current_epoch) {
+    B2_NVTX;
+    REQUIRE(ctx && ctx->sl.H, "slasher_advance: no slasher (b2_slasher_init)");
+    REQUIRE(current_epoch >= ctx->sl.cur && current_epoch < 0xffffffffull, "slasher_advance: the current epoch only moves forward and fits 32 bits");
+    if (current_epoch == ctx->sl.cur) return B2_OK;
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaDeviceSynchronize());      // updates enqueued on the caller's streams see the window they were enqueued with
+    int rc;
+    if ((rc = b2_slasher_advance_dev(ctx, current_epoch, ctx->s_main))) return rc;
     CK(cudaStreamSynchronize(ctx->s_main));
-    t.cur = (uint32_t)current_epoch;
     return B2_OK;
 }
 

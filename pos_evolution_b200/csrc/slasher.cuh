@@ -1,7 +1,9 @@
 // slasher.cuh -- detection of slashable attestations (is_slashable_attestation_data, pos-evolution.md:1128-1143): the double and
 // surround votes of every accepted aggregate, from per-validator span tables over a ring of H epochs.  Included by b200pos.cu only.
 //
-// Tables, validator-major (cell (v, e) at v * H + e mod H; the walks below run along e for one validator):
+// Tables, validator-major (cell (v, e) at (v - v_begin) * H + e mod H; the walks below run along e for one validator).  A slasher may
+// hold a range [v_begin, v_begin + n_rows) of the n_val validators only (one rank's share of a sharded registry): members outside it
+// are skipped without a guard bit, while everything per aggregate (status, id, column count, root log) is the same on every range.
 //   min_span u16: min over the accepted attestations (s, t) of v with s > e of t - e; none = SL_NONE
 //   max_span u16: max over those with s < e < t of t - e;                      none = 0
 //   first_id u16: id of the first accepted attestation of v with target e;     none = SL_NONE
@@ -36,8 +38,8 @@ struct slasher_view {
     uint16_t *min_span, *max_span, *first_id;      // u16[n_val][H]
     uint32_t* count;                               // u32[H] aggregates recorded per target column
     uint8_t* root;                                 // u8[H][K][32]
-    uint64_t n_val;
-    uint32_t H, K, cur, low;
+    uint64_t n_val, n_rows;                        // validators of the registry; rows held: v_begin .. v_begin + n_rows - 1
+    uint32_t v_begin, H, K, cur, low;
 };
 
 // 16-bit atomic min / max: a CAS loop that issues nothing when the cell already holds a value at least as good; returns the value
@@ -116,16 +118,18 @@ __global__ void __launch_bounds__(128) k_slasher_rows(slasher_view S, const uint
     agg_id[a] = id;
 }
 
-// selected member j of aggregate a -> validator v; false for a clear bit or an index outside the tables (GUARD_BAD_INDEX)
+// selected member j of aggregate a -> its row v - v_begin of the tables; false for a clear bit, an index outside the registry
+// (GUARD_BAD_INDEX) or a validator outside this slasher's range (silently: another range holds it)
 __device__ __forceinline__ bool sl_member(const slasher_view& S, const uint32_t* members, uint32_t o0, const uint8_t* bits, uint32_t stride,
-                                          uint32_t a, uint32_t j, uint32_t& v, uint32_t* guard) {
+                                          uint32_t a, uint32_t j, uint32_t& row, uint32_t* guard) {
     if (!((bits[(uint64_t)a * stride + (j >> 3)] >> (j & 7)) & 1)) return false;
-    v = members[o0 + j];
+    const uint32_t v = members[o0 + j];
     if (v >= S.n_val) {
         if (guard) atomicOr(guard, (uint32_t)GUARD_BAD_INDEX);
         return false;
     }
-    return true;
+    row = v - S.v_begin;      // wraps above n_rows for v < v_begin
+    return row < S.n_rows;
 }
 
 // Block per accepted aggregate (s, t), thread per member: first_id by atomic min on the id, then the two span walks.
@@ -213,7 +217,7 @@ __global__ void __launch_bounds__(128) k_slasher_check(slasher_view S, const uin
 
 // The window moves up: the columns of the epochs first .. first + n_cols - 1 (n_cols < H) become empty
 __global__ void __launch_bounds__(256) k_slasher_advance(slasher_view S, uint32_t first, uint32_t n_cols) {
-    const uint64_t total = S.n_val * n_cols;
+    const uint64_t total = S.n_rows * n_cols;
     for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (uint64_t)gridDim.x * blockDim.x) {
         const uint64_t cell = (i / n_cols) * S.H + (first + (uint32_t)(i % n_cols)) % S.H;
         S.min_span[cell] = (uint16_t)SL_NONE;

@@ -324,10 +324,14 @@ class Engine:
         self._ck(self.lib.b2_on_attester_slashing(self.h, _p(a), a.shape[0], _p(b), b.shape[0]))
 
     # ------------------------------------------------------------------ slasher (is_slashable_attestation_data, pos-evolution.md:1128-1143)
-    def slasher_init(self, n_validators: int, history_epochs: int, max_attestations_per_target: int, current_epoch: int = 0):
+    def slasher_init(self, n_validators: int, history_epochs: int, max_attestations_per_target: int, current_epoch: int = 0,
+                     v_begin: int = 0, v_end: int = None):
         """Device-resident attestation history of n_validators over a ring of history_epochs epochs (6 * n * H + 32 * H * max bytes);
-        raises B2Error(B2_ENOMEM) without allocating when that exceeds the free device memory."""
-        self._ck(self.lib.b2_slasher_init(self.h, int(n_validators), int(history_epochs), int(max_attestations_per_target), int(current_epoch)))
+        raises B2Error(B2_ENOMEM) without allocating when that exceeds the free device memory.  [v_begin, v_end): hold the validators
+        of that range only (6 * (v_end - v_begin) * H + 32 * H * max bytes); members outside it are skipped silently."""
+        v_end = n_validators if v_end is None else v_end
+        self._ck(self.lib.b2_slasher_init_range(self.h, int(n_validators), int(v_begin), int(v_end), int(history_epochs),
+                                                int(max_attestations_per_target), int(current_epoch)))
 
     def slasher_free(self):
         self._ck(self.lib.b2_slasher_free(self.h))
@@ -434,6 +438,11 @@ class Engine:
         self._ck(self.lib.b2_latest_messages_update_dev(self.h, d_members.data_ptr(), d_off.data_ptr(), d_bits.data_ptr(), d_bits.shape[1],
                                                         d_target_epoch.data_ptr(), d_block_idx.data_ptr(),
                                                         d_accept.data_ptr() if d_accept is not None else None, n_agg, self._stream()))
+
+    def slasher_advance_dev(self, current_epoch: int):
+        """b2_slasher_advance_dev on the current stream: the column reset is enqueued, nothing synchronises; updates enqueued later
+        on this stream see the new window"""
+        self._ck(self.lib.b2_slasher_advance_dev(self.h, int(current_epoch), self._stream()))
 
     def slasher_update_dev(self, d_members, d_off, d_bits, d_source_epoch, d_target_epoch, d_roots, d_accept, d_status, d_kind, d_conflict,
                            d_n_flagged):

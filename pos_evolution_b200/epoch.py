@@ -26,9 +26,15 @@ Multi-GPU, two layouts (SURVEY.md section 8e):
     after which EVERY rank applies update_latest_messages for ALL accepted aggregates to its replica of the LMD table
     (12 B per set bit, microseconds); then get_head: rank g scatters the votes of validators [g*N/world, (g+1)*N/world)
     only, one u64[n_blocks] all-reduce, head on every rank.  No collective touches the BLS data path.
+
+Slashing detection (`enable_slasher`): after each epoch's fork choice, on the fork-choice stream and so in epoch order, the slasher
+(include/b200pos.h, b2_slasher_*) records and checks every accepted aggregate of the epoch; `Ticket.slashings()` reports the flagged
+member slots.  Sharded, rank g holds the history of validators [g*N/world, (g+1)*N/world) only -- the range of its vote scatter --
+and reports those; the ranks' reports together are the unsharded one, with no collective added.
 """
 import collections
 
+import numpy as np
 import torch
 
 from .engine import Engine
@@ -36,13 +42,22 @@ from .engine import Engine
 MAX_DEPTH = 16      # == B2_EPOCH_SLOTS (include/b200pos.h)
 
 
+Slashings = collections.namedtuple("Slashings", "status aggregate position validator kind surrounded_target surrounding_target")
+Slashings.__doc__ = """What the slasher found in one epoch (numpy arrays).  status: int32[n_agg], B2_SLASHER_* per aggregate.  One entry per
+flagged member slot: aggregate index, position in the committee, validator index, kind (B2_SLASHABLE_* bits: 1 double, 2 surrounds,
+4 surrounded), the smallest target among the attestations it surrounds and the largest target among those surrounding it
+(0xffffffff where that bit is clear).  A conflicting target names the epoch batch that holds the partner attestation."""
+
+
 class _Ticket:
     """Result of one submitted epoch: verdict bytes + head index (+ the aggregate signatures), valid after .wait() and until
-    `depth` further epochs have been submitted."""
+    `depth` further epochs have been submitted; with the slasher on, also its findings (.slashings())."""
 
-    def __init__(self, slot, d_ok, d_head, d_agg_sig, event, h_ok=None, h_head=None, h_agg_sig=None):
+    def __init__(self, slot, d_ok, d_head, d_agg_sig, event, h_ok=None, h_head=None, h_agg_sig=None, slashings=None, slasher_event=None,
+                 n_flagged=None):
         self.slot, self.d_ok, self.d_head, self.d_agg_sig, self.event = slot, d_ok, d_head, d_agg_sig, event
         self.h_ok, self.h_head, self.h_agg_sig = h_ok, h_head, h_agg_sig
+        self._slashings, self.slasher_event, self._n_flagged = slashings, slasher_event, n_flagged
 
     def wait(self):
         self.event.synchronize()
@@ -54,6 +69,17 @@ class _Ticket:
         """bls.Aggregate's result for every committee of the epoch (uint8[n_agg, 96]); host tensor in the host form."""
         self.event.synchronize()
         return self.h_agg_sig.clone() if self.h_agg_sig is not None else self.d_agg_sig
+
+    def slashings(self) -> Slashings:
+        """The slasher's findings for this epoch (waits for its update, which runs after the head); EpochProcessor.enable_slasher first."""
+        assert self._slashings is not None, "no slasher: EpochProcessor.enable_slasher"
+        return self._slashings()
+
+    def n_flagged(self) -> int:
+        """Only the number of flagged member slots of this epoch (waits for the slasher's update; no kind or conflict copy)."""
+        assert self._slashings is not None, "no slasher: EpochProcessor.enable_slasher"
+        self.slasher_event.synchronize()
+        return self._n_flagged()
 
 
 class EpochProcessor:
@@ -117,6 +143,8 @@ class EpochProcessor:
         self.always_team = tail_form == "team"
         # ... except at the end of a batch: the last `team_last` epochs take the team form (see drain_hint)
         self.team_last = 1
+        self.slasher = False          # enable_slasher
+        self.ev_sl = [None] * S       # per slot: the slasher update of the epoch that last used the slot
 
     def set_committees(self, members, off):
         """members u32[n_sig] (committee order), off u32[n_agg+1] for the WHOLE epoch; signature j belongs to member j."""
@@ -129,10 +157,86 @@ class EpochProcessor:
         self.d_members_loc = self.d_members[self.m0:self.m1]
         self.d_off_loc = torch.as_tensor((off64[self.a0:self.a1 + 1] - off64[self.a0]).astype("int32"), device=self.dev)
         self.s_sigs = self._alloc_sig_slots(self.n_sig_loc)
+        self.h_members, self.h_off = np.asarray(members).astype(np.int64), off64
 
     def local_signatures(self, sigs):
         """The slice of an epoch's individual signatures (uint8[n_sig, 96], committee order) this rank aggregates."""
         return sigs[self.m0:self.m1]
+
+    # ------------------------------------------------------------------ slashing detection
+    def enable_slasher(self, history_epochs: int, max_attestations_per_target: int = None, current_epoch: int = 0):
+        """Detect the double and surround votes of every accepted aggregate of every epoch processed from now on, against a history of
+        `history_epochs` epochs on the device (Engine.slasher_init; B2Error(B2_ENOMEM) without allocating when it does not fit).
+        Unsharded the history covers the whole registry; sharded, this rank's validators [v0, v1) only (6 * (v1 - v0) * H bytes).
+        max_attestations_per_target defaults to 2 * n_agg (at most 65535).  Every entry point then needs source_epoch (per aggregate)
+        and current_epoch (the slasher's window moves to it before the epoch's update).
+        The slasher is fed the epoch's signing roots as attestation roots, so it must not be shared with Spec.find_attester_slashings,
+        which feeds data roots, on the same Engine."""
+        n_val = self.n_val if self.n_val is not None else self.eng.n_validators
+        v0, v1 = (self.v0, self.v1) if self.sharded else (0, n_val)
+        K = min(2 * self.n_agg, 65535) if max_attestations_per_target is None else int(max_attestations_per_target)
+        self.eng.slasher_init(n_val, history_epochs, K, current_epoch, v_begin=v0, v_end=v1)
+        d, S, cuda = self.dev, self.depth, self.dev.type == "cuda"
+        self.s_src = [torch.zeros(self.n_agg, dtype=torch.int64, device=d) for _ in range(S)]
+        self.d_sl_status = [torch.zeros(self.n_agg, dtype=torch.int32, device=d) for _ in range(S)]
+        self.d_sl_kind = [torch.zeros(self.n_sig, dtype=torch.uint8, device=d) for _ in range(S)]
+        self.d_sl_conflict = [torch.zeros((self.n_sig, 2), dtype=torch.int32, device=d) for _ in range(S)]
+        self.d_sl_flagged = [torch.zeros(1, dtype=torch.int32, device=d) for _ in range(S)]
+        self.h_sl_status = [torch.zeros(self.n_agg, dtype=torch.int32, pin_memory=cuda) for _ in range(S)]
+        self.h_sl_flagged = [torch.zeros(1, dtype=torch.int32, pin_memory=cuda) for _ in range(S)]
+        self.sl_range = (v0, v1)
+        self._sync_host = False
+        self._sl_cur = self._sl_next = int(current_epoch)
+        self.slasher = True
+
+    def _slasher_args(self, source_epoch, current_epoch):
+        """checked on entry, before anything of the epoch is enqueued"""
+        if not self.slasher:
+            return
+        assert source_epoch is not None and current_epoch is not None, "the slasher is enabled: source_epoch and current_epoch are required"
+        assert self._sl_next <= int(current_epoch) < 0xffffffff, "the slasher's current epoch only moves forward and fits 32 bits"
+        self._sl_next = int(current_epoch)
+
+    def _slasher_update(self, slot, d_bits, d_msgs, d_source_epoch, d_target_epoch, current_epoch, host):
+        """On the current stream, after the epoch's verdicts and fork choice: move the window if the epoch moved, then record and check
+        ALL aggregates of the epoch with accept = the verdicts.  The roots are the epoch's signing roots, not the data roots the C ABI
+        names: only attestations with the same target are compared for a double vote, and compute_signing_root(data,
+        get_domain(DOMAIN_BEACON_ATTESTER, data.target.epoch)) uses one domain per target epoch on a chain, so two signing roots of one
+        target are equal exactly when the data roots are (up to SHA-256 collisions)."""
+        e = self.eng
+        if int(current_epoch) != self._sl_cur:
+            e.slasher_advance_dev(int(current_epoch))
+            self._sl_cur = int(current_epoch)
+        e.slasher_update_dev(self.d_members, self.d_off, d_bits, d_source_epoch, d_target_epoch, d_msgs, self.d_ok[slot], self.d_sl_status[slot],
+                             self.d_sl_kind[slot], self.d_sl_conflict[slot], self.d_sl_flagged[slot])
+        if host:
+            self.h_sl_status[slot].copy_(self.d_sl_status[slot], non_blocking=True)
+            self.h_sl_flagged[slot].copy_(self.d_sl_flagged[slot], non_blocking=True)
+
+    def _read_slashings(self, slot, host, event=None):
+        """the findings in slot `slot` as a Slashings tuple; kind and conflict targets cross to the host only when something was flagged"""
+        if event is not None:
+            event.synchronize()
+        elif self.dev.type == "cuda":
+            torch.cuda.current_stream().synchronize()
+        if host:
+            status, n = self.h_sl_status[slot].numpy().copy(), int(self.h_sl_flagged[slot][0])
+        else:
+            status, n = self.d_sl_status[slot].cpu().numpy(), int(self.d_sl_flagged[slot][0])
+        total = int(self.h_off[-1])
+        if n == 0:
+            none = np.zeros(0, dtype=np.int64)
+            return Slashings(status, none, none, none, np.zeros(0, np.uint8), np.zeros(0, np.uint32), np.zeros(0, np.uint32))
+        kind = self.d_sl_kind[slot][:total].cpu().numpy()
+        conflict = self.d_sl_conflict[slot][:total].cpu().numpy().view(np.uint32)
+        i = np.nonzero(kind)[0]
+        agg = np.searchsorted(self.h_off, i, side="right") - 1
+        return Slashings(status, agg, i - self.h_off[agg], self.h_members[i], kind[i], conflict[i, 0].copy(), conflict[i, 1].copy())
+
+    def slashings(self) -> Slashings:
+        """The slasher's findings for the last epoch of process_epoch_dev / process_epoch_host (synchronises the current stream)."""
+        assert self.slasher, "no slasher: enable_slasher"
+        return self._read_slashings(0, self._sync_host)
 
     # ------------------------------------------------------------------ the exchange + fork choice of one epoch
     def _rows(self, t):
@@ -196,8 +300,17 @@ class EpochProcessor:
             return self.d_out_loc[slot][:n * 96], self.d_out_loc[slot][n * 96:]
         return self.d_agg_sig[slot], self.d_ok[slot]
 
-    def process_epoch_dev(self, d_sigs, d_bits, d_msgs, d_target_epoch, d_block_idx, justified_idx=0, boost_idx=-1, boost_score=0):
-        """d_sigs: this rank's signatures (all of them when not sharded); every other array covers the whole epoch."""
+    def process_epoch_dev(self, d_sigs, d_bits, d_msgs, d_target_epoch, d_block_idx, justified_idx=0, boost_idx=-1, boost_score=0,
+                          source_epoch=None, current_epoch=None):
+        """d_sigs: this rank's signatures (all of them when not sharded); every other array covers the whole epoch.  With the slasher
+        on: source_epoch int64[n_agg] (device) and the current epoch; the findings are read with slashings()."""
+        self._slasher_args(source_epoch, current_epoch)
+        self._sync_host = False
+        return self._process_epoch_dev(d_sigs, d_bits, d_msgs, d_target_epoch, d_block_idx, justified_idx, boost_idx, boost_score,
+                                       source_epoch, current_epoch, False)
+
+    def _process_epoch_dev(self, d_sigs, d_bits, d_msgs, d_target_epoch, d_block_idx, justified_idx, boost_idx, boost_score,
+                           source_epoch, current_epoch, host):
         e = self.eng
         o_sig, o_ok = self._local_outputs(0)
         if self.sharded:
@@ -210,17 +323,26 @@ class EpochProcessor:
             e.fast_aggregate_verify_dev(self.d_members, self.d_off, d_bits, d_msgs, o_sig, o_ok)
             e.latest_messages_update_dev(self.d_members, self.d_off, d_bits, d_target_epoch, d_block_idx, o_ok)
         self._fork_choice(0, justified_idx, boost_idx, boost_score)
+        if self.slasher:
+            self._slasher_update(0, d_bits, d_msgs, source_epoch, d_target_epoch, current_epoch, host)
         return self.d_ok[0], self.d_head[0]
 
-    def process_epoch_host(self, h_sigs, h_bits, h_msgs, h_target_epoch, h_block_idx, justified_idx=0, boost_idx=-1, boost_score=0):
-        """Pinned host tensors in, (verdict bytes, head index) out on the host; returns when the epoch is done."""
+    def process_epoch_host(self, h_sigs, h_bits, h_msgs, h_target_epoch, h_block_idx, justified_idx=0, boost_idx=-1, boost_score=0,
+                           source_epoch=None, current_epoch=None):
+        """Pinned host tensors in, (verdict bytes, head index) out on the host; returns when the epoch is done.  With the slasher on:
+        source_epoch int64[n_agg] (pinned host) and the current epoch; the findings are read with slashings()."""
+        self._slasher_args(source_epoch, current_epoch)
+        self._sync_host = True
         s = 0
         self.s_sigs[s].copy_(h_sigs, non_blocking=True)
         self.s_bits[s].copy_(h_bits, non_blocking=True)
         self.s_msgs[s].copy_(h_msgs, non_blocking=True)
         self.s_epoch[s].copy_(h_target_epoch, non_blocking=True)
         self.s_blk[s].copy_(h_block_idx, non_blocking=True)
-        self.process_epoch_dev(self.s_sigs[s], self.s_bits[s], self.s_msgs[s], self.s_epoch[s], self.s_blk[s], justified_idx, boost_idx, boost_score)
+        if self.slasher:
+            self.s_src[s].copy_(source_epoch, non_blocking=True)
+        self._process_epoch_dev(self.s_sigs[s], self.s_bits[s], self.s_msgs[s], self.s_epoch[s], self.s_blk[s], justified_idx, boost_idx, boost_score,
+                                self.s_src[s] if self.slasher else None, current_epoch, True)
         self.h_ok[s].copy_(self.d_ok[0], non_blocking=True)
         self.h_head[s].copy_(self.d_head[0], non_blocking=True)
         self.h_agg_sig[s].copy_(self.d_agg_sig[0], non_blocking=True)
@@ -228,7 +350,7 @@ class EpochProcessor:
         return self.h_ok[s], int(self.h_head[s][0])
 
     # ------------------------------------------------------------------ pipelined form
-    def _submit(self, slot, d_sigs, d_bits, d_msgs, fc, host, last=False):
+    def _submit(self, slot, d_sigs, d_bits, d_msgs, fc, host, last=False, current_epoch=None):
         e = self.eng
         team = last or self.always_team
         if team != self._team_form:                       # last epoch of a batch: nothing will overlap its tail, so take the short form
@@ -253,10 +375,20 @@ class EpochProcessor:
                 self.h_agg_sig[slot].copy_(self.d_agg_sig[slot], non_blocking=True)
             ev = torch.cuda.Event()
             ev.record()
+            ev_sl = None
+            if self.slasher:                              # after the head: the head's latency does not include it
+                self._slasher_update(slot, self.s_bits[slot], self.s_msgs[slot], self.s_src[slot], self.s_epoch[slot], current_epoch, host)
+                ev_sl = torch.cuda.Event()
+                ev_sl.record()
         self.ev_fc[slot] = ev
+        self.ev_sl[slot] = ev_sl
+        report = count = None
+        if ev_sl is not None:
+            report = lambda s=slot, h=host, x=ev_sl: self._read_slashings(s, h, x)                                    # noqa: E731
+            count = lambda s=slot, h=host: int((self.h_sl_flagged if h else self.d_sl_flagged)[s][0])              # noqa: E731
         self._inflight.append(_Ticket(slot, self.d_ok[slot], self.d_head[slot], self.d_agg_sig[slot], ev,
                                       self.h_ok[slot] if host else None, self.h_head[slot] if host else None,
-                                      self.h_agg_sig[slot] if host else None))
+                                      self.h_agg_sig[slot] if host else None, report, ev_sl, count))
         self.k += 1
         return self._inflight.popleft() if len(self._inflight) >= self.depth else None
 
@@ -266,6 +398,8 @@ class EpochProcessor:
         self.eng.epoch_wait_dev(slot)                     # (on the current stream == `stream`)
         if self.ev_fc[slot] is not None:
             stream.wait_event(self.ev_fc[slot])
+        if self.ev_sl[slot] is not None:                  # the slasher read the slot's bits, messages, epochs and verdicts
+            stream.wait_event(self.ev_sl[slot])
         return slot
 
     def drain_hint(self, remaining: int) -> bool:
@@ -273,19 +407,29 @@ class EpochProcessor:
         of a batch cannot hide a thread-form tail (≈ 30 ms) behind decompressions that are no longer coming."""
         return remaining < self.team_last
 
-    def submit_dev(self, d_sigs, d_bits, d_msgs, d_target_epoch, d_block_idx, justified_idx=0, boost_idx=-1, boost_score=0, last=False):
+    def submit_dev(self, d_sigs, d_bits, d_msgs, d_target_epoch, d_block_idx, justified_idx=0, boost_idx=-1, boost_score=0, last=False,
+                   source_epoch=None, current_epoch=None):
         """Enqueue one epoch (device-resident inputs, which must stay untouched until its ticket has been waited for; d_sigs =
         this rank's signatures, the other arrays cover the whole epoch).  Returns the ticket of the epoch submitted depth-1
         calls earlier (None while the pipeline fills).  `last=True` says no further epoch follows soon: its pairing tail is
-        enqueued in the short-critical-path (team) form."""
+        enqueued in the short-critical-path (team) form.  With the slasher on: source_epoch int64[n_agg] (device) and the
+        current epoch; the slasher reads copies of the bits, messages and epochs, so the inputs are free after wait() as without it."""
+        self._slasher_args(source_epoch, current_epoch)
         slot = self._claim_slot(torch.cuda.current_stream())
         self.s_epoch[slot].copy_(d_target_epoch)
         self.s_blk[slot].copy_(d_block_idx)
-        return self._submit(slot, d_sigs, d_bits, d_msgs, (justified_idx, boost_idx, boost_score), False, last)
+        if self.slasher:
+            self.s_bits[slot].copy_(d_bits)
+            self.s_msgs[slot].copy_(d_msgs)
+            self.s_src[slot].copy_(source_epoch)
+        return self._submit(slot, d_sigs, d_bits, d_msgs, (justified_idx, boost_idx, boost_score), False, last, current_epoch)
 
-    def submit_host(self, h_sigs, h_bits, h_msgs, h_target_epoch, h_block_idx, justified_idx=0, boost_idx=-1, boost_score=0, last=False):
+    def submit_host(self, h_sigs, h_bits, h_msgs, h_target_epoch, h_block_idx, justified_idx=0, boost_idx=-1, boost_score=0, last=False,
+                    source_epoch=None, current_epoch=None):
         """Pinned host tensors in (untouched until the returned-later ticket has been waited for).  The H2D copies go on a
-        separate stream so that they overlap with the epochs in flight."""
+        separate stream so that they overlap with the epochs in flight.  With the slasher on: source_epoch int64[n_agg] (pinned
+        host) and the current epoch; the status and flagged count of every epoch come back in pinned buffers."""
+        self._slasher_args(source_epoch, current_epoch)
         cur = torch.cuda.current_stream()
         with torch.cuda.stream(self.copy_stream):
             slot = self._claim_slot(self.copy_stream)
@@ -294,25 +438,32 @@ class EpochProcessor:
             self.s_msgs[slot].copy_(h_msgs, non_blocking=True)
             self.s_epoch[slot].copy_(h_target_epoch, non_blocking=True)
             self.s_blk[slot].copy_(h_block_idx, non_blocking=True)
+            if self.slasher:
+                self.s_src[slot].copy_(source_epoch, non_blocking=True)
             ev = torch.cuda.Event()
             ev.record()
         cur.wait_event(ev)
-        return self._submit(slot, self.s_sigs[slot], self.s_bits[slot], self.s_msgs[slot], (justified_idx, boost_idx, boost_score), True, last)
+        return self._submit(slot, self.s_sigs[slot], self.s_bits[slot], self.s_msgs[slot], (justified_idx, boost_idx, boost_score), True, last,
+                            current_epoch)
 
     def drain(self):
-        """Tickets of the epochs still in flight, oldest first; the current stream waits for all of them."""
+        """Tickets of the epochs still in flight, oldest first; the current stream waits for all of them (their slasher updates included)."""
         out = list(self._inflight)
         self._inflight.clear()
         for t in out:
             torch.cuda.current_stream().wait_event(t.event)
+            if t.slasher_event is not None:
+                torch.cuda.current_stream().wait_event(t.slasher_event)
         return out
 
     @property
     def h2d_bytes(self):
         """host -> device bytes per epoch of this rank (submit_host): its signatures + the epoch's bits, messages, epochs, blocks"""
-        return (self.s_sigs[0].numel() + self.s_bits[0].numel() + self.s_msgs[0].numel() + 8 * self.s_epoch[0].numel() + 4 * self.s_blk[0].numel())
+        return (self.s_sigs[0].numel() + self.s_bits[0].numel() + self.s_msgs[0].numel() + 8 * self.s_epoch[0].numel() + 4 * self.s_blk[0].numel()
+                + (8 * self.n_agg if self.slasher else 0))
 
     @property
     def d2h_bytes(self):
-        """device -> host bytes per epoch (submit_host): verdicts + head index + the aggregate signatures"""
-        return self.h_ok[0].numel() + 4 + self.h_agg_sig[0].numel()
+        """device -> host bytes per epoch (submit_host): verdicts + head index + the aggregate signatures (+ the slasher's statuses and
+        flagged count; its kind and conflict targets only when something was flagged)"""
+        return self.h_ok[0].numel() + 4 + self.h_agg_sig[0].numel() + ((4 * self.n_agg + 4) if self.slasher else 0)

@@ -12,7 +12,7 @@ cd "$(dirname "$0")/.."
 OUT="${OUT:-$(mktemp -d)}"
 mkdir -p "$OUT"
 SAN=/usr/local/cuda/bin/compute-sanitizer
-SMALL="tests/test_gpu_bls.py tests/test_gpu_bls_adversarial.py tests/test_gpu_aggregate_verify.py tests/test_gpu_sync_aggregate.py tests/test_gpu_forkchoice.py tests/test_gpu_gather.py tests/test_gpu_participation.py tests/test_gpu_epoch.py tests/test_gpu_slasher.py"
+SMALL="tests/test_gpu_bls.py tests/test_gpu_bls_adversarial.py tests/test_gpu_aggregate_verify.py tests/test_gpu_sync_aggregate.py tests/test_gpu_forkchoice.py tests/test_gpu_gather.py tests/test_gpu_participation.py tests/test_gpu_epoch.py tests/test_gpu_slasher.py tests/test_gpu_epoch_slasher.py"
 RACE="tests/test_gpu_bls.py::test_fast_aggregate_verify_vs_oracle tests/test_gpu_bls.py::test_g1_aggregate_all_minimal_committees tests/test_gpu_forkchoice.py tests/test_gpu_gather.py"
 run() {  # name, timeout, command...
     local name=$1 tmo=$2; shift 2
