@@ -15,6 +15,8 @@ Two ways to drive it:
     high-priority streams inside the library) and with their fork choice (on this object's fork-choice stream); in the
     host form the H2D copy of epoch k+1 overlaps too.  `submit_*` returns the ticket of the epoch submitted depth-1
     calls earlier.
+The synchronous forms and `get_head` use slot 0 and the one vote accumulator of the pipeline, so they need it drained: while
+submitted epochs are in flight (until `drain()` has returned) they raise AssertionError before enqueueing anything.
 
 Multi-GPU, two layouts (SURVEY.md section 8e):
   * `shard=None` (weak scaling): every rank owns its OWN validator set and epoch; the only exchange is the u64[n_blocks]
@@ -33,6 +35,7 @@ member slots.  Sharded, rank g holds the history of validators [g*N/world, (g+1)
 and reports those; the ranks' reports together are the unsharded one, with no collective added.
 """
 import collections
+import contextlib
 
 import numpy as np
 import torch
@@ -49,37 +52,65 @@ flagged member slot: aggregate index, position in the committee, validator index
 (0xffffffff where that bit is clear).  A conflicting target names the epoch batch that holds the partner attestation."""
 
 
+class _Slot:
+    """Everything one epoch in flight owns (slot i of the pipeline; the synchronous forms use slot 0)."""
+
+    def __init__(self, i, ep):
+        z, h, n_agg = ep._zeros, ep._pinned, ep.n_agg
+        self.i = i
+        # staged inputs (EpochProcessor._stage); set_committees sizes the signatures, enable_slasher adds the source epochs
+        self.sigs = self.src = None
+        self.bits, self.msgs = z((n_agg, ep.bits_stride), torch.uint8), z((n_agg, 32), torch.uint8)
+        self.tgt, self.blk = z(n_agg, torch.int64), z(n_agg, torch.int32)
+        # device outputs
+        self.agg_sig, self.agg_status = z((n_agg, 96), torch.uint8), z(ep.n_loc, torch.int32)
+        self.ok, self.head = z(n_agg, torch.uint8), z(1, torch.int32)
+        if ep.sharded:
+            # this rank's outputs packed for ONE all-gather per epoch: n_loc aggregate signatures, then n_loc verdict bytes
+            self.out_loc, self.out_all = z(ep.n_loc * 97, torch.uint8), z((ep.world, ep.n_loc * 97), torch.uint8)
+        # pinned host readback
+        self.h_ok, self.h_head, self.h_agg_sig = h(n_agg, torch.uint8), h(1, torch.int32), h((n_agg, 96), torch.uint8)
+        # pipelined forms: the fork choice (+ D2H) and the slasher update of the epoch that last used the slot
+        self.ev_fc = self.ev_sl = None
+
+    def enable_slasher(self, ep):
+        z, h = ep._zeros, ep._pinned
+        self.src = z(ep.n_agg, torch.int64)
+        self.sl_status, self.sl_kind = z(ep.n_agg, torch.int32), z(ep.n_sig, torch.uint8)
+        self.sl_conflict, self.sl_flagged = z((ep.n_sig, 2), torch.int32), z(1, torch.int32)
+        self.h_sl_status, self.h_sl_flagged = h(ep.n_agg, torch.int32), h(1, torch.int32)
+
+
 class _Ticket:
     """Result of one submitted epoch: verdict bytes + head index (+ the aggregate signatures), valid after .wait() and until
     `depth` further epochs have been submitted; with the slasher on, also its findings (.slashings())."""
 
-    def __init__(self, slot, d_ok, d_head, d_agg_sig, event, h_ok=None, h_head=None, h_agg_sig=None, slashings=None, slasher_event=None,
-                 n_flagged=None):
-        self.slot, self.d_ok, self.d_head, self.d_agg_sig, self.event = slot, d_ok, d_head, d_agg_sig, event
-        self.h_ok, self.h_head, self.h_agg_sig = h_ok, h_head, h_agg_sig
-        self._slashings, self.slasher_event, self._n_flagged = slashings, slasher_event, n_flagged
+    def __init__(self, ep, slot, host):
+        self._ep, self._slot, self._host = ep, slot, host
+        self.slot = slot.i                                # the pipeline slot the epoch ran in (EpochProcessor.d_agg_status[slot])
+        self.d_agg_sig, self.event, self.slasher_event = slot.agg_sig, slot.ev_fc, slot.ev_sl
 
     def wait(self):
         self.event.synchronize()
-        if self.h_ok is not None:
-            return self.h_ok.clone(), int(self.h_head[0])
-        return self.d_ok, int(self.d_head[0])
+        if self._host:
+            return self._slot.h_ok.clone(), int(self._slot.h_head[0])
+        return self._slot.ok, int(self._slot.head[0])
 
     def aggregate_signatures(self):
         """bls.Aggregate's result for every committee of the epoch (uint8[n_agg, 96]); host tensor in the host form."""
         self.event.synchronize()
-        return self.h_agg_sig.clone() if self.h_agg_sig is not None else self.d_agg_sig
+        return self._slot.h_agg_sig.clone() if self._host else self.d_agg_sig
 
     def slashings(self) -> Slashings:
         """The slasher's findings for this epoch (waits for its update, which runs after the head); EpochProcessor.enable_slasher first."""
-        assert self._slashings is not None, "no slasher: EpochProcessor.enable_slasher"
-        return self._slashings()
+        assert self.slasher_event is not None, "no slasher: EpochProcessor.enable_slasher"
+        return self._ep._read_slashings(self._slot, self._host, self.slasher_event)
 
     def n_flagged(self) -> int:
         """Only the number of flagged member slots of this epoch (waits for the slasher's update; no kind or conflict copy)."""
-        assert self._slashings is not None, "no slasher: EpochProcessor.enable_slasher"
+        assert self.slasher_event is not None, "no slasher: EpochProcessor.enable_slasher"
         self.slasher_event.synchronize()
-        return self._n_flagged()
+        return int((self._slot.h_sl_flagged if self._host else self._slot.sl_flagged)[0])
 
 
 class EpochProcessor:
@@ -93,10 +124,9 @@ class EpochProcessor:
         self.dev = device if device is not None else torch.device("cuda", engine.device)
         self.pg = process_group
         self.n_agg, self.n_sig, self.n_blocks, self.bits_stride = n_agg, n_sig, n_blocks, bits_stride
-        d = self.dev
         cuda = self.dev.type == "cuda"
         assert 2 <= depth <= MAX_DEPTH, "depth must be 2..B2_EPOCH_SLOTS"
-        self.depth = S = depth
+        self.depth = depth
         if shard is not None:
             self.rank, self.world = int(shard[0]), int(shard[1])
             assert 0 <= self.rank < self.world and n_agg % self.world == 0, "aggregates must divide evenly over the ranks"
@@ -109,30 +139,15 @@ class EpochProcessor:
         self.n_loc = self.a1 - self.a0
         if self.sharded:
             self.v0, self.v1 = self.rank * n_validators // self.world, (self.rank + 1) * n_validators // self.world
-        z = lambda shape, dt: torch.zeros(shape, dtype=dt, device=d)            # noqa: E731
-        self.d_agg_sig = [z((n_agg, 96), torch.uint8) for _ in range(S)]
-        self.d_agg_status = [z(self.n_loc, torch.int32) for _ in range(S)]
-        self.d_ok = [z(n_agg, torch.uint8) for _ in range(S)]
-        self.d_head = [z(1, torch.int32) for _ in range(S)]
-        self.d_votes = z(n_blocks, torch.int64)
-        if self.sharded:
-            # per-rank outputs packed for ONE all-gather per epoch: n_loc aggregate signatures, then n_loc verdict bytes
-            self.d_out_loc = [z(self.n_loc * 97, torch.uint8) for _ in range(S)]
-            self.d_out_all = [z((self.world, self.n_loc * 97), torch.uint8) for _ in range(S)]
-        # per-slot copies of everything the asynchronous tail / side streams read, and staging for the host entry points
+        self.d_votes = self._zeros(n_blocks, torch.int64)
         self.n_sig_loc = None        # set by set_committees
-        self._alloc_sig_slots = lambda n: [z((n, 96), torch.uint8) for _ in range(S)]       # noqa: E731
-        self.s_sigs = None
-        self.s_bits = [z((n_agg, bits_stride), torch.uint8) for _ in range(S)]
-        self.s_msgs = [z((n_agg, 32), torch.uint8) for _ in range(S)]
-        self.s_epoch = [z(n_agg, torch.int64) for _ in range(S)]
-        self.s_blk = [z(n_agg, torch.int32) for _ in range(S)]
-        self.h_ok = [torch.zeros(n_agg, dtype=torch.uint8, pin_memory=cuda) for _ in range(S)]
-        self.h_head = [torch.zeros(1, dtype=torch.int32, pin_memory=cuda) for _ in range(S)]
-        self.h_agg_sig = [torch.zeros((n_agg, 96), dtype=torch.uint8, pin_memory=cuda) for _ in range(S)]
-        self.copy_stream = torch.cuda.Stream(device=d) if cuda else None
-        self.fc_stream = torch.cuda.Stream(device=d) if cuda else None
-        self.ev_fc = [None] * S       # per slot: fork choice (+ D2H) of the epoch that last used the slot
+        self.slots = [_Slot(i, self) for i in range(depth)]
+        # each slot's aggregate signatures and bls.Aggregate statuses, indexed by slot (Ticket.slot); the slots' own tensors
+        self.d_agg_sig = [s.agg_sig for s in self.slots]
+        self.h_agg_sig = [s.h_agg_sig for s in self.slots]
+        self.d_agg_status = [s.agg_status for s in self.slots]
+        self.copy_stream = torch.cuda.Stream(device=self.dev) if cuda else None
+        self.fc_stream = torch.cuda.Stream(device=self.dev) if cuda else None
         self.k = 0
         self._inflight = collections.deque()      # tickets of the submitted, not yet returned epochs
         self._team_form = False
@@ -144,7 +159,12 @@ class EpochProcessor:
         # ... except at the end of a batch: the last `team_last` epochs take the team form (see drain_hint)
         self.team_last = 1
         self.slasher = False          # enable_slasher
-        self.ev_sl = [None] * S       # per slot: the slasher update of the epoch that last used the slot
+
+    def _zeros(self, shape, dtype):
+        return torch.zeros(shape, dtype=dtype, device=self.dev)
+
+    def _pinned(self, shape, dtype):
+        return torch.zeros(shape, dtype=dtype, pin_memory=self.dev.type == "cuda")
 
     def set_committees(self, members, off):
         """members u32[n_sig] (committee order), off u32[n_agg+1] for the WHOLE epoch; signature j belongs to member j."""
@@ -156,7 +176,8 @@ class EpochProcessor:
         # this rank's rows: members of its aggregates and offsets relative to its first member
         self.d_members_loc = self.d_members[self.m0:self.m1]
         self.d_off_loc = torch.as_tensor((off64[self.a0:self.a1 + 1] - off64[self.a0]).astype("int32"), device=self.dev)
-        self.s_sigs = self._alloc_sig_slots(self.n_sig_loc)
+        for s in self.slots:
+            s.sigs = self._zeros((self.n_sig_loc, 96), torch.uint8)
         self.h_members, self.h_off = np.asarray(members).astype(np.int64), off64
 
     def local_signatures(self, sigs):
@@ -176,16 +197,9 @@ class EpochProcessor:
         v0, v1 = (self.v0, self.v1) if self.sharded else (0, n_val)
         K = min(2 * self.n_agg, 65535) if max_attestations_per_target is None else int(max_attestations_per_target)
         self.eng.slasher_init(n_val, history_epochs, K, current_epoch, v_begin=v0, v_end=v1)
-        d, S, cuda = self.dev, self.depth, self.dev.type == "cuda"
-        self.s_src = [torch.zeros(self.n_agg, dtype=torch.int64, device=d) for _ in range(S)]
-        self.d_sl_status = [torch.zeros(self.n_agg, dtype=torch.int32, device=d) for _ in range(S)]
-        self.d_sl_kind = [torch.zeros(self.n_sig, dtype=torch.uint8, device=d) for _ in range(S)]
-        self.d_sl_conflict = [torch.zeros((self.n_sig, 2), dtype=torch.int32, device=d) for _ in range(S)]
-        self.d_sl_flagged = [torch.zeros(1, dtype=torch.int32, device=d) for _ in range(S)]
-        self.h_sl_status = [torch.zeros(self.n_agg, dtype=torch.int32, pin_memory=cuda) for _ in range(S)]
-        self.h_sl_flagged = [torch.zeros(1, dtype=torch.int32, pin_memory=cuda) for _ in range(S)]
+        for s in self.slots:
+            s.enable_slasher(self)
         self.sl_range = (v0, v1)
-        self._sync_host = False
         self._sl_cur = self._sl_next = int(current_epoch)
         self.slasher = True
 
@@ -197,7 +211,7 @@ class EpochProcessor:
         assert self._sl_next <= int(current_epoch) < 0xffffffff, "the slasher's current epoch only moves forward and fits 32 bits"
         self._sl_next = int(current_epoch)
 
-    def _slasher_update(self, slot, d_bits, d_msgs, d_source_epoch, d_target_epoch, current_epoch, host):
+    def _slasher_update(self, s, d_bits, d_msgs, d_source_epoch, d_target_epoch, current_epoch, host):
         """On the current stream, after the epoch's verdicts and fork choice: move the window if the epoch moved, then record and check
         ALL aggregates of the epoch with accept = the verdicts.  The roots are the epoch's signing roots, not the data roots the C ABI
         names: only attestations with the same target are compared for a double vote, and compute_signing_root(data,
@@ -207,28 +221,28 @@ class EpochProcessor:
         if int(current_epoch) != self._sl_cur:
             e.slasher_advance_dev(int(current_epoch))
             self._sl_cur = int(current_epoch)
-        e.slasher_update_dev(self.d_members, self.d_off, d_bits, d_source_epoch, d_target_epoch, d_msgs, self.d_ok[slot], self.d_sl_status[slot],
-                             self.d_sl_kind[slot], self.d_sl_conflict[slot], self.d_sl_flagged[slot])
+        e.slasher_update_dev(self.d_members, self.d_off, d_bits, d_source_epoch, d_target_epoch, d_msgs, s.ok, s.sl_status, s.sl_kind,
+                             s.sl_conflict, s.sl_flagged)
         if host:
-            self.h_sl_status[slot].copy_(self.d_sl_status[slot], non_blocking=True)
-            self.h_sl_flagged[slot].copy_(self.d_sl_flagged[slot], non_blocking=True)
+            s.h_sl_status.copy_(s.sl_status, non_blocking=True)
+            s.h_sl_flagged.copy_(s.sl_flagged, non_blocking=True)
 
-    def _read_slashings(self, slot, host, event=None):
-        """the findings in slot `slot` as a Slashings tuple; kind and conflict targets cross to the host only when something was flagged"""
+    def _read_slashings(self, s, host, event=None):
+        """the findings in slot s as a Slashings tuple; kind and conflict targets cross to the host only when something was flagged"""
         if event is not None:
             event.synchronize()
         elif self.dev.type == "cuda":
             torch.cuda.current_stream().synchronize()
         if host:
-            status, n = self.h_sl_status[slot].numpy().copy(), int(self.h_sl_flagged[slot][0])
+            status, n = s.h_sl_status.numpy().copy(), int(s.h_sl_flagged[0])
         else:
-            status, n = self.d_sl_status[slot].cpu().numpy(), int(self.d_sl_flagged[slot][0])
+            status, n = s.sl_status.cpu().numpy(), int(s.sl_flagged[0])
         total = int(self.h_off[-1])
         if n == 0:
             none = np.zeros(0, dtype=np.int64)
             return Slashings(status, none, none, none, np.zeros(0, np.uint8), np.zeros(0, np.uint32), np.zeros(0, np.uint32))
-        kind = self.d_sl_kind[slot][:total].cpu().numpy()
-        conflict = self.d_sl_conflict[slot][:total].cpu().numpy().view(np.uint32)
+        kind = s.sl_kind[:total].cpu().numpy()
+        conflict = s.sl_conflict[:total].cpu().numpy().view(np.uint32)
         i = np.nonzero(kind)[0]
         agg = np.searchsorted(self.h_off, i, side="right") - 1
         return Slashings(status, agg, i - self.h_off[agg], self.h_members[i], kind[i], conflict[i, 0].copy(), conflict[i, 1].copy())
@@ -236,26 +250,22 @@ class EpochProcessor:
     def slashings(self) -> Slashings:
         """The slasher's findings for the last epoch of process_epoch_dev / process_epoch_host (synchronises the current stream)."""
         assert self.slasher, "no slasher: enable_slasher"
-        return self._read_slashings(0, self._sync_host)
+        return self._read_slashings(self.slots[0], False)
 
     # ------------------------------------------------------------------ the exchange + fork choice of one epoch
-    def _rows(self, t):
-        return t[self.a0:self.a1]
-
-    def _exchange(self, slot, d_bits, d_target_epoch, d_block_idx):
+    def _exchange(self, s, d_bits, d_target_epoch, d_block_idx):
         """Sharded epoch, after the local tail: all-gather (aggregate signature, verdict) of every rank's aggregates, then
         update_latest_messages for ALL accepted aggregates of the epoch on this rank's replica of the LMD table."""
         n = self.n_loc
-        loc, allr = self.d_out_loc[slot], self.d_out_all[slot]
         if self.pg is None:                           # one rank of a sharded epoch on its own (bench.py --emulate-world): no peers to gather from
-            allr[self.rank].copy_(loc)
+            s.out_all[self.rank].copy_(s.out_loc)
         else:
-            torch.distributed.all_gather_into_tensor(allr.view(-1), loc, group=self.pg)
-        self.d_agg_sig[slot].view(self.world, n * 96).copy_(allr[:, :n * 96])
-        self.d_ok[slot].view(self.world, n).copy_(allr[:, n * 96:])
-        self.eng.latest_messages_update_dev(self.d_members, self.d_off, d_bits, d_target_epoch, d_block_idx, self.d_ok[slot])
+            torch.distributed.all_gather_into_tensor(s.out_all.view(-1), s.out_loc, group=self.pg)
+        s.agg_sig.view(self.world, n * 96).copy_(s.out_all[:, :n * 96])
+        s.ok.view(self.world, n).copy_(s.out_all[:, n * 96:])
+        self.eng.latest_messages_update_dev(self.d_members, self.d_off, d_bits, d_target_epoch, d_block_idx, s.ok)
 
-    def _fork_choice(self, slot, justified_idx, boost_idx, boost_score):
+    def _fork_choice(self, s, justified_idx, boost_idx, boost_score):
         e = self.eng
         if self.sharded:
             e.vote_weights_range_dev(self.v0, self.v1, self.d_votes)
@@ -263,7 +273,7 @@ class EpochProcessor:
             e.vote_weights_dev(self.d_votes)
         if self.pg is not None and torch.distributed.get_world_size(self.pg) > 1:
             torch.distributed.all_reduce(self.d_votes, group=self.pg)
-        e.head_from_votes_dev(self.d_votes, self.d_head[slot], justified_idx, boost_idx, boost_score)
+        e.head_from_votes_dev(self.d_votes, s.head, justified_idx, boost_idx, boost_score)
 
     def enable_fused_get_head(self):
         """Sharded mode: set up get_head as ONE kernel per rank with the vote all-reduce fused in over NVLink peer memory
@@ -284,123 +294,121 @@ class EpochProcessor:
         """get_head over the current LMD table through the multi-rank path; returns the head index on the host.  COLLECTIVE.
         fused (default: whether enable_fused_get_head was called): one kernel per rank -- vote scatter of this rank's validators,
         64-bit reductions into every rank's accumulator over NVLink, flag exchange, tree phase, zero-copy result.  Otherwise the
-        three-stage form: scatter kernel, NCCL all-reduce of u64[n_blocks], tree kernel, device-to-host copy."""
+        three-stage form: scatter kernel, NCCL all-reduce of u64[n_blocks], tree kernel, device-to-host copy.  Needs a drained pipeline."""
+        assert not self._inflight, "submitted epochs are in flight: drain() first"
         if fused is None:
             fused = getattr(self, "_fused_head", False)
         if fused:
             return self.eng.get_head_multi(self.v0, self.v1, justified_idx, boost_idx, boost_score)
-        self._fork_choice(0, justified_idx, boost_idx, boost_score)
-        return int(self.d_head[0].item())
+        self._fork_choice(self.slots[0], justified_idx, boost_idx, boost_score)
+        return int(self.slots[0].head.item())
+
+    # ------------------------------------------------------------------ one epoch, both forms
+    def _stage(self, s, host, sigs, bits, msgs, tgt, blk, src):
+        """Copy an epoch's inputs into slot s on the current stream; returns (sigs, bits, msgs, tgt, blk, src) with each copied array
+        replaced by the slot's.  From the host everything is copied.  From the device only what the asynchronous tail reads after
+        the call has returned: the target epochs and block indices of the LMD update (a caller may rewrite them for the next epoch),
+        and with the slasher the bits, messages and source epochs, which its update reads after the ticket's event."""
+        def put(buf, a):
+            buf.copy_(a, non_blocking=True)
+            return buf
+        if host:
+            sigs, bits, msgs = put(s.sigs, sigs), put(s.bits, bits), put(s.msgs, msgs)
+        tgt, blk = put(s.tgt, tgt), put(s.blk, blk)
+        if self.slasher:
+            if not host:
+                bits, msgs = put(s.bits, bits), put(s.msgs, msgs)
+            src = put(s.src, src)
+        return sigs, bits, msgs, tgt, blk, src
+
+    @staticmethod
+    def _record():
+        ev = torch.cuda.Event()
+        ev.record()
+        return ev
+
+    def _epoch(self, s, x, fc, host, current_epoch, pipelined, last=False):
+        """The epoch of slot s with inputs x = (sigs, bits, msgs, tgt, blk, src): verify, exchange (sharded), fork choice (fc =
+        justified_idx, boost_idx, boost_score), host readback (host), slasher update.  Synchronous: Engine.epoch_dev and the rest on the
+        current stream.  Pipelined: epoch_start_dev / epoch_tail_dev on the current stream, then the rest on the fork-choice stream
+        after epoch_wait_dev, enqueued BEFORE the next epoch's tail (whose LMD update waits for this scatter), recording the slot's
+        events."""
+        e = self.eng
+        sigs, bits, msgs, tgt, blk, src = x
+        if self.sharded:                                  # this rank's aggregates; their LMD update waits for the exchange
+            n = self.n_loc
+            members, off, v_bits, v_msgs, v_tgt, v_blk = self.d_members_loc, self.d_off_loc, bits[self.a0:self.a1], msgs[self.a0:self.a1], None, None
+            o_sig, o_ok = s.out_loc[:n * 96], s.out_loc[n * 96:]
+        else:
+            members, off, v_bits, v_msgs, v_tgt, v_blk = self.d_members, self.d_off, bits, msgs, tgt, blk
+            o_sig, o_ok = s.agg_sig, s.ok
+        if pipelined:
+            team = last or self.always_team
+            if team != self._team_form:                   # last epoch of a batch: nothing will overlap its tail, so take the short form
+                e.epoch_set_pairing_form(team)
+                self._team_form = team
+            e.epoch_start_dev(s.i, sigs, members, off, v_bits, v_msgs, s.agg_status)
+            e.epoch_tail_dev(s.i, members, off, v_bits, v_tgt, v_blk, o_sig, s.agg_status, o_ok)
+        else:
+            e.epoch_dev(sigs, members, off, v_bits, v_msgs, v_tgt, v_blk, o_sig, s.agg_status, o_ok)
+        with torch.cuda.stream(self.fc_stream) if pipelined else contextlib.nullcontext():
+            if pipelined:
+                e.epoch_wait_dev(s.i)
+            if self.sharded:
+                self._exchange(s, bits, tgt, blk)
+            self._fork_choice(s, *fc)
+            if host:
+                s.h_ok.copy_(s.ok, non_blocking=True)
+                s.h_head.copy_(s.head, non_blocking=True)
+                s.h_agg_sig.copy_(s.agg_sig, non_blocking=True)
+            if pipelined:
+                s.ev_fc = self._record()
+            if self.slasher:                              # after the head: the head's latency does not include it
+                self._slasher_update(s, bits, msgs, src, tgt, current_epoch, host)
+                if pipelined:
+                    s.ev_sl = self._record()
 
     # ------------------------------------------------------------------ synchronous form
-    def _local_outputs(self, slot):
-        """(aggregate-signature rows, verdict rows) the library writes for this rank's aggregates."""
-        if self.sharded:
-            n = self.n_loc
-            return self.d_out_loc[slot][:n * 96], self.d_out_loc[slot][n * 96:]
-        return self.d_agg_sig[slot], self.d_ok[slot]
-
     def process_epoch_dev(self, d_sigs, d_bits, d_msgs, d_target_epoch, d_block_idx, justified_idx=0, boost_idx=-1, boost_score=0,
                           source_epoch=None, current_epoch=None):
         """d_sigs: this rank's signatures (all of them when not sharded); every other array covers the whole epoch.  With the slasher
-        on: source_epoch int64[n_agg] (device) and the current epoch; the findings are read with slashings()."""
+        on: source_epoch int64[n_agg] (device) and the current epoch; the findings are read with slashings().  Needs a drained pipeline."""
+        assert not self._inflight, "submitted epochs are in flight: drain() first"
         self._slasher_args(source_epoch, current_epoch)
-        self._sync_host = False
-        return self._process_epoch_dev(d_sigs, d_bits, d_msgs, d_target_epoch, d_block_idx, justified_idx, boost_idx, boost_score,
-                                       source_epoch, current_epoch, False)
-
-    def _process_epoch_dev(self, d_sigs, d_bits, d_msgs, d_target_epoch, d_block_idx, justified_idx, boost_idx, boost_score,
-                           source_epoch, current_epoch, host):
-        e = self.eng
-        o_sig, o_ok = self._local_outputs(0)
-        if self.sharded:
-            e.epoch_dev(d_sigs, self.d_members_loc, self.d_off_loc, self._rows(d_bits), self._rows(d_msgs), None, None, o_sig, self.d_agg_status[0], o_ok)
-            self._exchange(0, d_bits, d_target_epoch, d_block_idx)
-        elif hasattr(e, "epoch_dev"):
-            e.epoch_dev(d_sigs, self.d_members, self.d_off, d_bits, d_msgs, d_target_epoch, d_block_idx, o_sig, self.d_agg_status[0], o_ok)
-        else:                                           # engines without the fused entry point (tests' stand-ins)
-            e.aggregate_dev(d_sigs, self.d_off, o_sig, self.d_agg_status[0])
-            e.fast_aggregate_verify_dev(self.d_members, self.d_off, d_bits, d_msgs, o_sig, o_ok)
-            e.latest_messages_update_dev(self.d_members, self.d_off, d_bits, d_target_epoch, d_block_idx, o_ok)
-        self._fork_choice(0, justified_idx, boost_idx, boost_score)
-        if self.slasher:
-            self._slasher_update(0, d_bits, d_msgs, source_epoch, d_target_epoch, current_epoch, host)
-        return self.d_ok[0], self.d_head[0]
+        s = self.slots[0]
+        self._epoch(s, (d_sigs, d_bits, d_msgs, d_target_epoch, d_block_idx, source_epoch), (justified_idx, boost_idx, boost_score), False,
+                    current_epoch, pipelined=False)
+        return s.ok, s.head
 
     def process_epoch_host(self, h_sigs, h_bits, h_msgs, h_target_epoch, h_block_idx, justified_idx=0, boost_idx=-1, boost_score=0,
                            source_epoch=None, current_epoch=None):
         """Pinned host tensors in, (verdict bytes, head index) out on the host; returns when the epoch is done.  With the slasher on:
-        source_epoch int64[n_agg] (pinned host) and the current epoch; the findings are read with slashings()."""
+        source_epoch int64[n_agg] (pinned host) and the current epoch; the findings are read with slashings().  Needs a drained
+        pipeline."""
+        assert not self._inflight, "submitted epochs are in flight: drain() first"
         self._slasher_args(source_epoch, current_epoch)
-        self._sync_host = True
-        s = 0
-        self.s_sigs[s].copy_(h_sigs, non_blocking=True)
-        self.s_bits[s].copy_(h_bits, non_blocking=True)
-        self.s_msgs[s].copy_(h_msgs, non_blocking=True)
-        self.s_epoch[s].copy_(h_target_epoch, non_blocking=True)
-        self.s_blk[s].copy_(h_block_idx, non_blocking=True)
-        if self.slasher:
-            self.s_src[s].copy_(source_epoch, non_blocking=True)
-        self._process_epoch_dev(self.s_sigs[s], self.s_bits[s], self.s_msgs[s], self.s_epoch[s], self.s_blk[s], justified_idx, boost_idx, boost_score,
-                                self.s_src[s] if self.slasher else None, current_epoch, True)
-        self.h_ok[s].copy_(self.d_ok[0], non_blocking=True)
-        self.h_head[s].copy_(self.d_head[0], non_blocking=True)
-        self.h_agg_sig[s].copy_(self.d_agg_sig[0], non_blocking=True)
+        s = self.slots[0]
+        x = self._stage(s, True, h_sigs, h_bits, h_msgs, h_target_epoch, h_block_idx, source_epoch)
+        self._epoch(s, x, (justified_idx, boost_idx, boost_score), True, current_epoch, pipelined=False)
         torch.cuda.current_stream().synchronize()
-        return self.h_ok[s], int(self.h_head[s][0])
+        return s.h_ok, int(s.h_head[0])
 
     # ------------------------------------------------------------------ pipelined form
-    def _submit(self, slot, d_sigs, d_bits, d_msgs, fc, host, last=False, current_epoch=None):
-        e = self.eng
-        team = last or self.always_team
-        if team != self._team_form:                       # last epoch of a batch: nothing will overlap its tail, so take the short form
-            e.epoch_set_pairing_form(team)
-            self._team_form = team
-        o_sig, o_ok = self._local_outputs(slot)
-        if self.sharded:
-            e.epoch_start_dev(slot, d_sigs, self.d_members_loc, self.d_off_loc, self._rows(d_bits), self._rows(d_msgs), self.d_agg_status[slot])
-            e.epoch_tail_dev(slot, self.d_members_loc, self.d_off_loc, self._rows(d_bits), None, None, o_sig, self.d_agg_status[slot], o_ok)
-        else:
-            e.epoch_start_dev(slot, d_sigs, self.d_members, self.d_off, d_bits, d_msgs, self.d_agg_status[slot])
-            e.epoch_tail_dev(slot, self.d_members, self.d_off, d_bits, self.s_epoch[slot], self.s_blk[slot], o_sig, self.d_agg_status[slot], o_ok)
-        # fork choice of this epoch: on its own stream, enqueued BEFORE the next epoch's tail (whose LMD update waits for this scatter)
-        with torch.cuda.stream(self.fc_stream):
-            e.epoch_wait_dev(slot)
-            if self.sharded:
-                self._exchange(slot, d_bits, self.s_epoch[slot], self.s_blk[slot])
-            self._fork_choice(slot, *fc)
-            if host:
-                self.h_ok[slot].copy_(self.d_ok[slot], non_blocking=True)
-                self.h_head[slot].copy_(self.d_head[slot], non_blocking=True)
-                self.h_agg_sig[slot].copy_(self.d_agg_sig[slot], non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record()
-            ev_sl = None
-            if self.slasher:                              # after the head: the head's latency does not include it
-                self._slasher_update(slot, self.s_bits[slot], self.s_msgs[slot], self.s_src[slot], self.s_epoch[slot], current_epoch, host)
-                ev_sl = torch.cuda.Event()
-                ev_sl.record()
-        self.ev_fc[slot] = ev
-        self.ev_sl[slot] = ev_sl
-        report = count = None
-        if ev_sl is not None:
-            report = lambda s=slot, h=host, x=ev_sl: self._read_slashings(s, h, x)                                    # noqa: E731
-            count = lambda s=slot, h=host: int((self.h_sl_flagged if h else self.d_sl_flagged)[s][0])              # noqa: E731
-        self._inflight.append(_Ticket(slot, self.d_ok[slot], self.d_head[slot], self.d_agg_sig[slot], ev,
-                                      self.h_ok[slot] if host else None, self.h_head[slot] if host else None,
-                                      self.h_agg_sig[slot] if host else None, report, ev_sl, count))
+    def _submit(self, s, x, fc, host, last, current_epoch):
+        self._epoch(s, x, fc, host, current_epoch, pipelined=True, last=last)
+        self._inflight.append(_Ticket(self, s, host))
         self.k += 1
         return self._inflight.popleft() if len(self._inflight) >= self.depth else None
 
     def _claim_slot(self, stream):
         """`stream` is about to overwrite the slot's inputs/outputs: its previous epoch (tail and fork choice) must be done."""
-        slot = self.k % self.depth
-        self.eng.epoch_wait_dev(slot)                     # (on the current stream == `stream`)
-        if self.ev_fc[slot] is not None:
-            stream.wait_event(self.ev_fc[slot])
-        if self.ev_sl[slot] is not None:                  # the slasher read the slot's bits, messages, epochs and verdicts
-            stream.wait_event(self.ev_sl[slot])
-        return slot
+        s = self.slots[self.k % self.depth]
+        self.eng.epoch_wait_dev(s.i)                      # (on the current stream == `stream`)
+        if s.ev_fc is not None:
+            stream.wait_event(s.ev_fc)
+        if s.ev_sl is not None:                           # the slasher read the slot's bits, messages, epochs and verdicts
+            stream.wait_event(s.ev_sl)
+        return s
 
     def drain_hint(self, remaining: int) -> bool:
         """True when an epoch with `remaining` epochs still to come after it should take the short-latency (team) tail: the last epochs
@@ -415,14 +423,9 @@ class EpochProcessor:
         enqueued in the short-critical-path (team) form.  With the slasher on: source_epoch int64[n_agg] (device) and the
         current epoch; the slasher reads copies of the bits, messages and epochs, so the inputs are free after wait() as without it."""
         self._slasher_args(source_epoch, current_epoch)
-        slot = self._claim_slot(torch.cuda.current_stream())
-        self.s_epoch[slot].copy_(d_target_epoch)
-        self.s_blk[slot].copy_(d_block_idx)
-        if self.slasher:
-            self.s_bits[slot].copy_(d_bits)
-            self.s_msgs[slot].copy_(d_msgs)
-            self.s_src[slot].copy_(source_epoch)
-        return self._submit(slot, d_sigs, d_bits, d_msgs, (justified_idx, boost_idx, boost_score), False, last, current_epoch)
+        s = self._claim_slot(torch.cuda.current_stream())
+        x = self._stage(s, False, d_sigs, d_bits, d_msgs, d_target_epoch, d_block_idx, source_epoch)
+        return self._submit(s, x, (justified_idx, boost_idx, boost_score), False, last, current_epoch)
 
     def submit_host(self, h_sigs, h_bits, h_msgs, h_target_epoch, h_block_idx, justified_idx=0, boost_idx=-1, boost_score=0, last=False,
                     source_epoch=None, current_epoch=None):
@@ -432,19 +435,11 @@ class EpochProcessor:
         self._slasher_args(source_epoch, current_epoch)
         cur = torch.cuda.current_stream()
         with torch.cuda.stream(self.copy_stream):
-            slot = self._claim_slot(self.copy_stream)
-            self.s_sigs[slot].copy_(h_sigs, non_blocking=True)
-            self.s_bits[slot].copy_(h_bits, non_blocking=True)
-            self.s_msgs[slot].copy_(h_msgs, non_blocking=True)
-            self.s_epoch[slot].copy_(h_target_epoch, non_blocking=True)
-            self.s_blk[slot].copy_(h_block_idx, non_blocking=True)
-            if self.slasher:
-                self.s_src[slot].copy_(source_epoch, non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record()
+            s = self._claim_slot(self.copy_stream)
+            x = self._stage(s, True, h_sigs, h_bits, h_msgs, h_target_epoch, h_block_idx, source_epoch)
+            ev = self._record()
         cur.wait_event(ev)
-        return self._submit(slot, self.s_sigs[slot], self.s_bits[slot], self.s_msgs[slot], (justified_idx, boost_idx, boost_score), True, last,
-                            current_epoch)
+        return self._submit(s, x, (justified_idx, boost_idx, boost_score), True, last, current_epoch)
 
     def drain(self):
         """Tickets of the epochs still in flight, oldest first; the current stream waits for all of them (their slasher updates included)."""
@@ -459,11 +454,11 @@ class EpochProcessor:
     @property
     def h2d_bytes(self):
         """host -> device bytes per epoch of this rank (submit_host): its signatures + the epoch's bits, messages, epochs, blocks"""
-        return (self.s_sigs[0].numel() + self.s_bits[0].numel() + self.s_msgs[0].numel() + 8 * self.s_epoch[0].numel() + 4 * self.s_blk[0].numel()
-                + (8 * self.n_agg if self.slasher else 0))
+        s = self.slots[0]
+        return s.sigs.numel() + s.bits.numel() + s.msgs.numel() + 8 * s.tgt.numel() + 4 * s.blk.numel() + (8 * self.n_agg if self.slasher else 0)
 
     @property
     def d2h_bytes(self):
         """device -> host bytes per epoch (submit_host): verdicts + head index + the aggregate signatures (+ the slasher's statuses and
         flagged count; its kind and conflict targets only when something was flagged)"""
-        return self.h_ok[0].numel() + 4 + self.h_agg_sig[0].numel() + ((4 * self.n_agg + 4) if self.slasher else 0)
+        return self.slots[0].h_ok.numel() + 4 + self.slots[0].h_agg_sig.numel() + ((4 * self.n_agg + 4) if self.slasher else 0)

@@ -331,7 +331,7 @@ def test_enabled_slasher_requires_source_and_current_epoch():
     ep = EpochProcessor(eng, N_AGG, N_AGG * CSIZE, 1, N_BLK, device=dev, depth=3)
     ep.set_committees(members, off)
     ep.enable_slasher(8, current_epoch=CUR0)
-    assert ep.sl_range == (0, N_VAL) and ep.d_sl_kind[0].numel() == N_AGG * CSIZE
+    assert ep.sl_range == (0, N_VAL) and ep.slots[0].sl_kind.numel() == N_AGG * CSIZE
     e = _inputs(eng, members, off)[0]
     d = [torch.as_tensor(e[x], device=dev) for x in ("sigs", "bits", "msgs", "tgt", "blk")]
     src = torch.as_tensor(e["src"], device=dev)

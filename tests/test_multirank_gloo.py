@@ -25,14 +25,8 @@ class _OracleEngine:
         self.parent, self.roots, self.leaf_viable = tree
         self.shard = shard
 
-    def aggregate_dev(self, *a):
-        pass
-
-    def fast_aggregate_verify_dev(self, d_members, d_off, d_bits, d_msgs, d_sigs, d_ok):
+    def epoch_dev(self, d_sigs, d_members, d_off, d_bits, d_msgs, d_target_epoch, d_block_idx, d_agg_sig, d_agg_status, d_ok):
         d_ok.fill_(1)
-
-    def latest_messages_update_dev(self, *a):
-        pass
 
     def vote_weights_dev(self, d_votes):
         msg_block, has_msg, equiv, active, eff = self.shard
