@@ -247,6 +247,44 @@ int b2_slasher_update_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t
                           uint32_t n_agg, int32_t* d_att_status_out, uint8_t* d_kind_out, uint32_t* d_conflict_target_out,
                           uint32_t* d_n_flagged_out, void* stream);
 
+/* ---- block packing: BeaconBlockBody.attestations (List[Attestation, MAX_ATTESTATIONS], pos-evolution.md:639; "well-packed aggregate
+ * attestations", :659) chosen from a pool, the proposing-side counterpart of process_attestation (:722-754).
+ * Committee k = members[committee_off[k] .. committee_off[k+1]) with participation table committee_table[k] (0 current, 1 previous; the
+ * tables of b2_participation_load, a table never loaded counts as all-zero).  Candidate c (pool order) = committee cand_committee[c],
+ * data id cand_data[c] (< n_cand; equal ids = the same AttestationData, so the same committee and mask), bit row
+ * bits[c * bits_stride ...] (bits at or past the committee size are ignored), flag mask cand_flag_mask[c] (bit f = participation flag f;
+ * bits 3..7 ignored) and signature sig96[c].  Precondition: the committees of one table are pairwise disjoint and repeat no member.
+ *   1. a candidate whose signature does not decode is excluded (cand_status 1; no subgroup check, as bls.Aggregate);
+ *   2. fold, per data id in pool order: a candidate joins the first folded aggregate of its data id (creation order) whose union row is
+ *      disjoint from its row, else opens a new one; folded aggregates are numbered by the pool position of their first constituent;
+ *   3. gain of a folded aggregate against participation P = sum over its members v and flags f of its mask not in P[v] of
+ *      (eff[v] / effective_balance_increment) * base_reward_per_increment * (14, 26, 14)[f] -- the numerator b2_participation_update credits;
+ *   4. up to max_out times, pick the largest gain > 0 (tie: lowest committee, then lowest folded number) and set its flags in a private
+ *      copy of P.
+ * Outputs in pick order: *n_out; per output committee, data id, union bit row (bits_stride bytes, zero padded), the gain as a u64
+ * numerator, constituents out_src[out_src_off[o] .. out_src_off[o+1]) in pool order, and the signature (bls.Aggregate of the
+ * constituents; one constituent: its bytes unchanged).  Slots past n_out are zero; out_src_off has max_out + 1 entries (past n_out they
+ * repeat the total); out_src holds n_cand entries (zero past the total).  cand_status u8[n_cand]: 0 folded, 1 undecodable.  Neither the
+ * registry nor the participation tables change.  Applying the outputs in order with b2_participation_update returns the numerators.
+ * B2_EINVAL (nothing written): no registry, max_out == 0, bits_stride == 0 or > 256, a committee larger than 8 * bits_stride, a member
+ * index >= n_validators, overlapping committees of one table, a table byte > 1, cand_committee >= n_committees, a data id >= n_cand or
+ * with two committees or two masks. */
+int b2_pack_attestations(b2_ctx* ctx, const uint32_t* members, const uint32_t* committee_off, const uint8_t* committee_table, uint32_t n_committees,
+                         const uint32_t* cand_committee, const uint32_t* cand_data, const uint8_t* cand_flag_mask, const uint8_t* bits, uint32_t bits_stride,
+                         const uint8_t* sig96, uint32_t n_cand, uint32_t max_out, uint64_t effective_balance_increment, uint64_t base_reward_per_increment,
+                         uint32_t* n_out, uint32_t* out_committee, uint32_t* out_data, uint8_t* out_bits, uint8_t* out_sig96, uint64_t* out_numerator,
+                         uint32_t* out_src_off, uint32_t* out_src, uint8_t* cand_status);
+/* the same on device arrays, asynchronous on `stream` (d_n_out is written on the device).  Self-guarding: a candidate committee index
+ * >= n_committees excludes the candidate (cand_status 2, B2_GUARD_BAD_INDEX); a member index >= n_validators earns nothing
+ * (B2_GUARD_BAD_INDEX); overlapping committees of one table, a malformed committee row (also B2_GUARD_BAD_ROW), a table byte > 1, or a
+ * data id >= n_cand or with two committees or masks set B2_GUARD_BAD_POOL and the call selects nothing (n_out = 0). */
+int b2_pack_attestations_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_committee_off, const uint8_t* d_committee_table,
+                             uint32_t n_committees, const uint32_t* d_cand_committee, const uint32_t* d_cand_data, const uint8_t* d_cand_flag_mask,
+                             const uint8_t* d_bits, uint32_t bits_stride, const uint8_t* d_sig96, uint32_t n_cand, uint32_t max_out,
+                             uint64_t effective_balance_increment, uint64_t base_reward_per_increment, uint32_t* d_n_out, uint32_t* d_out_committee,
+                             uint32_t* d_out_data, uint8_t* d_out_bits, uint8_t* d_out_sig96, uint64_t* d_out_numerator, uint32_t* d_out_src_off,
+                             uint32_t* d_out_src, uint8_t* d_cand_status, void* stream);
+
 /* Store.blocks (pos-evolution.md:898) as arrays in topological order (parent[b] < b, parent[0] ignored; block 0 =
  * store.justified_checkpoint.root).  leaf_viable[b]: the get_filtered_block_tree leaf test (:1104, prose :1121-1124). */
 int b2_tree_load(b2_ctx* ctx, const uint32_t* parent, const uint64_t* slot, const uint8_t* root32, const uint8_t* leaf_viable,
@@ -263,8 +301,8 @@ int b2_get_head(b2_ctx* ctx, uint32_t justified_idx, int32_t boost_idx, uint64_t
  * its segment is reported undecodable -- nothing is read or written out of bounds, and the event is recorded in a guard word.
  * Precondition that cannot be checked on the device: off[n_agg] <= length of the members array.
  * b2_guard_flags: synchronises, returns and clears that word (bit0 member index >= n_validators, bit1 malformed offsets row,
- * bit2 target epoch does not fit 32 bits). */
-enum { B2_GUARD_BAD_INDEX = 1, B2_GUARD_BAD_ROW = 2, B2_GUARD_BAD_EPOCH = 4 };
+ * bit2 target epoch does not fit 32 bits, bit3 a pool b2_pack_attestations_dev refused). */
+enum { B2_GUARD_BAD_INDEX = 1, B2_GUARD_BAD_ROW = 2, B2_GUARD_BAD_EPOCH = 4, B2_GUARD_BAD_POOL = 8 };
 int b2_guard_flags(b2_ctx* ctx, uint32_t* flags_out);
 int b2_aggregate_dev(b2_ctx* ctx, const uint8_t* d_sig96, const uint32_t* d_seg_off, uint32_t n_seg, uint64_t n_sig, uint8_t* d_out96,
                      int32_t* d_seg_status, void* stream);

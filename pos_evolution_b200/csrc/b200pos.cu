@@ -17,6 +17,7 @@
 #include "aggverify.cuh"
 #include "syncagg.cuh"
 #include "slasher.cuh"
+#include "pack.cuh"
 
 using namespace b2;
 
@@ -89,6 +90,13 @@ struct slasher_tables {
     uint64_t n_val = 0, n_rows = 0;      // validators of the registry; rows held, for validators v_begin .. v_begin + n_rows - 1
     uint32_t v_begin = 0;
     uint32_t H = 0, K = 0, cur = 0;      // H == 0: not initialised
+};
+
+// block packing (b2_pack_attestations_dev): the scratch of pack_view (pack.cuh), the decompressed candidate signatures, the gathered
+// constituents and their segment sums
+struct pack_scratch {
+    dbuf cnt, off, list, fold_of, fdata, fcnt, frow, fmask, egain, eslot, claim, dcomm, dmask, ctl, sel, ord;
+    dbuf aff, st, gaff, gst, sumjac, seg_status;
 };
 
 struct vslot {
@@ -169,6 +177,7 @@ struct b2_ctx {
     std::vector<dbuf> stage;                          // the synchronous entry points' host inputs and outputs (struct staging)
     sync_tables sync;
     slasher_tables sl;
+    pack_scratch pk;
 };
 
 struct nvtx_scope {
@@ -339,6 +348,7 @@ int b2_init(int device, b2_ctx** out) {
     }
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_get_head_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, TREE_SMEM_BYTES);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_get_head_fused_nvl, cudaFuncAttributeMaxDynamicSharedMemorySize, TREE_SMEM_BYTES);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(k_pack_committee, cudaFuncAttributeMaxDynamicSharedMemorySize, PACK_SMEM_ROWS);
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_rlc_seed.p, 32);
     if (e == cudaSuccess) e = cudaMemset(ctx->d_rlc_seed, 0, 32);
     if (e == cudaSuccess) e = cudaMalloc(&ctx->d_guard.p, 256);
@@ -1589,6 +1599,150 @@ int b2_slasher_update(b2_ctx* ctx, const uint32_t* members, const uint32_t* off,
     uint32_t* dflag = st.out(n_flagged_out, 1);
     if ((rc = st.rc) ||
         (rc = b2_slasher_update_dev(ctx, dm, dof, db, bits_stride, dse, dte, droot, dacc, n_agg, dst, dkind, dconf, dflag, ctx->s_main)))
+        return rc;
+    return st.finish();
+}
+
+// ------------------------------------------------------------------------------------------ block packing (pack.cuh)
+int b2_pack_attestations_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_committee_off, const uint8_t* d_committee_table,
+                             uint32_t n_committees, const uint32_t* d_cand_committee, const uint32_t* d_cand_data, const uint8_t* d_cand_flag_mask,
+                             const uint8_t* d_bits, uint32_t bits_stride, const uint8_t* d_sig96, uint32_t n_cand, uint32_t max_out,
+                             uint64_t effective_balance_increment, uint64_t base_reward_per_increment, uint32_t* d_n_out, uint32_t* d_out_committee,
+                             uint32_t* d_out_data, uint8_t* d_out_bits, uint8_t* d_out_sig96, uint64_t* d_out_numerator, uint32_t* d_out_src_off,
+                             uint32_t* d_out_src, uint8_t* d_cand_status, void* stream) {
+    B2_NVTX;
+    REQUIRE(ctx && d_committee_off && (n_committees == 0 || (d_members && d_committee_table)) &&
+                (n_cand == 0 || (d_cand_committee && d_cand_data && d_cand_flag_mask && d_bits && d_sig96 && d_out_src && d_cand_status)) && d_n_out &&
+                d_out_committee && d_out_data && d_out_bits && d_out_sig96 && d_out_numerator && d_out_src_off && max_out > 0 && bits_stride > 0 &&
+                bits_stride <= PACK_MAX_WORDS * 4 && effective_balance_increment > 0,
+            "pack_attestations_dev: bad arguments (max_out > 0, 0 < bits_stride <= 256, increment > 0)");
+    REQUIRE(ctx->n_val > 0, "pack_attestations: registry not loaded");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    pack_scratch& S = ctx->pk;
+    const size_t C = std::max<uint32_t>(n_cand, 1), K = n_committees, M = max_out, wstride = (bits_stride + 3) / 4;
+    const size_t claim_words = 2 * ((ctx->n_val + 31) / 32);
+    int rc;
+    if ((rc = ensure(ctx, S.cnt, K * 4)) || (rc = ensure(ctx, S.off, (K + 1) * 4)) || (rc = ensure(ctx, S.list, C * 4)) || (rc = ensure(ctx, S.fold_of, C * 4)) ||
+        (rc = ensure(ctx, S.fdata, C * 4)) || (rc = ensure(ctx, S.fcnt, C * 4)) || (rc = ensure(ctx, S.frow, C * wstride * 4)) || (rc = ensure(ctx, S.fmask, C)) ||
+        (rc = ensure(ctx, S.egain, C * 8)) || (rc = ensure(ctx, S.eslot, C * 4)) || (rc = ensure(ctx, S.claim, claim_words * 4)) ||
+        (rc = ensure(ctx, S.dcomm, C * 4)) || (rc = ensure(ctx, S.dmask, C * 4)) || (rc = ensure(ctx, S.ctl, 16)) || (rc = ensure(ctx, S.sel, M * 4)) ||
+        (rc = ensure(ctx, S.ord, M * 4)) || (rc = ensure(ctx, S.aff, C * 192 + 16)) || (rc = ensure(ctx, S.st, C + 16)) || (rc = ensure(ctx, S.gaff, C * 192 + 16)) ||
+        (rc = ensure(ctx, S.gst, C + 16)) || (rc = ensure(ctx, S.sumjac, M * 288)) || (rc = ensure(ctx, S.seg_status, M * 4)))
+        return rc;
+    const registry_tables& R = ctx->reg;
+    pack_view P = {d_members, d_committee_off, d_committee_table, d_cand_committee, d_cand_data, d_cand_flag_mask, d_bits, S.st, R.eff,
+                   {R.part[0], R.part[1]}, n_committees, n_cand, bits_stride, (uint32_t)wstride, max_out, ctx->n_val, effective_balance_increment,
+                   base_reward_per_increment, S.cnt, S.off, S.list, S.fold_of, S.fdata, S.fcnt, S.frow, S.fmask, S.egain, S.eslot, S.claim, S.dcomm,
+                   S.dmask, S.ctl, S.sel, S.ord, d_cand_status, ctx->d_guard};
+    CK(cudaMemsetAsync(S.ctl, 0, 16, s));
+    CK(cudaMemsetAsync(S.claim, 0, claim_words * 4, s));
+    if (K) CK(cudaMemsetAsync(S.cnt, 0, K * 4, s));
+    if (n_cand) {
+        CK(cudaMemsetAsync(S.dcomm, 0xff, (size_t)n_cand * 4, s));
+        CK(cudaMemsetAsync(S.dmask, 0xff, (size_t)n_cand * 4, s));
+        CK(cudaMemsetAsync(d_out_src, 0, (size_t)n_cand * 4, s));
+        k_g2_decompress<<<blocks_for(n_cand, ctx->dec_block), ctx->dec_block, 0, s>>>(d_sig96, n_cand, S.aff, S.st);
+        CKL(ctx);
+    }
+    if (K) {
+        k_pack_claim<<<n_committees, 128, 0, s>>>(P);
+        CKL(ctx);
+    }
+    if (n_cand) {
+        k_pack_prep<<<blocks_for(n_cand, 128), 128, 0, s>>>(P);
+        CKL(ctx);
+    }
+    k_pack_scan<<<1, 1024, 0, s>>>(P);
+    CKL(ctx);
+    if (n_cand) {
+        k_pack_scatter<<<blocks_for(n_cand, 128), 128, 0, s>>>(P);
+        CKL(ctx);
+    }
+    if (K) {
+        k_pack_committee<<<n_committees, 256, PACK_SMEM_ROWS, s>>>(P);
+        CKL(ctx);
+    }
+    k_pack_select<<<1, 1024, 0, s>>>(P);
+    CKL(ctx);
+    k_pack_rank<<<blocks_for(max_out, 128), 128, 0, s>>>(P);
+    CKL(ctx);
+    k_pack_offsets<<<1, 1024, 0, s>>>(P, d_out_src_off, d_n_out);
+    CKL(ctx);
+    k_pack_emit<<<max_out, 128, 0, s>>>(P, d_out_src_off, d_out_committee, d_out_data, d_out_bits, (unsigned long long*)d_out_numerator, d_out_src);
+    CKL(ctx);
+    if (n_cand) {
+        k_pack_gather<<<blocks_for(n_cand, 128), 128, 0, s>>>(S.aff, S.st, d_out_src, d_out_src_off + max_out, S.gaff, S.gst);
+        CKL(ctx);
+    }
+    k_g2_segment_sum<<<max_out, 32, 0, s>>>(S.gaff, S.gst, d_out_src_off, max_out, S.sumjac, S.seg_status, n_cand, ctx->d_guard);
+    CKL(ctx);
+    k_g2_finish<<<blocks_for(max_out, 32), 32, 0, s>>>(S.sumjac, S.seg_status, max_out, d_out_sig96, nullptr, nullptr);
+    CKL(ctx);
+    if (n_cand) {
+        k_pack_single<<<blocks_for(max_out, 128), 128, 0, s>>>(d_sig96, d_out_src_off, d_out_src, max_out, d_out_sig96);
+        CKL(ctx);
+    }
+    return B2_OK;
+}
+
+int b2_pack_attestations(b2_ctx* ctx, const uint32_t* members, const uint32_t* committee_off, const uint8_t* committee_table, uint32_t n_committees,
+                         const uint32_t* cand_committee, const uint32_t* cand_data, const uint8_t* cand_flag_mask, const uint8_t* bits, uint32_t bits_stride,
+                         const uint8_t* sig96, uint32_t n_cand, uint32_t max_out, uint64_t effective_balance_increment, uint64_t base_reward_per_increment,
+                         uint32_t* n_out, uint32_t* out_committee, uint32_t* out_data, uint8_t* out_bits, uint8_t* out_sig96, uint64_t* out_numerator,
+                         uint32_t* out_src_off, uint32_t* out_src, uint8_t* cand_status) {
+    B2_NVTX;
+    REQUIRE(ctx && committee_off && (n_committees == 0 || (members && committee_table)) &&
+                (n_cand == 0 || (cand_committee && cand_data && cand_flag_mask && bits && sig96 && out_src && cand_status)) && n_out && out_committee &&
+                out_data && out_bits && out_sig96 && out_numerator && out_src_off && max_out > 0 && bits_stride > 0 && bits_stride <= PACK_MAX_WORDS * 4 &&
+                effective_balance_increment > 0,
+            "pack_attestations: bad arguments (max_out > 0, 0 < bits_stride <= 256, increment > 0)");
+    REQUIRE(ctx->n_val > 0, "pack_attestations: registry not loaded");
+    int rc;
+    if ((rc = check_batch(ctx, members, committee_off, bits_stride, n_committees, ctx->n_val))) return rc;
+    // the committees of one table are pairwise disjoint and repeat no member
+    std::vector<uint8_t> claimed(2 * ctx->n_val, 0);
+    for (uint32_t k = 0; k < n_committees; k++) {
+        REQUIRE(committee_table[k] <= 1, "pack_attestations: committee_table entries are 0 (current) or 1 (previous)");
+        uint8_t* seen = claimed.data() + (size_t)committee_table[k] * ctx->n_val;
+        for (uint32_t i = committee_off[k]; i < committee_off[k + 1]; i++) {
+            REQUIRE(!seen[members[i]], "pack_attestations: committees of one participation table overlap or repeat a member");
+            seen[members[i]] = 1;
+        }
+    }
+    // one data id = one AttestationData: one committee and one flag mask
+    std::vector<uint32_t> dcomm(n_cand, PACK_NONE), dmask(n_cand, PACK_NONE);
+    for (uint32_t c = 0; c < n_cand; c++) {
+        REQUIRE(cand_committee[c] < n_committees, "pack_attestations: candidate committee index out of range");
+        REQUIRE(cand_data[c] < n_cand, "pack_attestations: data id >= n_cand");
+        const uint32_t d = cand_data[c], m = cand_flag_mask[c] & 7u;
+        REQUIRE((dcomm[d] == PACK_NONE || dcomm[d] == cand_committee[c]) && (dmask[d] == PACK_NONE || dmask[d] == m),
+                "pack_attestations: a data id with two committees or two flag masks");
+        dcomm[d] = cand_committee[c];
+        dmask[d] = m;
+    }
+    CK(cudaSetDevice(ctx->device));
+    staging st(ctx);
+    const uint32_t* dm = st.in(members, n_committees ? committee_off[n_committees] : 0, 4);
+    const uint32_t* doff = st.in(committee_off, (size_t)n_committees + 1);
+    const uint8_t* dtab = st.in(committee_table, n_committees, 4);
+    const uint32_t* dcc = st.in(cand_committee, n_cand, 4);
+    const uint32_t* dcd = st.in(cand_data, n_cand, 4);
+    const uint8_t* dcm = st.in(cand_flag_mask, n_cand, 4);
+    const uint8_t* db = st.in(bits, (size_t)n_cand * bits_stride, 16);
+    const uint8_t* dsig = st.in(sig96, (size_t)n_cand * 96, 16);
+    uint32_t* dn = st.out(n_out, 1);
+    uint32_t* dk = st.out(out_committee, max_out);
+    uint32_t* dd = st.out(out_data, max_out);
+    uint8_t* dbits = st.out(out_bits, (size_t)max_out * bits_stride);
+    uint8_t* dsig96 = st.out(out_sig96, (size_t)max_out * 96);
+    uint64_t* dnum = st.out(out_numerator, max_out);
+    uint32_t* dsoff = st.out(out_src_off, (size_t)max_out + 1);
+    uint32_t* dsrc = n_cand ? st.out(out_src, n_cand) : nullptr;
+    uint8_t* dstat = n_cand ? st.out(cand_status, n_cand) : nullptr;
+    if ((rc = st.rc) || (rc = b2_pack_attestations_dev(ctx, dm, doff, dtab, n_committees, dcc, dcd, dcm, db, bits_stride, dsig, n_cand, max_out,
+                                                       effective_balance_increment, base_reward_per_increment, dn, dk, dd, dbits, dsig96, dnum, dsoff, dsrc,
+                                                       dstat, ctx->s_main)))
         return rc;
     return st.finish();
 }

@@ -53,7 +53,7 @@ __global__ void __launch_bounds__(128) k_registry_load(const uint8_t* __restrict
 // Every kernel that follows caller-supplied indices therefore checks them itself: a committee row whose offsets run backwards or
 // whose size exceeds the bit row, a member index >= n_val, or a target epoch that does not fit the 32-bit key field is SKIPPED
 // (the aggregate then fails verification / contributes nothing) and recorded in the context's guard word (b2_guard_flags).
-enum GuardBits : uint32_t { GUARD_BAD_INDEX = 1, GUARD_BAD_ROW = 2, GUARD_BAD_EPOCH = 4 };
+enum GuardBits : uint32_t { GUARD_BAD_INDEX = 1, GUARD_BAD_ROW = 2, GUARD_BAD_EPOCH = 4, GUARD_BAD_POOL = 8 /* pack.cuh */ };
 __device__ __forceinline__ uint32_t guarded_row_size(const uint32_t* off, uint32_t a, uint32_t bits_stride, uint32_t* guard) {
     const uint32_t o0 = off[a], o1 = off[a + 1];
     if (o1 < o0 || o1 - o0 > bits_stride * 8u) {

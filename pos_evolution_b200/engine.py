@@ -5,11 +5,16 @@ Everything here takes/returns flat numpy arrays (host entry points) or torch CUD
 and bench.py are built on it.  No CPU fallback: constructing an Engine without an H100 (sm_90) raises.
 """
 import ctypes
+from collections import namedtuple
 
 import numpy as np
 
 from . import _lib
 from ._lib import B2Error
+
+# Engine.pack_attestations: per pick (in pick order) committee, data id, union bit row, u64 numerator; constituents src[src_off[o] ..
+# src_off[o+1]) in pool order; signature (bls.Aggregate of the constituents); cand_status per candidate (0 folded, 1 undecodable)
+PackResult = namedtuple("PackResult", "committee data bits numerator src_off src signature cand_status")
 
 
 def _c(a, dtype):
@@ -355,6 +360,46 @@ class Engine:
         self._ck(self.lib.b2_slasher_update(self.h, _p(members), _p(off), _p(bits), stride, _p(se), _p(te), _p(roots), _p(acc), n_agg,
                                             _p(status), _p(kind), _p(conflict), ctypes.byref(flagged)))
         return status, kind, conflict, int(flagged.value)
+
+    # ------------------------------------------------------------------ block packing (BeaconBlockBody.attestations, pos-evolution.md:639)
+    def pack_attestations(self, members, committee_off, committee_table, cand_committee, cand_data, cand_flag_mask, bits, sigs96, max_out: int,
+                          increment: int, base_reward_per_increment: int) -> "PackResult":
+        """Fold disjoint aggregates of one vote and pick up to max_out folded aggregates greedily by proposer-reward numerator against
+        the device participation tables (include/b200pos.h, b2_pack_attestations).  bits: uint8[n_cand, bits_stride].  Returns a
+        PackResult trimmed to the n_out picks, in pick order."""
+        members, off = _c(members, np.uint32), _c(committee_off, np.uint32)
+        table = _c(committee_table, np.uint8)
+        cc, cd, cm = _c(cand_committee, np.uint32), _c(cand_data, np.uint32), _c(cand_flag_mask, np.uint8)
+        n_cand, n_comm = cc.shape[0], off.shape[0] - 1
+        b = _c(bits, np.uint8)
+        b = b if b.ndim == 2 else b.reshape(n_cand, -1)
+        stride = b.shape[1]
+        sigs = _c(sigs96, np.uint8).reshape(n_cand, 96)
+        assert table.shape == (n_comm,) and cd.shape == (n_cand,) and cm.shape == (n_cand,) and max_out > 0
+        n_out = ctypes.c_uint32(0)
+        o_comm, o_data = np.zeros(max_out, dtype=np.uint32), np.zeros(max_out, dtype=np.uint32)
+        o_bits, o_sig = np.zeros((max_out, stride), dtype=np.uint8), np.zeros((max_out, 96), dtype=np.uint8)
+        o_num, o_soff = np.zeros(max_out, dtype=np.uint64), np.zeros(max_out + 1, dtype=np.uint32)
+        o_src, status = np.zeros(max(n_cand, 1), dtype=np.uint32), np.zeros(max(n_cand, 1), dtype=np.uint8)
+        self._ck(self.lib.b2_pack_attestations(self.h, _p(members), _p(off), _p(table), n_comm, _p(cc), _p(cd), _p(cm), _p(b), stride, _p(sigs), n_cand,
+                                               int(max_out), int(increment), int(base_reward_per_increment), ctypes.byref(n_out), _p(o_comm),
+                                               _p(o_data), _p(o_bits), _p(o_sig), _p(o_num), _p(o_soff), _p(o_src), _p(status)))
+        n = int(n_out.value)
+        return PackResult(o_comm[:n], o_data[:n], o_bits[:n], o_num[:n], o_soff[:n + 1], o_src[:int(o_soff[n])], o_sig[:n], status[:n_cand])
+
+    def pack_attestations_dev(self, d_members, d_committee_off, d_committee_table, d_cand_committee, d_cand_data, d_cand_flag_mask, d_bits, d_sigs,
+                              max_out: int, increment: int, base_reward_per_increment: int, d_n_out, d_out_committee, d_out_data, d_out_bits,
+                              d_out_sig, d_out_numerator, d_out_src_off, d_out_src, d_cand_status):
+        """b2_pack_attestations_dev on torch CUDA tensors (asynchronous on the current stream; d_n_out uint32[1] is written on the device).
+        Outputs sized as the host form before trimming: max_out rows, max_out + 1 offsets, n_cand sources and statuses."""
+        n_cand = d_cand_committee.numel()
+        self._ck(self.lib.b2_pack_attestations_dev(self.h, d_members.data_ptr(), d_committee_off.data_ptr(), d_committee_table.data_ptr(),
+                                                   d_committee_off.numel() - 1, d_cand_committee.data_ptr(), d_cand_data.data_ptr(),
+                                                   d_cand_flag_mask.data_ptr(), d_bits.data_ptr(), d_bits.shape[1], d_sigs.data_ptr(), n_cand,
+                                                   int(max_out), int(increment), int(base_reward_per_increment), d_n_out.data_ptr(),
+                                                   d_out_committee.data_ptr(), d_out_data.data_ptr(), d_out_bits.data_ptr(), d_out_sig.data_ptr(),
+                                                   d_out_numerator.data_ptr(), d_out_src_off.data_ptr(), d_out_src.data_ptr(), d_cand_status.data_ptr(),
+                                                   self._stream()))
 
     def tree_load(self, parent, slot, roots32, leaf_viable):
         parent, slot = _c(parent, np.uint32), _c(slot, np.uint64)

@@ -50,6 +50,7 @@ class Preset:
     PROPOSER_SCORE_BOOST: int = 40
     SYNC_COMMITTEE_SIZE: int = 512
     EPOCHS_PER_SYNC_COMMITTEE_PERIOD: int = 256
+    MAX_ATTESTATIONS: int = 128                   # BeaconBlockBody.attestations limit (:639)
 
 
 MAINNET = Preset("mainnet", 32, 64, 128, 90, 65536, 8192)
@@ -667,6 +668,56 @@ class Spec:
             tables[which][:] = eng.participation_read(which).tolist()
             for v in num:
                 state.balances[proposer] += int(v) // denominator
+
+    # ------------------------------------------------------------------ block packing (BeaconBlockBody.attestations :639, :659)
+    def get_attestations_for_block(self, state, pool, max_attestations=None) -> List[Attestation]:
+        """The attestations a proposer at state.slot includes: the pool entries process_attestation would accept (signatures are
+        assumed gossip-validated and not verified here), disjoint aggregates of one AttestationData folded into one, then up to
+        max_attestations (MAX_ATTESTATIONS) folded aggregates chosen greedily by proposer-reward numerator against the state's
+        participation -- one GPU call (b2_pack_attestations).  Returned in pick order, ready for process_attestations."""
+        max_out = self.p.MAX_ATTESTATIONS if max_attestations is None else int(max_attestations)
+        committees, data_ids, datas = {}, {}, []
+        members, off, table = [], [0], []
+        cand_comm, cand_data, masks, rows, sigs = [], [], [], [], []
+        cur = self.get_current_epoch(state)
+        for att in pool:
+            try:
+                committee, flag_indices = self._check_attestation(state, att)
+            except AssertionError:
+                continue
+            d = att.data
+            k = committees.get((d.slot, d.index))
+            if k is None:
+                k = committees[(d.slot, d.index)] = len(table)
+                members += committee
+                off.append(len(members))
+                table.append(0 if d.target.epoch == cur else 1)
+            root = hash_tree_root_attestation_data(d)
+            if root not in data_ids:
+                data_ids[root] = len(datas)
+                datas.append(d)
+            cand_comm.append(k)
+            cand_data.append(data_ids[root])
+            masks.append(sum(1 << f for f in flag_indices))
+            rows.append(att.aggregation_bits)
+            sig = bytes(att.signature)
+            sigs.append(sig if len(sig) == 96 else bytes(96))          # a wrong length never decodes
+        if not rows or max_out <= 0:
+            return []
+        self.sync_registry(state)              # first: a registry reload drops the device participation tables
+        eng = self.engine
+        eng.participation_load(0, np.asarray(state.current_epoch_participation, dtype=np.uint8))
+        eng.participation_load(1, np.asarray(state.previous_epoch_participation, dtype=np.uint8))
+        sizes = np.diff(np.asarray(off, dtype=np.int64))
+        res = eng.pack_attestations(np.asarray(members, dtype=np.uint32), off, table, cand_comm, cand_data, masks,
+                                    pack_bits(rows, stride=max(1, (int(sizes.max()) + 7) // 8)), np.frombuffer(b"".join(sigs), dtype=np.uint8),
+                                    max_out, self.p.EFFECTIVE_BALANCE_INCREMENT, self.get_base_reward_per_increment(state))
+        out = []
+        for o in range(len(res.committee)):
+            n = int(sizes[int(res.committee[o])])
+            row = np.unpackbits(res.bits[o], bitorder="little")[:n]
+            out.append(Attestation([bool(x) for x in row], datas[int(res.data[o])], res.signature[o].tobytes()))
+        return out
 
     # ------------------------------------------------------------------ sync committee (:371-372, :540-590; Altair)
     def compute_sync_committee_period(self, epoch):                            # :586-587
