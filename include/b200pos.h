@@ -379,6 +379,23 @@ uint32_t b2_tree_size(b2_ctx* ctx);
  * Reading clears them: a slot that no call since the last read has written reads 0. */
 int b2_debug_head_clocks(b2_ctx* ctx, uint64_t* out32);
 
+/* ---- hash_tree_root of the beacon state's large fields (pos-evolution.md:338-374, checked at :423 and :1078).
+ * b2_ssz_validators_load    builds the device node cache of List[Validator, 2^40] from n records of 121 bytes (the SSZ serialisation
+ *                           of Validator, :36-45), n < 2^32 (0 allowed), and returns the list's root.  The cache holds 2C x 32 bytes,
+ *                           C = next_pow2(max(n, 1)); it replaces the previous one only once complete.
+ * b2_ssz_validators_update  replaces records idx[0..k) (strictly increasing, < n) in place, re-hashes those leaves and their paths to
+ *                           the root, and returns the new root; k = 0 returns the current root.  B2_EINVAL, with nothing changed, on
+ *                           unsorted, duplicate or out-of-range indices or without a loaded cache.  A registry that grows is re-loaded.
+ * b2_ssz_chunks_root        the root of n_bytes of packed basic values: 32-byte chunks, the last zero-padded, merkleized to depth
+ *                           limit_depth (n_bytes <= 32 * 2^limit_depth, limit_depth <= 64), then mix_in_length(root, length) when mix_in
+ *                           is set.  The form of every basic-type list and vector of the state (balances, participation, inactivity
+ *                           scores, randao_mixes, block_roots, state_roots, slashings).  Uses scratch only.
+ * A context that never calls these allocates nothing for them. */
+int b2_ssz_validators_load(b2_ctx* ctx, const uint8_t* rec121, uint64_t n, uint8_t* root32_out);
+int b2_ssz_validators_update(b2_ctx* ctx, const uint32_t* idx, const uint8_t* rec121, uint64_t k, uint8_t* root32_out);
+int b2_ssz_chunks_root(b2_ctx* ctx, const uint8_t* data, uint64_t n_bytes, uint32_t limit_depth, int mix_in, uint64_t length,
+                       uint8_t* root32_out);
+
 #ifdef __cplusplus
 }
 #endif

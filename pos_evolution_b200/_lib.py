@@ -99,6 +99,9 @@ SIGNATURES = {
     "b2_fc_exchange_open": (c_int, [c_void_p, c_int, c_int, c_void_p]),
     "b2_get_head_multi": (c_int, [c_void_p, c_uint64, c_uint64, c_uint32, c_int32, c_uint64, c_void_p]),
     "b2_debug_head_clocks": (c_int, [c_void_p, c_void_p]),
+    "b2_ssz_validators_load": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p]),
+    "b2_ssz_validators_update": (c_int, [c_void_p, c_void_p, c_void_p, c_uint64, c_void_p]),
+    "b2_ssz_chunks_root": (c_int, [c_void_p, c_void_p, c_uint64, c_uint32, c_int, c_uint64, c_void_p]),
 }
 
 

@@ -18,6 +18,7 @@
 #include "syncagg.cuh"
 #include "slasher.cuh"
 #include "pack.cuh"
+#include "ssz.cuh"
 
 using namespace b2;
 
@@ -99,6 +100,14 @@ struct pack_scratch {
     dbuf aff, st, gaff, gst, sumjac, seg_status;
 };
 
+// hash_tree_root (ssz.cuh): the validators tree's node cache over C leaves (heap layout, 2C nodes of 8 words) and the scratch tree of
+// b2_ssz_chunks_root
+struct ssz_tables {
+    dbuf cache;
+    uint64_t n = 0, C = 0;      // C == 0: no cache
+    dbuf chunks;
+};
+
 struct vslot {
     dbuf haff, hflag, pkjac, pkst, saff, sflag, f, sumjac;
     dbuf g2aff, g2st;                                      // the slot's own decompressed signatures (pipelined epochs)
@@ -178,6 +187,7 @@ struct b2_ctx {
     sync_tables sync;
     slasher_tables sl;
     pack_scratch pk;
+    ssz_tables ssz;
 };
 
 struct nvtx_scope {
@@ -2037,6 +2047,122 @@ int b2_get_head(b2_ctx* ctx, uint32_t justified_idx, int32_t boost_idx, uint64_t
     CK(cudaStreamSynchronize(s));
     *head_idx_out = h;
     return B2_OK;
+}
+
+// ------------------------------------------------------------------------------------------ hash_tree_root (ssz.cuh)
+constexpr uint32_t SSZ_REGISTRY_DEPTH = 40;      // VALIDATOR_REGISTRY_LIMIT = 2^40
+
+static const ssz_zero_hashes& ssz_zeros() {
+    static const ssz_zero_hashes Z = [] {
+        ssz_zero_hashes z = {};
+        for (int l = 1; l < SSZ_MAX_DEPTH; l++) sha256_node_pair(z.z[l - 1], z.z[l - 1], z.z[l]);
+        return z;
+    }();
+    return Z;
+}
+
+static uint32_t ssz_log2(uint64_t pow2) {
+    uint32_t l = 0;
+    while ((1ull << l) < pow2) l++;
+    return l;
+}
+
+static uint64_t ssz_leaves_for(uint64_t n) {
+    uint64_t C = 1;
+    while (C < n) C <<= 1;
+    return C;
+}
+
+// every inner node of a heap whose C leaves are in place: one subtree launch per SSZ_SUBTREE_LEVELS levels (2^20 leaves: 3 launches)
+static int ssz_reduce(b2_ctx* ctx, uint32_t* cache, uint64_t C) {
+    for (uint64_t m = C; m > 1;) {
+        const uint32_t levels = std::min<uint32_t>(SSZ_SUBTREE_LEVELS, ssz_log2(m));
+        k_ssz_subtree<<<(unsigned)(m >> levels), 256, 0, ctx->s_main>>>(cache, m, levels);
+        CKL(ctx);
+        m >>= levels;
+    }
+    return B2_OK;
+}
+
+// node 1 of the heap, padded with zero subtrees from depth log2 C to `depth`, then mixed with the length when mix_in is set
+static int ssz_root(b2_ctx* ctx, const uint32_t* cache, uint64_t C, uint32_t depth, int mix_in, uint64_t length, uint8_t* d_root32) {
+    k_ssz_root<<<1, 32, 0, ctx->s_main>>>(cache + 8, ssz_log2(C), depth, ssz_zeros(), mix_in, length, d_root32);
+    CKL(ctx);
+    return B2_OK;
+}
+
+int b2_ssz_validators_load(b2_ctx* ctx, const uint8_t* rec121, uint64_t n, uint8_t* root32_out) {
+    B2_NVTX;
+    REQUIRE(ctx && root32_out && (n == 0 || rec121) && n < (1ull << 32), "ssz_validators_load: bad arguments (n < 2^32)");
+    CK(cudaSetDevice(ctx->device));
+    ssz_tables t;      // built aside: a failed load leaves the previous cache answering
+    t.n = n;
+    t.C = ssz_leaves_for(n);
+    int rc;
+    if ((rc = ensure(ctx, t.cache, t.C * 64))) return rc;
+    staging st(ctx);
+    const uint8_t* drec = st.in(rec121, n * SSZ_VALIDATOR_BYTES);
+    uint8_t* droot = st.out(root32_out, 32);
+    if (st.rc) return st.rc;
+    cudaStream_t s = ctx->s_main;
+    if (n) {
+        k_ssz_validator_leaves<<<blocks_for(n, SSZ_LEAF_THREADS), SSZ_LEAF_THREADS, 0, s>>>(drec, nullptr, n, t.cache, t.C);
+        CKL(ctx);
+    }
+    CK(cudaMemsetAsync((uint32_t*)t.cache + (t.C + n) * 8, 0, (t.C - n) * 32, s));      // the zero leaves past n
+    if ((rc = ssz_reduce(ctx, t.cache, t.C)) || (rc = ssz_root(ctx, t.cache, t.C, SSZ_REGISTRY_DEPTH, 1, n, droot)) || (rc = st.finish()))
+        return rc;
+    t.chunks = std::move(ctx->ssz.chunks);
+    ctx->ssz = std::move(t);
+    return B2_OK;
+}
+
+int b2_ssz_validators_update(b2_ctx* ctx, const uint32_t* idx, const uint8_t* rec121, uint64_t k, uint8_t* root32_out) {
+    B2_NVTX;
+    REQUIRE(ctx && root32_out && (k == 0 || (idx && rec121)), "ssz_validators_update: bad arguments");
+    ssz_tables& t = ctx->ssz;
+    REQUIRE(t.C, "ssz_validators_update: no validators tree (b2_ssz_validators_load)");
+    for (uint64_t j = 0; j < k; j++)
+        REQUIRE(idx[j] < t.n && (j == 0 || idx[j - 1] < idx[j]), "ssz_validators_update: indices must be strictly increasing and below n");
+    CK(cudaSetDevice(ctx->device));
+    staging st(ctx);
+    const uint32_t* didx = st.in(idx, k);
+    const uint8_t* drec = st.in(rec121, k * SSZ_VALIDATOR_BYTES);
+    uint8_t* droot = st.out(root32_out, 32);
+    if (st.rc) return st.rc;
+    cudaStream_t s = ctx->s_main;
+    if (k) {
+        k_ssz_validator_leaves<<<blocks_for(k, SSZ_LEAF_THREADS), SSZ_LEAF_THREADS, 0, s>>>(drec, didx, k, t.cache, t.C);
+        CKL(ctx);
+        for (uint32_t shift = 1, depth = ssz_log2(t.C); shift <= depth; shift++) {
+            k_ssz_update_level<<<blocks_for(k, 128), 128, 0, s>>>(t.cache, didx, k, t.C, shift);
+            CKL(ctx);
+        }
+    }
+    int rc;
+    if ((rc = ssz_root(ctx, t.cache, t.C, SSZ_REGISTRY_DEPTH, 1, t.n, droot))) return rc;
+    return st.finish();
+}
+
+int b2_ssz_chunks_root(b2_ctx* ctx, const uint8_t* data, uint64_t n_bytes, uint32_t limit_depth, int mix_in, uint64_t length,
+                       uint8_t* root32_out) {
+    B2_NVTX;
+    REQUIRE(ctx && root32_out && (n_bytes == 0 || data) && n_bytes < (1ull << 40) && limit_depth <= SSZ_MAX_DEPTH,
+            "ssz_chunks_root: bad arguments (n_bytes < 2^40, limit_depth <= 64)");
+    const uint64_t C = ssz_leaves_for((n_bytes + 31) / 32);
+    REQUIRE(ssz_log2(C) <= limit_depth, "ssz_chunks_root: more chunks than 2^limit_depth");
+    CK(cudaSetDevice(ctx->device));
+    int rc;
+    if ((rc = ensure(ctx, ctx->ssz.chunks, C * 64))) return rc;
+    staging st(ctx);
+    const uint8_t* dd = st.in(data, n_bytes);
+    uint8_t* droot = st.out(root32_out, 32);
+    if (st.rc) return st.rc;
+    uint32_t* tree = ctx->ssz.chunks;
+    k_ssz_chunk_leaves<<<blocks_for(C * 8, 256), 256, 0, ctx->s_main>>>(dd, n_bytes, tree, C);
+    CKL(ctx);
+    if ((rc = ssz_reduce(ctx, tree, C)) || (rc = ssz_root(ctx, tree, C, limit_depth, mix_in != 0, length, droot))) return rc;
+    return st.finish();
 }
 
 }  // extern "C"

@@ -37,6 +37,7 @@ class Engine:
         self.device = device
         self.n_validators = 0
         self.n_blocks = 0
+        self.ssz_loads = 0          # successful ssz_validators_load calls: which tree is on the device
 
     def close(self):
         if getattr(self, "h", None):
@@ -231,6 +232,35 @@ class Engine:
         out = np.zeros((n, 32), dtype=np.uint8)
         self._ck(self.lib.b2_sha256_batch(self.h, _p(m) if msg_len else None, msg_len, n, _p(out)))
         return out
+
+    # ------------------------------------------------------------------ hash_tree_root (pos-evolution.md:423, :1078)
+    def ssz_validators_load(self, records) -> bytes:
+        """Build the device tree of List[Validator, 2^40] from uint8[n, 121] SSZ-serialised records (spec.serialize_validators);
+        returns its 32-byte root."""
+        rec = _c(records, np.uint8).reshape(-1, 121)
+        out = np.zeros(32, dtype=np.uint8)
+        self._ck(self.lib.b2_ssz_validators_load(self.h, _p(rec), rec.shape[0], _p(out)))
+        self.ssz_loads += 1
+        return out.tobytes()
+
+    def ssz_validators_update(self, idx, records) -> bytes:
+        """Replace the records at idx (uint32, strictly increasing, below n) in the device tree and return the new root; re-hashes
+        only those leaves and their paths."""
+        idx = _c(idx, np.uint32)
+        rec = _c(records, np.uint8).reshape(-1, 121)
+        assert rec.shape[0] == idx.shape[0]
+        out = np.zeros(32, dtype=np.uint8)
+        self._ck(self.lib.b2_ssz_validators_update(self.h, _p(idx), _p(rec), idx.shape[0], _p(out)))
+        return out.tobytes()
+
+    def ssz_chunks_root(self, array, limit_depth: int, length=None) -> bytes:
+        """Root of the bytes of `array` (little-endian basic values or 32-byte roots) packed into chunks and merkleized to depth
+        limit_depth; with `length`, mix_in_length(root, length) -- the root of a List, without it of a Vector."""
+        data = np.ascontiguousarray(array).view(np.uint8).reshape(-1)
+        out = np.zeros(32, dtype=np.uint8)
+        self._ck(self.lib.b2_ssz_chunks_root(self.h, _p(data), data.shape[0], limit_depth, int(length is not None),
+                                             0 if length is None else int(length), _p(out)))
+        return out.tobytes()
 
     def attestations_decode(self, wire: bytes, woff, bits_stride: int, max_bits: int):
         """SSZ wire decode of n Attestations (pos-evolution.md:714-717) -> (bits u8[n][stride], bit_len u32[n], data128 u8[n][128],

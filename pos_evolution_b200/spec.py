@@ -51,10 +51,15 @@ class Preset:
     SYNC_COMMITTEE_SIZE: int = 512
     EPOCHS_PER_SYNC_COMMITTEE_PERIOD: int = 256
     MAX_ATTESTATIONS: int = 128                   # BeaconBlockBody.attestations limit (:639)
+    VALIDATOR_REGISTRY_LIMIT: int = 2**40         # list limits and vector lengths of BeaconState (:338-374)
+    HISTORICAL_ROOTS_LIMIT: int = 2**24
+    EPOCHS_PER_SLASHINGS_VECTOR: int = 8192
+    EPOCHS_PER_ETH1_VOTING_PERIOD: int = 64
 
 
 MAINNET = Preset("mainnet", 32, 64, 128, 90, 65536, 8192)
-MINIMAL = Preset("minimal", 8, 4, 4, 10, 64, 64, SYNC_COMMITTEE_SIZE=32, EPOCHS_PER_SYNC_COMMITTEE_PERIOD=8)
+MINIMAL = Preset("minimal", 8, 4, 4, 10, 64, 64, SYNC_COMMITTEE_SIZE=32, EPOCHS_PER_SYNC_COMMITTEE_PERIOD=8, EPOCHS_PER_SLASHINGS_VECTOR=64,
+                 EPOCHS_PER_ETH1_VOTING_PERIOD=4)
 
 
 # ----------------------------------------------------------------------------- containers
@@ -65,6 +70,9 @@ class Validator:                       # pos-evolution.md:36-45
     slashed: bool = False
     activation_epoch: int = 0
     exit_epoch: int = FAR_FUTURE_EPOCH
+    withdrawal_credentials: bytes = ZERO32
+    activation_eligibility_epoch: int = 0
+    withdrawable_epoch: int = FAR_FUTURE_EPOCH
 
 
 @dataclass(frozen=True)
@@ -134,7 +142,41 @@ class SyncAggregate:                   # Altair BeaconBlockBody.sync_aggregate
 
 
 @dataclass
-class BeaconState:                     # :338-374 (fields the path reads/writes)
+class BeaconBlockHeader:               # named in BeaconState (:343); fields as in upstream phase 0
+    slot: int = 0
+    proposer_index: int = 0
+    parent_root: bytes = ZERO32
+    state_root: bytes = ZERO32
+    body_root: bytes = ZERO32
+
+
+@dataclass
+class Eth1Data:                        # named in BeaconState (:348-349); fields as in upstream phase 0
+    deposit_root: bytes = ZERO32
+    deposit_count: int = 0
+    block_hash: bytes = ZERO32
+
+
+@dataclass
+class ExecutionPayloadHeader:          # named in BeaconState (:374); fields as in upstream Bellatrix
+    parent_hash: bytes = ZERO32
+    fee_recipient: bytes = bytes(20)
+    state_root: bytes = ZERO32
+    receipts_root: bytes = ZERO32
+    logs_bloom: bytes = bytes(256)
+    prev_randao: bytes = ZERO32
+    block_number: int = 0
+    gas_limit: int = 0
+    gas_used: int = 0
+    timestamp: int = 0
+    extra_data: bytes = b""            # ByteList[32]
+    base_fee_per_gas: int = 0          # uint256
+    block_hash: bytes = ZERO32
+    transactions_root: bytes = ZERO32
+
+
+@dataclass
+class BeaconState:                     # :338-374; the fields after next_sync_committee only enter hash_tree_root_state
     slot: int
     fork: Fork
     genesis_validators_root: bytes
@@ -150,6 +192,16 @@ class BeaconState:                     # :338-374 (fields the path reads/writes)
     justification_bits: List[int] = field(default_factory=lambda: [0] * JUSTIFICATION_BITS_LENGTH)
     current_sync_committee: Optional[SyncCommittee] = None          # :371
     next_sync_committee: Optional[SyncCommittee] = None             # :372
+    genesis_time: int = 0
+    latest_block_header: BeaconBlockHeader = field(default_factory=BeaconBlockHeader)
+    state_roots: Optional[List[bytes]] = None                        # Vector[Root, SLOTS_PER_HISTORICAL_ROOT]; None = all zero
+    historical_roots: List[bytes] = field(default_factory=list)
+    eth1_data: Eth1Data = field(default_factory=Eth1Data)
+    eth1_data_votes: List[Eth1Data] = field(default_factory=list)
+    eth1_deposit_index: int = 0
+    slashings: Optional[List[int]] = None                            # Vector[Gwei, EPOCHS_PER_SLASHINGS_VECTOR]; None = all zero
+    inactivity_scores: List[int] = field(default_factory=list)
+    latest_execution_payload_header: ExecutionPayloadHeader = field(default_factory=ExecutionPayloadHeader)
 
 
 @dataclass
@@ -215,6 +267,35 @@ def serialize_attestation(att: Attestation) -> bytes:
     return (228).to_bytes(4, "little") + serialize_attestation_data(att.data) + bytes(att.signature) + bytes(bl)
 
 
+def serialize_validators(validators) -> np.ndarray:
+    """SSZ serialisation of each Validator (:36-45) -> uint8[n, 121]: pubkey 48, withdrawal_credentials 32, effective_balance u64,
+    slashed 1, activation_eligibility_epoch, activation_epoch, exit_epoch, withdrawable_epoch u64, little-endian.  The record format of
+    Engine.ssz_validators_load / ssz_validators_update."""
+    n = len(validators)
+    out = np.zeros((n, 121), dtype=np.uint8)
+    if n == 0:
+        return out
+    u64 = lambda f: np.array([getattr(v, f) for v in validators], dtype="<u8").view(np.uint8).reshape(n, 8)      # noqa: E731
+    out[:, 0:48] = np.frombuffer(b"".join(bytes(v.pubkey) for v in validators), dtype=np.uint8).reshape(n, 48)
+    out[:, 48:80] = np.frombuffer(b"".join(bytes(v.withdrawal_credentials) for v in validators), dtype=np.uint8).reshape(n, 32)
+    out[:, 80:88] = u64("effective_balance")
+    out[:, 88] = [1 if v.slashed else 0 for v in validators]
+    for k, f in enumerate(("activation_eligibility_epoch", "activation_epoch", "exit_epoch", "withdrawable_epoch")):
+        out[:, 89 + 8 * k:97 + 8 * k] = u64(f)
+    return out
+
+
+def _chunk_depth(limit: int, size: int) -> int:
+    """depth of the chunk tree of `limit` basic values (or roots) of `size` bytes"""
+    return ((limit * size + 31) // 32 - 1).bit_length()
+
+
+def _pubkey_root(pk: bytes) -> bytes:
+    """hash_tree_root(BLSPubkey): the 48 bytes in two chunks, the second zero-padded"""
+    assert len(pk) == 48
+    return sha256(bytes(pk) + bytes(16))
+
+
 def compute_domain(domain_type: bytes, fork_version: bytes, genesis_validators_root: bytes) -> bytes:
     fork_data_root = _merkle([bytes(fork_version) + bytes(28), bytes(genesis_validators_root)])
     return bytes(domain_type) + fork_data_root[:28]
@@ -271,8 +352,11 @@ class Spec:
         self.registry_valid = None         # KeyValidate verdict per validator of the registry on the device (uint8[n])
         self._sync_key = None              # (length, hash of the pubkey bytes) of the sync committee on the device
         self.sync_committee_valid = None   # KeyValidate verdict per position of that committee (uint8[SYNC_COMMITTEE_SIZE])
+        self._ssz_records = None           # serialised validators of the device tree of hash_tree_root_state (uint8[n, 121])
+        self._ssz_load_id = None           # engine.ssz_loads after this Spec's last load: another load replaced the tree when it differs
         self._slasher = None               # slasher_start: size and current epoch of the device history, accepted attestations by target epoch
-        self.stats = {"registry_uploads": 0, "balance_refreshes": 0, "store_uploads": 0, "lmd_device_updates": 0, "sync_committee_uploads": 0}
+        self.stats = {"registry_uploads": 0, "balance_refreshes": 0, "store_uploads": 0, "lmd_device_updates": 0, "sync_committee_uploads": 0,
+                      "ssz_validator_loads": 0, "ssz_validator_updates": 0}
         # full: fingerprint = hash of ALL pubkeys on every call (O(n) host work, catches any in-place replacement);
         # sampled: first / last / 62 strided pubkeys (O(1)); auto: full up to 65 536 validators, sampled above
         self.registry_check = "auto"
@@ -1030,3 +1114,83 @@ class Spec:
     def get_head(self, store):                                                 # :1102-1116
         order, index, boost_idx, boost_score = self._sync_store(store)
         return order[self.engine.get_head(0, boost_idx, boost_score)]
+
+    # ------------------------------------------------------------------ hash_tree_root(state) (:423, :1078)
+    def validators_root(self, state) -> bytes:
+        """hash_tree_root(state.validators) from the device tree: the records are diffed against those of the previous call and only
+        the changed ones are sent as an update; a registry of another size, or a tree another caller loaded since, is re-loaded."""
+        rec = serialize_validators(state.validators)
+        old = self._ssz_records
+        if old is None or old.shape[0] != rec.shape[0] or self.engine.ssz_loads != self._ssz_load_id:
+            root = self.engine.ssz_validators_load(rec)
+            self._ssz_load_id = self.engine.ssz_loads
+            self.stats["ssz_validator_loads"] += 1
+        else:
+            idx = np.flatnonzero((old != rec).any(axis=1)).astype(np.uint32)
+            root = self.engine.ssz_validators_update(idx, rec[idx])
+            self.stats["ssz_validator_updates"] += 1
+        self._ssz_records = rec
+        return root
+
+    def hash_tree_root_state(self, state) -> bytes:
+        """hash_tree_root of the Bellatrix BeaconState (:338-374): its 25 field roots, padded to 32 leaves.  The validators, the other
+        registry-sized lists and the large vectors are merkleized on the GPU; the small fields on the host.  A vector field left as
+        None and a sync committee left as None hash as their SSZ default (all zero)."""
+        p, eng = self.p, self.engine
+        limit = p.VALIDATOR_REGISTRY_LIMIT
+
+        def roots(values, length, depth, as_list=False):       # Vector / List of 32-byte roots
+            values = [ZERO32] * length if values is None else values
+            assert as_list or len(values) == length
+            data = np.frombuffer(b"".join(bytes(r) for r in values), dtype=np.uint8)
+            return eng.ssz_chunks_root(data, depth, len(values) if as_list else None)
+
+        def basic_list(values, dtype):
+            a = np.asarray(values, dtype=dtype)
+            return eng.ssz_chunks_root(a, _chunk_depth(limit, a.itemsize), len(a))
+
+        def sync_committee(c):
+            pks, agg = ([bytes(48)] * p.SYNC_COMMITTEE_SIZE, bytes(48)) if c is None else (c.pubkeys, c.aggregate_pubkey)
+            return _merkle([_merkle([_pubkey_root(pk) for pk in pks]), _pubkey_root(agg)])
+
+        slashings = np.zeros(p.EPOCHS_PER_SLASHINGS_VECTOR, dtype="<u8") if state.slashings is None else np.asarray(state.slashings, dtype="<u8")
+        assert slashings.shape == (p.EPOCHS_PER_SLASHINGS_VECTOR,)
+        h, e1, x = state.latest_block_header, state.eth1_data, state.latest_execution_payload_header
+        eth1_root = lambda e: _merkle([bytes(e.deposit_root), _u64_chunk(e.deposit_count), bytes(e.block_hash)])     # noqa: E731
+        payload_header = _merkle([
+            bytes(x.parent_hash), bytes(x.fee_recipient).ljust(32, b"\0"), bytes(x.state_root), bytes(x.receipts_root),
+            _merkle([bytes(x.logs_bloom)[i:i + 32] for i in range(0, 256, 32)]), bytes(x.prev_randao), _u64_chunk(x.block_number),
+            _u64_chunk(x.gas_limit), _u64_chunk(x.gas_used), _u64_chunk(x.timestamp),
+            sha256(bytes(x.extra_data).ljust(32, b"\0") + len(x.extra_data).to_bytes(32, "little")),      # ByteList[32]: one chunk
+            int(x.base_fee_per_gas).to_bytes(32, "little"), bytes(x.block_hash), bytes(x.transactions_root)])
+        votes = np.frombuffer(b"".join(eth1_root(v) for v in state.eth1_data_votes), dtype=np.uint8)
+        justification = sum(1 << i for i, b in enumerate(state.justification_bits) if b)
+        fields = [
+            _u64_chunk(state.genesis_time),
+            bytes(state.genesis_validators_root),
+            _u64_chunk(state.slot),
+            _merkle([bytes(state.fork.previous_version).ljust(32, b"\0"), bytes(state.fork.current_version).ljust(32, b"\0"),
+                     _u64_chunk(state.fork.epoch)]),
+            _merkle([_u64_chunk(h.slot), _u64_chunk(h.proposer_index), bytes(h.parent_root), bytes(h.state_root), bytes(h.body_root)]),
+            roots(state.block_roots, p.SLOTS_PER_HISTORICAL_ROOT, _chunk_depth(p.SLOTS_PER_HISTORICAL_ROOT, 32)),
+            roots(state.state_roots, p.SLOTS_PER_HISTORICAL_ROOT, _chunk_depth(p.SLOTS_PER_HISTORICAL_ROOT, 32)),
+            roots(state.historical_roots, None, _chunk_depth(p.HISTORICAL_ROOTS_LIMIT, 32), as_list=True),
+            eth1_root(e1),
+            eng.ssz_chunks_root(votes, _chunk_depth(p.EPOCHS_PER_ETH1_VOTING_PERIOD * p.SLOTS_PER_EPOCH, 32), len(state.eth1_data_votes)),
+            _u64_chunk(state.eth1_deposit_index),
+            self.validators_root(state),
+            basic_list(state.balances, "<u8"),
+            roots(state.randao_mixes, p.EPOCHS_PER_HISTORICAL_VECTOR, _chunk_depth(p.EPOCHS_PER_HISTORICAL_VECTOR, 32)),
+            eng.ssz_chunks_root(slashings, _chunk_depth(p.EPOCHS_PER_SLASHINGS_VECTOR, 8)),
+            basic_list(state.previous_epoch_participation, np.uint8),
+            basic_list(state.current_epoch_participation, np.uint8),
+            justification.to_bytes(32, "little"),
+            hash_tree_root_checkpoint(state.previous_justified_checkpoint),
+            hash_tree_root_checkpoint(state.current_justified_checkpoint),
+            hash_tree_root_checkpoint(state.finalized_checkpoint),
+            basic_list(state.inactivity_scores, "<u8"),
+            sync_committee(state.current_sync_committee),
+            sync_committee(state.next_sync_committee),
+            payload_header,
+        ]
+        return _merkle(fields)

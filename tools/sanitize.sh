@@ -4,7 +4,7 @@
 #   1. compute-sanitizer --tool memcheck   over the small-configuration GPU tests (every kernel, out-of-bounds / misaligned accesses)
 #   2. compute-sanitizer --tool racecheck  over the tests whose kernels share data through shared memory: the 3-lane team pairing
 #      (__syncwarp between phases), the TMA-staged gather (mbarrier + cp.async.bulk), the vote scatter's shared bins, the tree kernel,
-#      the block packer's per-committee fold and greedy
+#      the block packer's per-committee fold and greedy, the SSZ leaf staging and subtree reduction
 #   3. compute-sanitizer --tool synccheck  on the same subset (illegal barrier use)
 #   4. the host side of the C ABI under AddressSanitizer + UBSan (pos_evolution_b200/libb200pos_asan.so, built by
 #      `python -m pos_evolution_b200.build --asan`) over the BLS / fork-choice / guard / error-contract tests
@@ -13,8 +13,8 @@ cd "$(dirname "$0")/.."
 OUT="${OUT:-$(mktemp -d)}"
 mkdir -p "$OUT"
 SAN=/usr/local/cuda/bin/compute-sanitizer
-SMALL="tests/test_gpu_bls.py tests/test_gpu_bls_adversarial.py tests/test_gpu_aggregate_verify.py tests/test_gpu_sync_aggregate.py tests/test_gpu_forkchoice.py tests/test_gpu_gather.py tests/test_gpu_participation.py tests/test_gpu_epoch.py tests/test_gpu_slasher.py tests/test_gpu_epoch_slasher.py tests/test_gpu_pack.py"
-RACE="tests/test_gpu_bls.py::test_fast_aggregate_verify_vs_oracle tests/test_gpu_bls.py::test_g1_aggregate_all_minimal_committees tests/test_gpu_forkchoice.py tests/test_gpu_gather.py tests/test_gpu_pack.py::test_pack_matches_oracle"
+SMALL="tests/test_gpu_bls.py tests/test_gpu_bls_adversarial.py tests/test_gpu_aggregate_verify.py tests/test_gpu_sync_aggregate.py tests/test_gpu_forkchoice.py tests/test_gpu_gather.py tests/test_gpu_participation.py tests/test_gpu_epoch.py tests/test_gpu_slasher.py tests/test_gpu_epoch_slasher.py tests/test_gpu_pack.py tests/test_gpu_ssz.py::test_validators_load tests/test_gpu_ssz.py::test_incremental_updates"
+RACE="tests/test_gpu_bls.py::test_fast_aggregate_verify_vs_oracle tests/test_gpu_bls.py::test_g1_aggregate_all_minimal_committees tests/test_gpu_forkchoice.py tests/test_gpu_gather.py tests/test_gpu_pack.py::test_pack_matches_oracle tests/test_gpu_ssz.py::test_validators_load"
 run() {  # name, timeout, command...
     local name=$1 tmo=$2; shift 2
     echo "== $name"
