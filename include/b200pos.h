@@ -293,6 +293,24 @@ int b2_tree_load(b2_ctx* ctx, const uint32_t* parent, const uint64_t* slot, cons
 int b2_get_weights(b2_ctx* ctx, int32_t boost_idx, uint64_t boost_score, uint64_t* weight_out);
 /* get_head (pos-evolution.md:1102-1116): index of the head block */
 int b2_get_head(b2_ctx* ctx, uint32_t justified_idx, int32_t boost_idx, uint64_t boost_score, uint32_t* head_idx_out);
+/* ---- changing the loaded tree on the device, without a reload.  After any sequence of these calls the context behaves exactly like
+ * b2_tree_load of the resulting arrays (parent, root, leaf_viable in id order): the same kernel form, weights, heads and tie-breaks.
+ * Each call is synchronous.  A rejected call (B2_EINVAL: no tree loaded, k == 0, a parent >= its own id, a prune root or a viability
+ * index >= n) changes nothing.  A change of size needs b2_fc_exchange_export / _open again before b2_get_head_multi.
+ *   b2_tree_add        on_block adds a block to store.blocks (pos-evolution.md:1015-1018): appends k blocks, which take ids n .. n+k-1;
+ *                      parent[j] < n + j, so a batch may parent within itself.  The arrays are those of b2_tree_load.
+ *   b2_tree_prune      the finalized checkpoint moves (:1033-1036): keeps the subtree of new_root, which becomes id 0; the kept blocks
+ *                      keep their order (parents still precede children).  map_out (the old n entries) receives map[old] = new id, or
+ *                      0xFFFFFFFF for a dropped block.  Every validator's latest-message block is re-mapped through it; the message
+ *                      epochs and equivocation flags are untouched, and a vote for a dropped block counts nowhere.  The re-map runs on
+ *                      the context's own stream: device-pointer work the caller queued on its streams that reads or writes the
+ *                      latest messages or a vote vector (b2_latest_messages_update_dev, b2_vote_weights_*dev, b2_epoch_*_dev) must be
+ *                      complete before the call.
+ *   b2_tree_set_viable the get_filtered_block_tree leaf test (:1104): sets the viability byte of blocks idx[0..k) (only leaves' bytes
+ *                      matter, as in b2_tree_load; a repeated index keeps its last value). */
+int b2_tree_add(b2_ctx* ctx, const uint32_t* parent, const uint64_t* slot, const uint8_t* root32, const uint8_t* leaf_viable, uint32_t k);
+int b2_tree_prune(b2_ctx* ctx, uint32_t new_root, uint32_t* map_out);
+int b2_tree_set_viable(b2_ctx* ctx, const uint32_t* idx, const uint8_t* viable, uint32_t k);
 
 /* ---- device-pointer entry points (asynchronous on `stream`) ------------------------------------------------------
  * The host cannot read what device pointers point to, so the checks the host entry points make before touching anything
@@ -369,7 +387,8 @@ int b2_head_from_votes_dev(b2_ctx* ctx, uint64_t* d_votes_preorder, uint32_t jus
  *   b2_get_head_multi      COLLECTIVE (every rank, same order): scatter the votes of this rank's validators [v_begin, v_end),
  *                          push the per-block sums into every rank's accumulator with 64-bit reductions over NVLink, flag
  *                          exchange, tree phase on the complete accumulator; returns the same head on every rank.
- * One process per GPU, at most 8 ranks, all on one NVLink/NVSwitch domain.  Re-export after b2_tree_load. */
+ * One process per GPU, at most 8 ranks, all on one NVLink/NVSwitch domain.  Re-export after b2_tree_load and after a b2_tree_add /
+ * b2_tree_prune that changed the tree's size: until then b2_get_head_multi refuses (B2_EINVAL). */
 int b2_fc_exchange_export(b2_ctx* ctx, uint8_t* handle64_out);
 int b2_fc_exchange_open(b2_ctx* ctx, int rank, int world, const uint8_t* handles64);
 int b2_get_head_multi(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, uint32_t justified_idx, int32_t boost_idx, uint64_t boost_score,

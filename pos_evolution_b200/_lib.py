@@ -79,6 +79,9 @@ SIGNATURES = {
                                          c_void_p, c_uint32, c_uint32, c_uint64, c_uint64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_tree_load": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32]),
+    "b2_tree_add": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32]),
+    "b2_tree_prune": (c_int, [c_void_p, c_uint32, c_void_p]),
+    "b2_tree_set_viable": (c_int, [c_void_p, c_void_p, c_void_p, c_uint32]),
     "b2_get_weights": (c_int, [c_void_p, c_int32, c_uint64, c_void_p]),
     "b2_get_head": (c_int, [c_void_p, c_uint32, c_int32, c_uint64, c_void_p]),
     "b2_aggregate_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_uint32, c_uint64, c_void_p, c_void_p, c_void_p]),

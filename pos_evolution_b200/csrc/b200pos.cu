@@ -19,6 +19,7 @@
 #include "slasher.cuh"
 #include "pack.cuh"
 #include "ssz.cuh"
+#include "tree.cuh"
 
 using namespace b2;
 
@@ -75,6 +76,10 @@ struct tree_tables {
     dbuf packed;                                      // shared-memory form: u32 size | rank << 15 | keep << 31
     dbuf size_keep, rank, next;                       // generic form: u32 size | keep << 31, u32 root rank, u32[n+1] marks
     dbuf prefix, w2;                                  // generic form: u64[n+1] prefix sums, u64 weights
+    // per block id, so that b2_tree_add / _prune / _set_viable change the tree on the device (tree.cuh); `pre` above is per id too
+    dbuf size, rank_id, parent, root, viable;         // u32 subtree size, u32 rank of (root, id), u32 parent, u8[32] root, u8 viability
+    dbuf pre_b, size_b, rank_b, parent_b, root_b, viable_b;      // the other side of the out-of-place steps (prune, grid insert)
+    dbuf scan, scan2, map;                            // u32[n+1] prefix-count scratch, u32[n] prune map
 };
 
 // sync committees (b2_sync_committee_load): n committees of `size` keys, replaced together
@@ -1819,7 +1824,15 @@ int b2_tree_load(b2_ctx* ctx, const uint32_t* parent, const uint64_t* slot, cons
     if (!smem && ((rc = ensure(ctx, t.size_keep, n4)) || (rc = ensure(ctx, t.rank, n4)) || (rc = ensure(ctx, t.next, n4 + 4)) ||
                   (rc = ensure(ctx, t.prefix, n8 + 8)) || (rc = ensure(ctx, t.w2, n8))))
         return rc;
+    if ((rc = ensure(ctx, t.size, n4)) || (rc = ensure(ctx, t.rank_id, n4)) || (rc = ensure(ctx, t.parent, n4)) || (rc = ensure(ctx, t.root, 32ull * n)) ||
+        (rc = ensure(ctx, t.viable, n)))
+        return rc;
     cudaStream_t s = ctx->s_main;
+    CK(cudaMemcpyAsync(t.size, size.data(), n4, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(t.rank_id, rank.data(), n4, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(t.parent, parent, n4, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(t.root, root32, 32ull * n, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(t.viable, leaf_viable, n, cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(t.pre, pre.data(), n4, cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(t.inv, inv.data(), n4, cudaMemcpyHostToDevice, s));
     if (smem) {
@@ -1833,6 +1846,136 @@ int b2_tree_load(b2_ctx* ctx, const uint32_t* parent, const uint64_t* slot, cons
     ctx->tree = std::move(t);
     ctx->n_blocks = n;
     return B2_OK;
+}
+
+// Room for a change from n_old blocks to n, all or nothing: every buffer too small for it is first allocated anew (geometrically, so
+// one block per slot does not reallocate each time) with the live contents copied over -- the per-id state and the tables of the current
+// form keep their n_old entries -- and only once every allocation has succeeded do the new buffers replace the old ones.  A failed
+// allocation therefore leaves the tree exactly as it was.  The scratch holds max(n_old, n) entries; the tables of n's form are
+// re-emitted after the change.
+static int tree_reserve(b2_ctx* ctx, uint32_t n_old, uint32_t n) {
+    tree_tables& t = ctx->tree;
+    const size_t k4 = (size_t)n_old * 4, m = std::max(n_old, n), m4 = m * 4, n4 = (size_t)n * 4, n8 = (size_t)n * 8;
+    const bool smem = tree_form_of(n).smem_tree;
+    struct want {
+        dbuf* b;
+        size_t keep, need;
+    };
+    const want all[] = {{&t.pre, k4, m4}, {&t.size, k4, m4}, {&t.rank_id, k4, m4}, {&t.parent, k4, m4}, {&t.root, 32 * (size_t)n_old, 32 * m},
+                        {&t.viable, n_old, m}, {&t.pre_b, 0, m4}, {&t.size_b, 0, m4}, {&t.rank_b, 0, m4}, {&t.parent_b, 0, m4},
+                        {&t.root_b, 0, 32 * m}, {&t.viable_b, 0, m}, {&t.scan, 0, m4 + 4}, {&t.scan2, 0, m4 + 4}, {&t.map, 0, m4},
+                        {&t.inv, k4, n4}, {&t.votes, 8 * (size_t)std::min(n_old, n), n8}, {&t.weight, 0, n8},
+                        {&t.packed, k4, smem ? n4 : 0}, {&t.size_keep, k4, smem ? 0 : n4}, {&t.rank, k4, smem ? 0 : n4},
+                        {&t.next, 0, smem ? 0 : n4 + 4}, {&t.prefix, 0, smem ? 0 : n8 + 8}, {&t.w2, 0, smem ? 0 : n8}};
+    constexpr size_t N_BUF = sizeof(all) / sizeof(all[0]);
+    dbuf fresh[N_BUF];
+    for (size_t i = 0; i < N_BUF; i++) {
+        const dbuf& b = *all[i].b;
+        if (!all[i].need || (b.p && all[i].need <= b.cap)) continue;
+        const size_t bytes = std::max<size_t>({all[i].need, 2 * b.cap, 256}), keep = b.p ? std::min(all[i].keep, b.cap) : 0;
+        CK(cudaMalloc(&fresh[i].p, bytes));
+        fresh[i].cap = bytes;
+        if (keep) CK(cudaMemcpyAsync(fresh[i].p, b.p, keep, cudaMemcpyDeviceToDevice, ctx->s_main));
+    }
+    for (size_t i = 0; i < N_BUF; i++)
+        if (fresh[i]) *all[i].b = std::move(fresh[i]);
+    return B2_OK;
+}
+
+static tree_ids ids_of(tree_tables& t, bool other) {
+    return other ? tree_ids{t.pre_b, t.size_b, t.rank_b, t.parent_b, t.root_b, t.viable_b} : tree_ids{t.pre, t.size, t.rank_id, t.parent, t.root, t.viable};
+}
+
+// re-emits the tables of the form of an n-block tree, waits for the change, and makes n the tree's size
+static int tree_emit(b2_ctx* ctx, uint32_t n) {
+    tree_tables& t = ctx->tree;
+    const tree_form f = tree_form_of(n);
+    k_tree_emit<<<1, 1024, 0, ctx->s_main>>>(t.pre, t.size, t.rank_id, t.viable, n, t.scan, t.inv, f.smem_tree ? (uint32_t*)t.packed : nullptr,
+                                             t.size_keep, t.rank);
+    CKL(ctx);
+    CK(cudaStreamSynchronize(ctx->s_main));
+    t.form = f;
+    ctx->n_blocks = n;
+    return B2_OK;
+}
+
+int b2_tree_add(b2_ctx* ctx, const uint32_t* parent, const uint64_t* slot, const uint8_t* root32, const uint8_t* leaf_viable, uint32_t k) {
+    B2_NVTX;
+    REQUIRE(ctx && parent && slot && root32 && leaf_viable, "tree_add: bad arguments");
+    REQUIRE(ctx->n_blocks > 0, "tree_add: no tree loaded (b2_tree_load)");
+    const uint32_t n0 = ctx->n_blocks;
+    REQUIRE(k > 0 && k < 0xffffffffu - n0, "tree_add: k must be at least 1 and the tree below 2^32 - 1 blocks");
+    for (uint32_t j = 0; j < k; j++) REQUIRE(parent[j] < n0 + j, "tree_add: a block's parent must precede it (parent < id)");
+    CK(cudaSetDevice(ctx->device));
+    const uint32_t n = n0 + k;
+    int rc;
+    if ((rc = tree_reserve(ctx, n0, n))) return rc;
+    tree_tables& t = ctx->tree;
+    cudaStream_t s = ctx->s_main;
+    // the new blocks' inputs go past the current n, where nothing reads them until the change is complete
+    CK(cudaMemcpyAsync((uint32_t*)t.parent + n0, parent, (size_t)k * 4, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync((uint8_t*)t.root + 32ull * n0, root32, 32ull * k, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync((uint8_t*)t.viable + n0, leaf_viable, k, cudaMemcpyHostToDevice, s));
+    CK(cudaMemsetAsync((uint64_t*)t.votes + n0, 0, (size_t)k * 8, s));      // the vote accumulator is clean between calls
+    if (tree_form_of(n).smem_tree) {
+        k_tree_insert_cta<<<1, 1024, 0, s>>>(t.pre, t.size, t.parent, n0, k);
+        CKL(ctx);
+    } else {
+        for (uint32_t j = 0; j < k; j++) {
+            k_tree_insert_grid<<<blocks_for(n0 + j + 1, 256), 256, 0, s>>>(t.pre, t.size, t.size_b, parent[j], n0 + j);
+            CKL(ctx);
+            std::swap(t.size, t.size_b);
+        }
+    }
+    k_tree_rank_old<<<blocks_for(n0, 256), 256, 0, s>>>(t.root, t.rank_id, n0, n);
+    CKL(ctx);
+    k_tree_rank_new<<<k, 256, 0, s>>>(t.root, t.rank_id, n0, n);
+    CKL(ctx);
+    return tree_emit(ctx, n);
+}
+
+int b2_tree_prune(b2_ctx* ctx, uint32_t new_root, uint32_t* map_out) {
+    B2_NVTX;
+    REQUIRE(ctx && map_out, "tree_prune: bad arguments");
+    REQUIRE(ctx->n_blocks > 0, "tree_prune: no tree loaded (b2_tree_load)");
+    const uint32_t n0 = ctx->n_blocks;
+    REQUIRE(new_root < n0, "tree_prune: new root out of range");
+    CK(cudaSetDevice(ctx->device));
+    tree_tables& t = ctx->tree;
+    uint32_t n = 0;      // the kept subtree's size decides the new form, so it is read before anything is allocated
+    CK(cudaMemcpy(&n, (uint32_t*)t.size + new_root, 4, cudaMemcpyDeviceToHost));
+    int rc;
+    if ((rc = tree_reserve(ctx, n0, n))) return rc;
+    cudaStream_t s = ctx->s_main;
+    k_tree_prune<<<1, 1024, 0, s>>>(ids_of(t, false), ids_of(t, true), n0, new_root, t.scan, t.scan2, t.map);
+    CKL(ctx);
+    if (ctx->n_val > 0) {
+        k_lmd_remap<<<blocks_for(ctx->n_val, 256), 256, 0, s>>>(ctx->reg.lmd_block, ctx->n_val, t.map, n0);
+        CKL(ctx);
+    }
+    std::swap(t.pre, t.pre_b), std::swap(t.size, t.size_b), std::swap(t.rank_id, t.rank_b);
+    std::swap(t.parent, t.parent_b), std::swap(t.root, t.root_b), std::swap(t.viable, t.viable_b);
+    CK(cudaMemcpyAsync(map_out, t.map, (size_t)n0 * 4, cudaMemcpyDeviceToHost, s));
+    return tree_emit(ctx, n);
+}
+
+int b2_tree_set_viable(b2_ctx* ctx, const uint32_t* idx, const uint8_t* viable, uint32_t k) {
+    B2_NVTX;
+    REQUIRE(ctx && idx && viable, "tree_set_viable: bad arguments");
+    REQUIRE(ctx->n_blocks > 0, "tree_set_viable: no tree loaded (b2_tree_load)");
+    REQUIRE(k > 0, "tree_set_viable: k must be at least 1");
+    for (uint32_t j = 0; j < k; j++) REQUIRE(idx[j] < ctx->n_blocks, "tree_set_viable: block index out of range");
+    CK(cudaSetDevice(ctx->device));
+    const uint32_t n = ctx->n_blocks;
+    int rc;
+    if ((rc = tree_reserve(ctx, n, n))) return rc;
+    staging st(ctx);
+    const uint32_t* didx = st.in(idx, k);
+    const uint8_t* dval = st.in(viable, k);
+    if (st.rc) return st.rc;
+    k_tree_set_viable<<<1, 1, 0, ctx->s_main>>>(ctx->tree.viable, didx, dval, k);
+    CKL(ctx);
+    return tree_emit(ctx, n);
 }
 
 // the vote scatter's view of the validators [v_begin, v_end) under the context's fork-choice variant

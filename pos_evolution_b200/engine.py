@@ -440,6 +440,33 @@ class Engine:
         self._ck(self.lib.b2_tree_load(self.h, _p(parent), _p(slot), _p(roots), _p(viable), n))
         self.n_blocks = n
 
+    def tree_add(self, parent, slot, roots32, leaf_viable):
+        """Append k blocks to the loaded tree (ids n .. n+k-1, parent[j] < n + j); the arrays are those of tree_load."""
+        parent, slot = _c(parent, np.uint32), _c(slot, np.uint64)
+        roots = _c(roots32, np.uint8).reshape(-1, 32)
+        viable = _c(leaf_viable, np.uint8)
+        k = parent.shape[0]
+        assert slot.shape == (k,) and roots.shape[0] == k and viable.shape == (k,)
+        self._ck(self.lib.b2_tree_add(self.h, _p(parent), _p(slot), _p(roots), _p(viable), k))
+        self.n_blocks += k
+
+    def tree_prune(self, new_root: int):
+        """Keep the subtree of block new_root, which becomes id 0; the latest messages are re-mapped on the device.  Returns the
+        uint32 map old id -> new id (0xFFFFFFFF for a dropped block)."""
+        m = np.zeros(self.n_blocks, dtype=np.uint32)
+        self._ck(self.lib.b2_tree_prune(self.h, int(new_root), _p(m)))
+        self.n_blocks = self.tree_size()
+        return m
+
+    def tree_set_viable(self, idx, viable):
+        """Set the leaf-viability byte of blocks idx (the get_filtered_block_tree test)."""
+        idx, viable = _c(idx, np.uint32), _c(viable, np.uint8)
+        assert idx.shape == viable.shape and idx.ndim == 1
+        self._ck(self.lib.b2_tree_set_viable(self.h, _p(idx), _p(viable), idx.shape[0]))
+
+    def tree_size(self) -> int:
+        return int(self.lib.b2_tree_size(self.h))
+
     def get_weights(self, boost_idx: int = -1, boost_score: int = 0):
         w = np.zeros(self.n_blocks, dtype=np.uint64)
         self._ck(self.lib.b2_get_weights(self.h, int(boost_idx), int(boost_score), _p(w)))

@@ -290,12 +290,48 @@ class EpochProcessor:
         self.fused_head_error = why
         return self._fused_head
 
+    # ------------------------------------------------------------------ changing the block tree between batches
+    def _check_tree(self):
+        """The vote scatter writes one entry per block of the engine's tree into d_votes: refuse before anything is enqueued when the
+        tree's size is not the one d_votes was sized for (a tree_load behind the processor's back; add_blocks / prune_tree re-size it)."""
+        if isinstance(self.eng, Engine) and self.eng.tree_size() != self.d_votes.numel():
+            raise ValueError("the engine's tree has %d blocks but this EpochProcessor's vote vector %d: change the tree through "
+                             "add_blocks / prune_tree" % (self.eng.tree_size(), self.d_votes.numel()))
+
+    def _tree_changed(self):
+        n = self.eng.tree_size()
+        if n != self.d_votes.numel():
+            self.d_votes = self._zeros(n, torch.int64)
+            self.n_blocks = n
+            self._fused_head = False          # the NVLink exchange block is sized by the tree: enable_fused_get_head again
+        return n
+
+    def add_blocks(self, parent, slot, roots32, leaf_viable):
+        """Engine.tree_add between batches (on_block); needs a drained pipeline."""
+        assert not self._inflight, "submitted epochs are in flight: drain() first"
+        self.eng.tree_add(parent, slot, roots32, leaf_viable)
+        self._tree_changed()
+
+    def prune_tree(self, new_root):
+        """Engine.tree_prune between batches (finalization): returns the map old id -> new id; block indices of later epochs use the new
+        ids.  Needs a drained pipeline."""
+        assert not self._inflight, "submitted epochs are in flight: drain() first"
+        m = self.eng.tree_prune(new_root)
+        self._tree_changed()
+        return m
+
+    def set_viable(self, idx, viable):
+        """Engine.tree_set_viable between batches; needs a drained pipeline."""
+        assert not self._inflight, "submitted epochs are in flight: drain() first"
+        self.eng.tree_set_viable(idx, viable)
+
     def get_head(self, justified_idx=0, boost_idx=-1, boost_score=0, fused=None):
         """get_head over the current LMD table through the multi-rank path; returns the head index on the host.  COLLECTIVE.
         fused (default: whether enable_fused_get_head was called): one kernel per rank -- vote scatter of this rank's validators,
         64-bit reductions into every rank's accumulator over NVLink, flag exchange, tree phase, zero-copy result.  Otherwise the
         three-stage form: scatter kernel, NCCL all-reduce of u64[n_blocks], tree kernel, device-to-host copy.  Needs a drained pipeline."""
         assert not self._inflight, "submitted epochs are in flight: drain() first"
+        self._check_tree()
         if fused is None:
             fused = getattr(self, "_fused_head", False)
         if fused:
@@ -374,6 +410,7 @@ class EpochProcessor:
         """d_sigs: this rank's signatures (all of them when not sharded); every other array covers the whole epoch.  With the slasher
         on: source_epoch int64[n_agg] (device) and the current epoch; the findings are read with slashings().  Needs a drained pipeline."""
         assert not self._inflight, "submitted epochs are in flight: drain() first"
+        self._check_tree()
         self._slasher_args(source_epoch, current_epoch)
         s = self.slots[0]
         self._epoch(s, (d_sigs, d_bits, d_msgs, d_target_epoch, d_block_idx, source_epoch), (justified_idx, boost_idx, boost_score), False,
@@ -386,6 +423,7 @@ class EpochProcessor:
         source_epoch int64[n_agg] (pinned host) and the current epoch; the findings are read with slashings().  Needs a drained
         pipeline."""
         assert not self._inflight, "submitted epochs are in flight: drain() first"
+        self._check_tree()
         self._slasher_args(source_epoch, current_epoch)
         s = self.slots[0]
         x = self._stage(s, True, h_sigs, h_bits, h_msgs, h_target_epoch, h_block_idx, source_epoch)
@@ -422,6 +460,7 @@ class EpochProcessor:
         calls earlier (None while the pipeline fills).  `last=True` says no further epoch follows soon: its pairing tail is
         enqueued in the short-critical-path (team) form.  With the slasher on: source_epoch int64[n_agg] (device) and the
         current epoch; the slasher reads copies of the bits, messages and epochs, so the inputs are free after wait() as without it."""
+        self._check_tree()
         self._slasher_args(source_epoch, current_epoch)
         s = self._claim_slot(torch.cuda.current_stream())
         x = self._stage(s, False, d_sigs, d_bits, d_msgs, d_target_epoch, d_block_idx, source_epoch)
@@ -432,6 +471,7 @@ class EpochProcessor:
         """Pinned host tensors in (untouched until the returned-later ticket has been waited for).  The H2D copies go on a
         separate stream so that they overlap with the epochs in flight.  With the slasher on: source_epoch int64[n_agg] (pinned
         host) and the current epoch; the status and flagged count of every epoch come back in pinned buffers."""
+        self._check_tree()
         self._slasher_args(source_epoch, current_epoch)
         cur = torch.cuda.current_stream()
         with torch.cuda.stream(self.copy_stream):

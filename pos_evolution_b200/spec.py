@@ -341,9 +341,13 @@ def pack_bits(rows, stride=None) -> np.ndarray:
 class Spec:
     """pyspec functions bound to a preset and a GPU engine."""
 
-    def __init__(self, preset: Preset = MAINNET, engine: Engine = None):
+    def __init__(self, preset: Preset = MAINNET, engine: Engine = None, incremental_tree: bool = False):
+        """incremental_tree: keep the device block tree current across new blocks and finalization (Engine.tree_add / tree_prune /
+        tree_set_viable, rooted at the finalized block) instead of re-uploading the store whenever its blocks or checkpoints change
+        (see _sync_store).  Heads and weights are the same either way."""
         self.p = preset
         self.engine = engine if engine is not None else Engine(0)
+        self.incremental_tree = incremental_tree
         self._registry_key = None          # (length, fingerprint of the pubkey bytes) of the registry on the device
         self._balances_key = None          # (state object, slot) whose effective balances / flags are on the device
         self._balances_state = None
@@ -356,7 +360,7 @@ class Spec:
         self._ssz_load_id = None           # engine.ssz_loads after this Spec's last load: another load replaced the tree when it differs
         self._slasher = None               # slasher_start: size and current epoch of the device history, accepted attestations by target epoch
         self.stats = {"registry_uploads": 0, "balance_refreshes": 0, "store_uploads": 0, "lmd_device_updates": 0, "sync_committee_uploads": 0,
-                      "ssz_validator_loads": 0, "ssz_validator_updates": 0}
+                      "ssz_validator_loads": 0, "ssz_validator_updates": 0, "tree_adds": 0, "tree_prunes": 0, "viability_updates": 0}
         # full: fingerprint = hash of ALL pubkeys on every call (O(n) host work, catches any in-place replacement);
         # sampled: first / last / 62 strided pubkeys (O(1)); auto: full up to 65 536 validators, sampled above
         self.registry_check = "auto"
@@ -894,7 +898,9 @@ class Spec:
                 store.latest_messages[i] = LatestMessage(epoch=target.epoch, root=root)
         m = self._mirror
         if m is not None and m["store"] is store:
-            blk = m["index"].get(root)
+            if self.incremental_tree and root not in m["index"] and root in store.blocks:
+                self._sync_blocks(store, m)          # a vote for a block on_block added since the last get_head
+            blk = m["index"].get(root) if self._mirror is m else None
             if blk is None or not indices or max(indices) >= m["n_val"] or target.epoch >= 0xFFFFFFFF:
                 self._mirror = None                  # a vote the device form cannot hold: fall back to a full re-upload
             else:
@@ -1033,14 +1039,24 @@ class Spec:
                     out.append(AttesterSlashing(pair[0], pair[1]))
         return out
 
-    def _store_arrays(self, store):
-        """Store (dicts) -> the array form of include/b200pos.h: blocks below the justified root in topological order."""
+    def _tree_root(self, store):
+        """The root of the incremental device tree: the finalized checkpoint's block when the justified block descends from it, else
+        the justified block (a store whose checkpoints are not on one chain)."""
+        froot, jroot = store.finalized_checkpoint.root, store.justified_checkpoint.root
+        r = jroot
+        while froot in store.blocks and r in store.blocks and store.blocks[r].slot > store.blocks[froot].slot:
+            r = store.blocks[r].parent_root
+        return froot if r == froot else jroot
+
+    def _store_arrays(self, store, root=None):
+        """Store (dicts) -> the array form of include/b200pos.h: `root` (default: the justified root) and the blocks below it in
+        topological order."""
         import collections
-        jroot = store.justified_checkpoint.root
+        root = store.justified_checkpoint.root if root is None else root
         children = {}
         for r, b in store.blocks.items():
             children.setdefault(b.parent_root, []).append(r)
-        order, queue = [], collections.deque([jroot])
+        order, queue = [], collections.deque([root])
         while queue:
             r = queue.popleft()
             order.append(r)
@@ -1056,28 +1072,101 @@ class Spec:
             if i:
                 parent[i] = index[b.parent_root]
             if r not in children:
-                hs = store.block_states[r]
-                cj = store.justified_checkpoint.epoch == GENESIS_EPOCH or hs.current_justified_checkpoint == store.justified_checkpoint
-                cf = store.finalized_checkpoint.epoch == GENESIS_EPOCH or hs.finalized_checkpoint == store.finalized_checkpoint
-                viable[i] = 1 if (cj and cf) else 0
+                viable[i] = self._leaf_viable(store, r)
         roots = np.frombuffer(b"".join(order), dtype=np.uint8).reshape(nb, 32)
         return order, index, parent, slot, roots, viable
 
+    @staticmethod
+    def _leaf_viable(store, root):                                             # the leaf test of get_filtered_block_tree (:1104)
+        hs = store.block_states[root]
+        cj = store.justified_checkpoint.epoch == GENESIS_EPOCH or hs.current_justified_checkpoint == store.justified_checkpoint
+        cf = store.finalized_checkpoint.epoch == GENESIS_EPOCH or hs.finalized_checkpoint == store.finalized_checkpoint
+        return 1 if (cj and cf) else 0
+
+    def _sync_blocks(self, store, m):
+        """incremental_tree: bring the device tree up to store.blocks without a reload.  The blocks on_block added since the last call
+        (in store order, so parents first) are appended with one tree_add; a finalized checkpoint that moved to a block of the tree is
+        applied with tree_prune, whose map re-numbers the mirror (the device re-maps the latest messages itself).  Blocks that do not
+        descend from the tree's root are not mirrored.  A finalized block outside the tree drops the mirror (full reload)."""
+        index, order, kids = m["index"], m["order"], m["kids"]
+        if len(store.blocks) != m["n_seen"]:
+            par, slot, roots, via = [], [], [], []
+            for r, b in list(store.blocks.items())[m["n_seen"]:]:
+                if r in index or b.parent_root not in index:
+                    continue
+                p = index[b.parent_root]
+                index[r] = len(order)
+                order.append(r)
+                kids.append(0)
+                kids[p] += 1
+                par.append(p)
+                slot.append(b.slot)
+                roots.append(r)
+                via.append(self._leaf_viable(store, r))
+            m["n_seen"] = len(store.blocks)
+            if par:
+                self.engine.tree_add(par, slot, np.frombuffer(b"".join(roots), dtype=np.uint8), via)
+                m["viable"].update(zip(range(len(order) - len(par), len(order)), via))
+                m["boost"] = None
+                self.stats["tree_adds"] += 1
+        if store.finalized_checkpoint != m["finalized"]:
+            froot = store.finalized_checkpoint.root
+            if froot not in index:
+                self._mirror = None
+                return
+            if index[froot] != 0:
+                mp = self.engine.tree_prune(index[froot])
+                keep = np.nonzero(mp != 0xFFFFFFFF)[0]
+                m["order"] = order = [order[i] for i in keep]
+                m["index"] = {r: i for i, r in enumerate(order)}
+                m["kids"] = [kids[i] for i in keep]
+                m["viable"] = {int(mp[i]): v for i, v in m["viable"].items() if mp[i] != 0xFFFFFFFF}
+                m["boost"] = None
+                self.stats["tree_prunes"] += 1
+            m["finalized"] = store.finalized_checkpoint
+
+    def _refresh_viability(self, store, m):
+        """incremental_tree: every leaf's test reads the checkpoints, so when they move the leaves whose byte changed are sent"""
+        cps = (store.justified_checkpoint, store.finalized_checkpoint)
+        if m["checkpoints"] == cps:
+            return
+        m["checkpoints"] = cps
+        changed = []
+        for i, r in enumerate(m["order"]):
+            if m["kids"][i] == 0:
+                v = self._leaf_viable(store, r)
+                if m["viable"].get(i) != v:
+                    m["viable"][i] = v
+                    changed.append((i, v))
+        if changed:
+            idx, val = zip(*changed)
+            self.engine.tree_set_viable(idx, val)
+            self.stats["viability_updates"] += 1
+
     def _sync_store(self, store):
-        """Device mirror of the store: block tree (b2_tree_load) and latest messages (b2_latest_messages_load) are uploaded when the
-        store's SHAPE changed -- another store object, justified / finalized checkpoint moved, a block was added (on_block), the
-        registry changed, or latest_messages / equivocating_indices were changed behind this class's back (their sizes differ from
-        what the mirror recorded).  Votes that arrive through on_attestation / update_latest_messages are applied to the device
-        table incrementally, so between blocks get_head / get_weight cost one kernel sequence."""
+        """Device mirror of the store: block tree (b2_tree_load) and latest messages (b2_latest_messages_load) are uploaded for another
+        store object, a registry change, or latest_messages / equivocating_indices changed behind this class's back (their sizes differ
+        from what the mirror recorded).  Without incremental_tree they are also uploaded when the justified / finalized checkpoint moved
+        or a block was added (on_block); the tree is then rooted at the justified block.  With incremental_tree the tree is rooted at
+        the finalized block: new blocks, finalization and leaf viability are applied on the device (_sync_blocks, _refresh_viability)
+        and the latest messages are never re-uploaded for them; a justified block outside the tree, or a vote for a block the tree
+        does not hold, falls back to the full upload.  Votes that arrive through on_attestation / update_latest_messages are applied
+        to the device table incrementally, so between blocks get_head / get_weight cost one kernel sequence.
+        Returns (order, index, justified block id, boost id, boost score)."""
         state = store.checkpoint_states[store.justified_checkpoint]
         self.sync_registry(state)
         m = self._mirror
-        live = (m is not None and m["store"] is store and m["justified"] == store.justified_checkpoint and m["finalized"] == store.finalized_checkpoint
-                and m["n_blocks"] == len(store.blocks) and m["n_msgs"] == len(store.latest_messages) and m["n_equiv"] == len(store.equivocating_indices)
+        inc = self.incremental_tree
+        live = (m is not None and m["store"] is store and m["n_msgs"] == len(store.latest_messages) and m["n_equiv"] == len(store.equivocating_indices)
                 and m["n_val"] == len(state.validators))
+        if live and not inc:
+            live = m["justified"] == store.justified_checkpoint and m["finalized"] == store.finalized_checkpoint and m["n_seen"] == len(store.blocks)
+        if live and inc:
+            self._sync_blocks(store, m)
+            live = self._mirror is m and store.justified_checkpoint.root in m["index"]
         if not live:
-            order, index, parent, slot, roots, viable = self._store_arrays(store)
-            self.engine.tree_load(parent, slot, roots, viable)
+            order, index, parent, slot, roots, via = self._store_arrays(store, self._tree_root(store) if inc else None)
+            self.engine.tree_load(parent, slot, roots, via)
             n = len(state.validators)
             epoch = np.zeros(n, dtype=np.uint64)
             blk = np.zeros(n, dtype=np.uint32)
@@ -1090,10 +1179,14 @@ class Spec:
                 if v < n:
                     eq[v] = 1
             self.engine.latest_messages_load(epoch, blk, has, eq)
-            m = self._mirror = dict(store=store, justified=store.justified_checkpoint, finalized=store.finalized_checkpoint, n_blocks=len(store.blocks),
+            kids = np.bincount(parent[1:], minlength=len(order)).tolist()
+            m = self._mirror = dict(store=store, justified=store.justified_checkpoint, finalized=store.finalized_checkpoint, n_seen=len(store.blocks),
                                     n_msgs=len(store.latest_messages), n_equiv=len(store.equivocating_indices), n_val=n, order=order, index=index,
-                                    boost=None)
+                                    kids=kids, viable={i: int(via[i]) for i in range(len(order)) if kids[i] == 0},
+                                    checkpoints=(store.justified_checkpoint, store.finalized_checkpoint), boost=None)
             self.stats["store_uploads"] += 1
+        if inc:
+            self._refresh_viability(store, m)
         bkey = (store.proposer_boost_root, self._balances_key)
         if m["boost"] is None or m["boost"][0] != bkey:
             boost_idx, boost_score = -1, 0
@@ -1103,17 +1196,17 @@ class Spec:
                 boost_score = (num // self.p.SLOTS_PER_EPOCH) * avg * self.p.PROPOSER_SCORE_BOOST // 100
                 boost_idx = m["index"][store.proposer_boost_root]
             m["boost"] = (bkey, boost_idx, boost_score)
-        return m["order"], m["index"], m["boost"][1], m["boost"][2]
+        return m["order"], m["index"], m["index"][store.justified_checkpoint.root], m["boost"][1], m["boost"][2]
 
     def get_latest_attesting_balance(self, store, root):                       # called at :1116 (v1.2.0 form)
-        order, index, boost_idx, boost_score = self._sync_store(store)
+        order, index, justified, boost_idx, boost_score = self._sync_store(store)
         return int(self.engine.get_weights(boost_idx, boost_score)[index[root]])
 
     get_weight = get_latest_attesting_balance
 
     def get_head(self, store):                                                 # :1102-1116
-        order, index, boost_idx, boost_score = self._sync_store(store)
-        return order[self.engine.get_head(0, boost_idx, boost_score)]
+        order, index, justified, boost_idx, boost_score = self._sync_store(store)
+        return order[self.engine.get_head(justified, boost_idx, boost_score)]
 
     # ------------------------------------------------------------------ hash_tree_root(state) (:423, :1078)
     def validators_root(self, state) -> bytes:
