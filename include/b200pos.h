@@ -247,6 +247,30 @@ int b2_slasher_update_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t
                           uint32_t n_agg, int32_t* d_att_status_out, uint8_t* d_kind_out, uint32_t* d_conflict_target_out,
                           uint32_t* d_n_flagged_out, void* stream);
 
+/* ---- equivocation discounting (pos-evolution.md:1405-1461): what the slasher found stops counting in the fork choice.
+ * b2_slasher_discount_dev: for every member slot i < n_slots with d_kind[i] != 0 (the d_kind_out of a b2_slasher_update_dev, members
+ *   parallel to it), validator d_members[i] joins Store.equivocating_indices -- what on_attester_slashing (:1447-1461) adds for every
+ *   AttesterSlashing formable from two accepted aggregates, whose attesting indices intersect in exactly the flagged validators.  From
+ *   then on the validator neither moves its latest message (b2_latest_messages_update*, :1435-1441) nor counts in any get_head form (:1411).
+ *   d_new_out[i] = 1 for exactly one slot of every validator this call newly marked (0 where it was marked before, by this call's other
+ *   slots or earlier: b2_on_attester_slashing, b2_latest_messages_load, an earlier discount), d_n_new_out = how many.  Only validators of
+ *   the slasher's range (b2_slasher_init_range) and of the registry are marked.  Asynchronous on `stream`; the tables are never un-marked
+ *   (b2_registry_load and b2_latest_messages_load/_reset replace them).  Epoch tails (b2_epoch_tail_dev, b2_epoch_dev) enqueued after this
+ *   call apply their latest messages only after it: enqueue the discount of epoch k before the tail of epoch k+1.
+ *   B2_EINVAL, with nothing enqueued, on bad arguments, no registry or no slasher. */
+int b2_slasher_discount_dev(b2_ctx* ctx, const uint32_t* d_members, const uint8_t* d_kind, uint64_t n_slots, uint8_t* d_new_out,
+                            uint32_t* d_n_new_out, void* stream);
+/* the same on host arrays (returns when done) */
+int b2_slasher_discount(b2_ctx* ctx, const uint32_t* members, const uint8_t* kind, uint64_t n_slots, uint8_t* new_out, uint32_t* n_new_out);
+/* Store.equivocating_indices as u8[n_validators] (nonzero = equivocating), after every mark enqueued so far (:1405-1461) */
+int b2_equivocating_read(b2_ctx* ctx, uint8_t* out, uint64_t n_validators);
+/* Sharded registries (pos-evolution.md:1405-1461): rank g discounts the validators of its slasher range only, so the ranks' replicas of
+ * the table are brought together by exchanging range slices.  _slice_dev copies the table's bytes [v_begin, v_end) to d_out;
+ * _merge_dev ORs d_table[0 .. v_end - v_begin) into them.  Both asynchronous on `stream`; a merge orders later epoch tails like a discount.
+ * B2_EINVAL unless v_begin < v_end <= n_validators of the loaded registry. */
+int b2_equivocating_slice_dev(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, uint8_t* d_out, void* stream);
+int b2_equivocating_merge_dev(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, const uint8_t* d_table, void* stream);
+
 /* ---- block packing: BeaconBlockBody.attestations (List[Attestation, MAX_ATTESTATIONS], pos-evolution.md:639; "well-packed aggregate
  * attestations", :659) chosen from a pool, the proposing-side counterpart of process_attestation (:722-754).
  * Committee k = members[committee_off[k] .. committee_off[k+1]) with participation table committee_table[k] (0 current, 1 previous; the

@@ -72,7 +72,12 @@ SIGNATURES = {
                                   c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_slasher_update_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32,
                                       c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
-    "b2_pack_attestations": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p,
+    "b2_slasher_discount_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_uint64, c_void_p, c_void_p, c_void_p]),
+    "b2_slasher_discount": (c_int, [c_void_p, c_void_p, c_void_p, c_uint64, c_void_p, c_void_p]),
+    "b2_equivocating_read": (c_int, [c_void_p, c_void_p, c_uint64]),
+    "b2_equivocating_slice_dev": (c_int, [c_void_p, c_uint64, c_uint64, c_void_p, c_void_p]),
+    "b2_equivocating_merge_dev": (c_int, [c_void_p, c_uint64, c_uint64, c_void_p, c_void_p]),
+    "b2_pack_attestations":(c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p,
                                      c_uint32, c_uint32, c_uint64, c_uint64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                      c_void_p, c_void_p]),
     "b2_pack_attestations_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p, c_uint32,

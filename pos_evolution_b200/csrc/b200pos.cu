@@ -141,6 +141,7 @@ struct b2_ctx {
     int dec_alternate = -1;                           // -1 auto, 0 never, 1 always
     unsigned dec_turn = 0;
     cudaEvent_t ev_votes_done = nullptr, ev_lmd_done = nullptr;
+    cudaEvent_t ev_equiv_done = nullptr;             // the last equivocation mark enqueued (b2_slasher_discount_dev, b2_equivocating_merge_dev)
     vslot slot[B2_EPOCH_SLOTS];
     char err[512] = {0};
     uint64_t launches = 0;
@@ -342,6 +343,7 @@ int b2_init(int device, b2_ctx** out) {
     for (int k = 0; k < 3 && e == cudaSuccess; k++) e = cudaEventCreateWithFlags(&ctx->ev_av[k], cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_lmd_done, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_votes_done, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_equiv_done, cudaEventDisableTiming);
     for (int i = 0; i < B2_EPOCH_SLOTS && e == cudaSuccess; i++) {
         cudaEvent_t* evs[6] = {&ctx->slot[i].ev_join0, &ctx->slot[i].ev_join1, &ctx->slot[i].ev_seg, &ctx->slot[i].ev_tail_done, &ctx->slot[i].ev_fork,
                                &ctx->slot[i].ev_in};
@@ -411,6 +413,7 @@ void b2_destroy(b2_ctx* ctx) {
         if (ctx->ev_av[k]) cudaEventDestroy(ctx->ev_av[k]);
     if (ctx->ev_lmd_done) cudaEventDestroy(ctx->ev_lmd_done);
     if (ctx->ev_votes_done) cudaEventDestroy(ctx->ev_votes_done);
+    if (ctx->ev_equiv_done) cudaEventDestroy(ctx->ev_equiv_done);
     if (ctx->h_head) cudaFreeHost((void*)ctx->h_head);
     delete ctx;      // frees every device buffer
 }
@@ -448,7 +451,8 @@ int b2_registry_load(b2_ctx* ctx, const uint8_t* pk48, const uint64_t* eff, cons
     registry_tables t;
     int rc;
     if ((rc = ensure(ctx, t.records, n * 96)) || (rc = ensure(ctx, t.valid, n)) || (rc = ensure(ctx, t.eff, n * 8)) || (rc = ensure(ctx, t.flags, n)) ||
-        (rc = ensure(ctx, t.lmd_key, n * 8)) || (rc = ensure(ctx, t.lmd_block, n * 4)) || (rc = ensure(ctx, t.equiv, n)))
+        (rc = ensure(ctx, t.lmd_key, n * 8)) || (rc = ensure(ctx, t.lmd_block, n * 4)) ||
+        (rc = ensure(ctx, t.equiv, (n + 3) & ~3ull)))      // whole words: k_slasher_discount marks by a 32-bit atomicOr
         return rc;
     staging st(ctx);
     const uint8_t* d_pk = st.in(pk48, n * 48);
@@ -827,6 +831,7 @@ static int epoch_tail(b2_ctx* ctx, int slot, const uint32_t* d_members, const ui
     if (d_target_epoch) {
         CK(cudaStreamWaitEvent(t, ctx->ev_votes_done, 0));  // do not move the LMD table under a vote scatter that is still reading it
         CK(cudaStreamWaitEvent(t, ctx->ev_lmd_done, 0));    // latest messages are applied in epoch order even when tails overlap
+        CK(cudaStreamWaitEvent(t, ctx->ev_equiv_done, 0));  // ... and skip every validator the epochs before this one were found to equivocate
         if ((rc = b2_latest_messages_update_dev(ctx, d_members, d_off, d_bits, bits_stride, d_target_epoch, d_block_idx, d_ok_out, n_agg, t))) return rc;
         CK(cudaEventRecord(ctx->ev_lmd_done, t));
     }   // else: the caller applies update_latest_messages itself, after exchanging the verdicts of all ranks (sharded epoch)
@@ -1616,6 +1621,69 @@ int b2_slasher_update(b2_ctx* ctx, const uint32_t* members, const uint32_t* off,
         (rc = b2_slasher_update_dev(ctx, dm, dof, db, bits_stride, dse, dte, droot, dacc, n_agg, dst, dkind, dconf, dflag, ctx->s_main)))
         return rc;
     return st.finish();
+}
+
+// ------------------------------------------------------------------------------------------ equivocation discounting (:1405-1461)
+int b2_slasher_discount_dev(b2_ctx* ctx, const uint32_t* d_members, const uint8_t* d_kind, uint64_t n_slots, uint8_t* d_new_out,
+                            uint32_t* d_n_new_out, void* stream) {
+    B2_NVTX;
+    REQUIRE(ctx && d_members && d_kind && d_new_out && d_n_new_out && n_slots > 0 && n_slots < (1ull << 32), "slasher_discount_dev: bad arguments");
+    REQUIRE(ctx->n_val > 0, "slasher_discount: registry not loaded");
+    REQUIRE(ctx->sl.H, "slasher_discount: no slasher (b2_slasher_init)");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    const slasher_tables& t = ctx->sl;
+    CK(cudaMemsetAsync(d_n_new_out, 0, 4, s));
+    k_slasher_discount<<<blocks_for(n_slots, 256), 256, 0, s>>>(d_members, d_kind, n_slots, ctx->n_val, t.v_begin, t.n_rows, ctx->reg.equiv,
+                                                                d_new_out, d_n_new_out);
+    CKL(ctx);
+    CK(cudaEventRecord(ctx->ev_equiv_done, s));      // the next epoch tail's LMD update waits for it
+    return B2_OK;
+}
+
+int b2_slasher_discount(b2_ctx* ctx, const uint32_t* members, const uint8_t* kind, uint64_t n_slots, uint8_t* new_out, uint32_t* n_new_out) {
+    B2_NVTX;
+    REQUIRE(ctx && members && kind && new_out && n_new_out && n_slots > 0 && n_slots < (1ull << 32), "slasher_discount: bad arguments");
+    REQUIRE(ctx->n_val > 0, "slasher_discount: registry not loaded");
+    REQUIRE(ctx->sl.H, "slasher_discount: no slasher (b2_slasher_init)");
+    CK(cudaSetDevice(ctx->device));
+    staging st(ctx);
+    const uint32_t* dm = st.in(members, n_slots);
+    const uint8_t* dk = st.in(kind, n_slots);
+    uint8_t* dnew = st.out(new_out, n_slots);
+    uint32_t* dn = st.out(n_new_out, 1);
+    int rc;
+    if ((rc = st.rc) || (rc = b2_slasher_discount_dev(ctx, dm, dk, n_slots, dnew, dn, ctx->s_main))) return rc;
+    return st.finish();
+}
+
+int b2_equivocating_read(b2_ctx* ctx, uint8_t* out, uint64_t n_validators) {
+    B2_NVTX;
+    REQUIRE(ctx && out && n_validators == ctx->n_val && n_validators > 0, "equivocating_read: bad arguments / registry size");
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaStreamWaitEvent(ctx->s_main, ctx->ev_equiv_done, 0));      // the marks enqueued on other streams so far
+    staging st(ctx);
+    st.out(out, ctx->reg.equiv, n_validators);
+    return st.finish();
+}
+
+int b2_equivocating_slice_dev(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, uint8_t* d_out, void* stream) {
+    B2_NVTX;
+    REQUIRE(ctx && d_out && v_begin < v_end && v_end <= ctx->n_val, "equivocating_slice_dev: bad arguments / registry not loaded");
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaMemcpyAsync(d_out, (const uint8_t*)ctx->reg.equiv + v_begin, v_end - v_begin, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    return B2_OK;
+}
+
+int b2_equivocating_merge_dev(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, const uint8_t* d_table, void* stream) {
+    B2_NVTX;
+    REQUIRE(ctx && d_table && v_begin < v_end && v_end <= ctx->n_val, "equivocating_merge_dev: bad arguments / registry not loaded");
+    CK(cudaSetDevice(ctx->device));
+    cudaStream_t s = (cudaStream_t)stream;
+    k_equiv_merge<<<blocks_for(v_end - v_begin, 256), 256, 0, s>>>(d_table, v_begin, v_end - v_begin, ctx->reg.equiv);
+    CKL(ctx);
+    CK(cudaEventRecord(ctx->ev_equiv_done, s));
+    return B2_OK;
 }
 
 // ------------------------------------------------------------------------------------------ block packing (pack.cuh)

@@ -215,6 +215,37 @@ __global__ void __launch_bounds__(128) k_slasher_check(slasher_view S, const uin
     }
 }
 
+// Equivocation discounting (pos-evolution.md:1405-1461): thread per member slot of an update (after its k_slasher_check).  A flagged
+// slot (kind != 0) marks its validator in the registry's equivocating table, so that from then on it neither moves its latest message
+// (k_lmd_phase1/2) nor counts in a head.  Marks are set by atomicOr on the aligned 32-bit word holding v's byte (the table is padded to
+// whole words), so exactly one slot -- the one that turned v's byte from 0 to nonzero -- reports v as newly marked, however many slots
+// flag v and whether or not v was marked before; newly marked slots are counted with one atomic per warp.  Only validators of the
+// slasher's rows [v_begin, v_begin + n_rows) can be flagged; the range test keeps a stray kind byte outside it from marking anything.
+__global__ void __launch_bounds__(256) k_slasher_discount(const uint32_t* __restrict__ members, const uint8_t* __restrict__ kind, uint64_t n_slots,
+                                                           uint64_t n_val, uint32_t v_begin, uint64_t n_rows, uint8_t* equiv, uint8_t* new_out,
+                                                           uint32_t* n_new) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    bool fresh = false;
+    if (i < n_slots) {
+        const uint32_t v = kind[i] ? members[i] : 0xffffffffu;
+        if (v < n_val && (uint32_t)(v - v_begin) < n_rows) {
+            const uint32_t shift = 8u * (v & 3u);
+            const uint32_t old = atomicOr(reinterpret_cast<uint32_t*>(equiv + (v & ~3u)), 1u << shift);
+            fresh = ((old >> shift) & 0xffu) == 0;
+        }
+        new_out[i] = fresh;
+    }
+    const unsigned m = __ballot_sync(B2_FULL_MASK, fresh);
+    if (m && (threadIdx.x & 31) == 0) atomicAdd(n_new, (uint32_t)__popc(m));
+}
+
+// Thread per validator of a range [v_begin, v_begin + n): equiv[v] |= table[v - v_begin] -- one rank's slice of the equivocating table
+// merged into another rank's replica (sharded epochs).  A byte has one writer, so no atomics.
+__global__ void __launch_bounds__(256) k_equiv_merge(const uint8_t* __restrict__ table, uint64_t v_begin, uint64_t n, uint8_t* equiv) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && table[i]) equiv[v_begin + i] |= table[i];
+}
+
 // The window moves up: the columns of the epochs first .. first + n_cols - 1 (n_cols < H) become empty
 __global__ void __launch_bounds__(256) k_slasher_advance(slasher_view S, uint32_t first, uint32_t n_cols) {
     const uint64_t total = S.n_rows * n_cols;

@@ -391,6 +391,25 @@ class Engine:
                                             _p(status), _p(kind), _p(conflict), ctypes.byref(flagged)))
         return status, kind, conflict, int(flagged.value)
 
+    # ------------------------------------------------------------------ equivocation discounting (pos-evolution.md:1405-1461)
+    def slasher_discount(self, members, kind):
+        """Every validator with a flagged member slot (kind != 0, the kind vector of slasher_update, members parallel to it) joins
+        Store.equivocating_indices: its votes stop counting.  -> (new uint8[len(kind)]: 1 on exactly one slot of each validator this
+        call newly marked, n_new)."""
+        k = _c(kind, np.uint8)
+        m = _c(members, np.uint32)[:k.shape[0]]
+        assert m.shape == k.shape
+        new = np.zeros(k.shape[0], dtype=np.uint8)
+        n_new = ctypes.c_uint32(0)
+        self._ck(self.lib.b2_slasher_discount(self.h, _p(m), _p(k), k.shape[0], _p(new), ctypes.byref(n_new)))
+        return new, int(n_new.value)
+
+    def equivocating(self):
+        """Store.equivocating_indices as uint8[n_validators] (nonzero = equivocating)"""
+        out = np.zeros(self.n_validators, dtype=np.uint8)
+        self._ck(self.lib.b2_equivocating_read(self.h, _p(out), self.n_validators))
+        return out
+
     # ------------------------------------------------------------------ block packing (BeaconBlockBody.attestations, pos-evolution.md:639)
     def pack_attestations(self, members, committee_off, committee_table, cand_committee, cand_data, cand_flag_mask, bits, sigs96, max_out: int,
                           increment: int, base_reward_per_increment: int) -> "PackResult":
@@ -556,6 +575,20 @@ class Engine:
                                                 d_accept.data_ptr() if d_accept is not None else None, n_agg, d_status.data_ptr(),
                                                 d_kind.data_ptr(), d_conflict.data_ptr() if d_conflict is not None else None,
                                                 d_n_flagged.data_ptr(), self._stream()))
+
+    def slasher_discount_dev(self, d_members, d_kind, d_new, d_n_new):
+        """b2_slasher_discount_dev on the current stream: d_members uint32 and d_kind uint8 (slasher_update_dev's) per member slot ->
+        d_new uint8 per slot, d_n_new uint32[1]"""
+        self._ck(self.lib.b2_slasher_discount_dev(self.h, d_members.data_ptr(), d_kind.data_ptr(), d_kind.numel(), d_new.data_ptr(),
+                                                  d_n_new.data_ptr(), self._stream()))
+
+    def equivocating_slice_dev(self, v_begin: int, v_end: int, d_out):
+        """the equivocating table's bytes [v_begin, v_end) -> d_out (uint8 device tensor), on the current stream"""
+        self._ck(self.lib.b2_equivocating_slice_dev(self.h, int(v_begin), int(v_end), d_out.data_ptr(), self._stream()))
+
+    def equivocating_merge_dev(self, v_begin: int, v_end: int, d_table):
+        """equivocating[v_begin:v_end] |= d_table[:v_end - v_begin], on the current stream"""
+        self._ck(self.lib.b2_equivocating_merge_dev(self.h, int(v_begin), int(v_end), d_table.data_ptr(), self._stream()))
 
     def epoch_dev(self, d_sigs, d_members, d_off, d_bits, d_msgs, d_target_epoch, d_block_idx, d_agg_sig, d_agg_status, d_ok):
         n_agg = d_off.numel() - 1

@@ -33,6 +33,12 @@ Slashing detection (`enable_slasher`): after each epoch's fork choice, on the fo
 (include/b200pos.h, b2_slasher_*) records and checks every accepted aggregate of the epoch; `Ticket.slashings()` reports the flagged
 member slots.  Sharded, rank g holds the history of validators [g*N/world, (g+1)*N/world) only -- the range of its vote scatter --
 and reports those; the ranks' reports together are the unsharded one, with no collective added.
+
+Equivocation discounting (`enable_slasher(..., discount=True)`, pos-evolution.md:1405-1461): right after each epoch's slasher update,
+every validator it flagged joins the device's Store.equivocating_indices, so from the next epoch on its votes neither move its latest
+message nor count in a head (:1411: votes of validators "not viewed to have equivocated at previous slots").  The marks only grow.
+Sharded, rank g marks its own range; each rank's slice of the table is then all-gathered and merged into every replica, on the
+fork-choice stream before the next epoch's exchange, so the replicas of the LMD table stay identical.
 """
 import collections
 import contextlib
@@ -73,12 +79,14 @@ class _Slot:
         # pipelined forms: the fork choice (+ D2H) and the slasher update of the epoch that last used the slot
         self.ev_fc = self.ev_sl = None
 
-    def enable_slasher(self, ep):
+    def enable_slasher(self, ep, discount):
         z, h = ep._zeros, ep._pinned
         self.src = z(ep.n_agg, torch.int64)
         self.sl_status, self.sl_kind = z(ep.n_agg, torch.int32), z(ep.n_sig, torch.uint8)
         self.sl_conflict, self.sl_flagged = z((ep.n_sig, 2), torch.int32), z(1, torch.int32)
         self.h_sl_status, self.h_sl_flagged = h(ep.n_agg, torch.int32), h(1, torch.int32)
+        if discount:      # per member slot: 1 where the discount newly marked its validator; how many
+            self.sl_new, self.sl_n_new, self.h_sl_n_new = z(ep.n_sig, torch.uint8), z(1, torch.int32), h(1, torch.int32)
 
 
 class _Ticket:
@@ -111,6 +119,12 @@ class _Ticket:
         assert self.slasher_event is not None, "no slasher: EpochProcessor.enable_slasher"
         self.slasher_event.synchronize()
         return int((self._slot.h_sl_flagged if self._host else self._slot.sl_flagged)[0])
+
+    def discounted(self):
+        """The validators this epoch's discount newly marked as equivocating, sorted (int64 numpy array; waits for the slasher's update);
+        enable_slasher(..., discount=True) first."""
+        assert self.slasher_event is not None and self._ep.discount, "no discount: EpochProcessor.enable_slasher(..., discount=True)"
+        return self._ep._read_discounted(self._slot, self._host, self.slasher_event)
 
 
 class EpochProcessor:
@@ -159,6 +173,7 @@ class EpochProcessor:
         # ... except at the end of a batch: the last `team_last` epochs take the team form (see drain_hint)
         self.team_last = 1
         self.slasher = False          # enable_slasher
+        self.discount = False
 
     def _zeros(self, shape, dtype):
         return torch.zeros(shape, dtype=dtype, device=self.dev)
@@ -185,20 +200,28 @@ class EpochProcessor:
         return sigs[self.m0:self.m1]
 
     # ------------------------------------------------------------------ slashing detection
-    def enable_slasher(self, history_epochs: int, max_attestations_per_target: int = None, current_epoch: int = 0):
+    def enable_slasher(self, history_epochs: int, max_attestations_per_target: int = None, current_epoch: int = 0, discount: bool = False):
         """Detect the double and surround votes of every accepted aggregate of every epoch processed from now on, against a history of
         `history_epochs` epochs on the device (Engine.slasher_init; B2Error(B2_ENOMEM) without allocating when it does not fit).
         Unsharded the history covers the whole registry; sharded, this rank's validators [v0, v1) only (6 * (v1 - v0) * H bytes).
         max_attestations_per_target defaults to 2 * n_agg (at most 65535).  Every entry point then needs source_epoch (per aggregate)
         and current_epoch (the slasher's window moves to it before the epoch's update).
         The slasher is fed the epoch's signing roots as attestation roots, so it must not be shared with Spec.find_attester_slashings,
-        which feeds data roots, on the same Engine."""
+        which feeds data roots, on the same Engine.
+        discount: every validator the slasher flags in an epoch becomes equivocating on the device right after that epoch's update
+        (Engine.slasher_discount_dev, pos-evolution.md:1405-1461), so it counts in no head and moves no latest message from the next
+        epoch on; Ticket.discounted() / discounted() name the newly marked validators, equivocating() reads the table."""
         n_val = self.n_val if self.n_val is not None else self.eng.n_validators
         v0, v1 = (self.v0, self.v1) if self.sharded else (0, n_val)
         K = min(2 * self.n_agg, 65535) if max_attestations_per_target is None else int(max_attestations_per_target)
         self.eng.slasher_init(n_val, history_epochs, K, current_epoch, v_begin=v0, v_end=v1)
         for s in self.slots:
-            s.enable_slasher(self)
+            s.enable_slasher(self, discount)
+        if discount and self.sharded and self.pg is not None:
+            # this rank's slice of the equivocating table, padded to the longest range, and every rank's after the all-gather
+            width = -(-n_val // self.world)
+            self._eq_loc, self._eq_all = self._zeros(width, torch.uint8), self._zeros((self.world, width), torch.uint8)
+        self.discount = bool(discount)
         self.sl_range = (v0, v1)
         self._sl_cur = self._sl_next = int(current_epoch)
         self.slasher = True
@@ -226,6 +249,44 @@ class EpochProcessor:
         if host:
             s.h_sl_status.copy_(s.sl_status, non_blocking=True)
             s.h_sl_flagged.copy_(s.sl_flagged, non_blocking=True)
+
+    def _discount(self, s, host):
+        """On the current stream, after the epoch's slasher update: mark every flagged validator as equivocating.  Sharded, every rank
+        marks its own range only; the ranks' range slices of the table are all-gathered and each other rank's range merged, so every
+        replica holds the same table before the next epoch's exchange applies its latest messages."""
+        e = self.eng
+        e.slasher_discount_dev(self.d_members, s.sl_kind, s.sl_new, s.sl_n_new)
+        if self.sharded and self.pg is not None:      # (bench.py --emulate-world: one rank on its own, nothing to gather)
+            e.equivocating_slice_dev(self.v0, self.v1, self._eq_loc)
+            torch.distributed.all_gather_into_tensor(self._eq_all.view(-1), self._eq_loc, group=self.pg)
+            for g in range(self.world):
+                if g != self.rank:
+                    v0, v1 = g * self.n_val // self.world, (g + 1) * self.n_val // self.world
+                    e.equivocating_merge_dev(v0, v1, self._eq_all[g])
+        if host:
+            s.h_sl_n_new.copy_(s.sl_n_new, non_blocking=True)
+
+    def _read_discounted(self, s, host, event=None):
+        if event is not None:
+            event.synchronize()
+        elif self.dev.type == "cuda":
+            torch.cuda.current_stream().synchronize()
+        n = int((s.h_sl_n_new if host else s.sl_n_new)[0])
+        if n == 0:
+            return np.zeros(0, dtype=np.int64)
+        new = s.sl_new[:int(self.h_off[-1])].cpu().numpy()
+        return np.sort(self.h_members[np.nonzero(new)[0]])
+
+    def discounted(self):
+        """The validators the last epoch of process_epoch_dev / process_epoch_host newly marked as equivocating, sorted (synchronises the
+        current stream)."""
+        assert self.discount, "no discount: enable_slasher(..., discount=True)"
+        return self._read_discounted(self.slots[0], False)
+
+    def equivocating(self):
+        """Store.equivocating_indices as uint8[n_validators] (nonzero = equivocating).  Needs a drained pipeline."""
+        assert not self._inflight, "submitted epochs are in flight: drain() first"
+        return self.eng.equivocating()
 
     def _read_slashings(self, s, host, event=None):
         """the findings in slot s as a Slashings tuple; kind and conflict targets cross to the host only when something was flagged"""
@@ -401,6 +462,8 @@ class EpochProcessor:
                 s.ev_fc = self._record()
             if self.slasher:                              # after the head: the head's latency does not include it
                 self._slasher_update(s, bits, msgs, src, tgt, current_epoch, host)
+                if self.discount:                         # before the next epoch's LMD update and head (the library orders its tail)
+                    self._discount(s, host)
                 if pipelined:
                     s.ev_sl = self._record()
 
@@ -500,5 +563,6 @@ class EpochProcessor:
     @property
     def d2h_bytes(self):
         """device -> host bytes per epoch (submit_host): verdicts + head index + the aggregate signatures (+ the slasher's statuses and
-        flagged count; its kind and conflict targets only when something was flagged)"""
-        return self.slots[0].h_ok.numel() + 4 + self.slots[0].h_agg_sig.numel() + ((4 * self.n_agg + 4) if self.slasher else 0)
+        flagged count, and with the discount its newly-marked count; its kind and conflict targets only when something was flagged)"""
+        return (self.slots[0].h_ok.numel() + 4 + self.slots[0].h_agg_sig.numel() + ((4 * self.n_agg + 4) if self.slasher else 0) +
+                (4 if self.discount else 0))
