@@ -392,6 +392,35 @@ int b2_epoch_wait_dev(b2_ctx* ctx, int slot, void* stream);
  * (fewest instructions: right while further epochs keep the chip busy), 1 = three lanes per pairing (shortest critical path: right for
  * the last epochs of a batch, whose tails drain with nothing left to overlap).  The synchronous entry points always use form 1. */
 int b2_epoch_set_pairing_form(b2_ctx* ctx, int form);
+/* ---- vote form of an epoch: committees whose members signed different AttestationData (pos-evolution.md:714-717 Attestation, :722-754
+ * process_attestation; a split committee is what proposer boost and equivocation discounting exist to defeat).  Committee c has members
+ * d_members[d_off[c] .. d_off[c+1]) and the vote ids [d_vote_off[c], d_vote_off[c+1]) (strictly increasing, d_vote_off[0] = 0,
+ * d_vote_off[n_committees] = n_votes: every committee has at least one id, a committee where nobody attested one placeholder).
+ * d_vote[j] = the id member j signed, or 0xFFFFFFFF if it did not attest.  b2_votes_group_dev stable-sorts each committee's positions
+ * by vote, one CTA per committee, keeping committee order within a vote; non-attesters go last and belong to the committee's last vote.
+ * Outputs, the arrays b2_epoch_dev / b2_epoch_start_dev / _tail_dev, b2_latest_messages_update_dev (update_latest_messages, :1435-1441)
+ * and the slasher take with n_agg = n_votes:
+ *   d_members_out u32[n_sig], d_pos_out u32[n_sig]  the grouped members and the committee position each came from;
+ *   d_seg_off u32[n_votes+1]                         vote v = grouped slots [d_seg_off[v], d_seg_off[v+1]), inside its committee's
+ *                                                    range: d_seg_off[d_vote_off[c]] = d_off[c], d_seg_off[n_votes] = d_off[n_committees];
+ *   d_bits_out u8[n_votes][bits_stride]              the first count_v bits set (count_v = the vote's attesters);
+ *   d_agg_bits_out u8[n_votes][bits_stride]          the vote's aggregation_bits over committee positions;
+ *   d_sig96_out                                      the signatures of committees [c_begin, c_end) grouped (index 0 = d_off[c_begin],
+ *                                                    as d_sig96), a non-attester's slot replaced by the infinity encoding 0xc0 || 0^95;
+ *   d_seg_off_loc (may be NULL) u32[...]             d_seg_off of the votes [d_vote_off[c_begin], d_vote_off[c_end)] minus d_off[c_begin]:
+ *                                                    the offsets of one rank's committees over its own signatures.
+ * With one vote per committee and everyone attesting the outputs equal the inputs.  Self-guarding: an id outside its committee's
+ * range (not 0xFFFFFFFF) counts as not attesting (B2_GUARD_BAD_INDEX); a malformed d_vote_off empties every vote of the call, and a
+ * committee row that is reversed, ends past n_sig, exceeds 8 * bits_stride members or votes, or (within [c_begin, c_end)) leaves the
+ * range's signatures empties that committee's votes (B2_GUARD_BAD_ROW); nothing is read or written out of bounds.  b2_votes_empty_dev
+ * then makes every vote without attester (bit 0 of its d_bits_out row clear) read like an empty segment after the epoch: status 2 and
+ * 96 zero bytes (its verdict is 0 and it moves no latest message anyway).  Both asynchronous on `stream`; bits_stride <= 256. */
+int b2_votes_group_dev(b2_ctx* ctx, const uint32_t* d_vote, const uint32_t* d_vote_off, uint32_t n_votes, const uint32_t* d_members, const uint32_t* d_off,
+                       uint32_t n_committees, uint64_t n_sig, uint32_t bits_stride, const uint8_t* d_sig96, uint32_t c_begin, uint32_t c_end,
+                       uint8_t* d_sig96_out, uint32_t* d_members_out, uint32_t* d_pos_out, uint32_t* d_seg_off, uint32_t* d_seg_off_loc,
+                       uint8_t* d_bits_out, uint8_t* d_agg_bits_out, void* stream);
+int b2_votes_empty_dev(b2_ctx* ctx, const uint8_t* d_bits, uint32_t bits_stride, uint32_t n_votes, uint8_t* d_agg_sig96, int32_t* d_agg_status,
+                       void* stream);
 int b2_latest_messages_update_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_off, const uint8_t* d_bits,
                                   uint32_t bits_stride, const uint64_t* d_target_epoch, const uint32_t* d_block_idx,
                                   const uint8_t* d_accept, uint32_t n_agg, void* stream);

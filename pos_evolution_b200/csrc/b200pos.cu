@@ -20,6 +20,7 @@
 #include "pack.cuh"
 #include "ssz.cuh"
 #include "tree.cuh"
+#include "votes.cuh"
 
 using namespace b2;
 
@@ -875,6 +876,31 @@ int b2_epoch_tail_dev(b2_ctx* ctx, int slot, const uint32_t* d_members, const ui
     CK(cudaSetDevice(ctx->device));
     return epoch_tail(ctx, slot, d_members, d_off, d_bits, bits_stride, d_target_epoch, d_block_idx, n_agg, d_agg_sig96, d_agg_status, d_ok_out,
                       ctx->slot[slot].s_tail, ctx->epoch_team);
+}
+// Vote form of the epoch (votes.cuh): group the members and signatures by vote so that the epoch entry points run one segment per vote.
+int b2_votes_group_dev(b2_ctx* ctx, const uint32_t* d_vote, const uint32_t* d_vote_off, uint32_t n_votes, const uint32_t* d_members, const uint32_t* d_off,
+                       uint32_t n_committees, uint64_t n_sig, uint32_t bits_stride, const uint8_t* d_sig96, uint32_t c_begin, uint32_t c_end,
+                       uint8_t* d_sig96_out, uint32_t* d_members_out, uint32_t* d_pos_out, uint32_t* d_seg_off, uint32_t* d_seg_off_loc,
+                       uint8_t* d_bits_out, uint8_t* d_agg_bits_out, void* stream) {
+    B2_NVTX;
+    REQUIRE(ctx && d_vote && d_vote_off && d_members && d_off && d_sig96 && d_sig96_out && d_members_out && d_pos_out && d_seg_off && d_bits_out &&
+                d_agg_bits_out && n_votes > 0 && n_committees > 0 && n_sig < (1ull << 32) && bits_stride > 0 && bits_stride <= 256 &&
+                c_begin < c_end && c_end <= n_committees,
+            "votes_group_dev: bad arguments");
+    CK(cudaSetDevice(ctx->device));
+    vote_group_args A = {d_vote, d_vote_off, d_off, d_members, n_committees, n_votes, bits_stride, n_sig, d_sig96, c_begin, c_end, d_sig96_out,
+                    d_members_out, d_pos_out, d_seg_off, d_seg_off_loc, d_bits_out, d_agg_bits_out, ctx->d_guard};
+    k_votes_group<<<n_committees, VOTES_THREADS, 0, (cudaStream_t)stream>>>(A);
+    CKL(ctx);
+    return B2_OK;
+}
+int b2_votes_empty_dev(b2_ctx* ctx, const uint8_t* d_bits, uint32_t bits_stride, uint32_t n_votes, uint8_t* d_agg_sig96, int32_t* d_agg_status, void* stream) {
+    B2_NVTX;
+    REQUIRE(ctx && d_bits && d_agg_sig96 && n_votes > 0 && bits_stride > 0, "votes_empty_dev: bad arguments");
+    CK(cudaSetDevice(ctx->device));
+    k_votes_empty<<<blocks_for((uint64_t)n_votes * 24, 256), 256, 0, (cudaStream_t)stream>>>(d_bits, bits_stride, n_votes, d_agg_sig96, d_agg_status);
+    CKL(ctx);
+    return B2_OK;
 }
 int b2_epoch_set_pairing_form(b2_ctx* ctx, int form) {
     B2_NVTX;

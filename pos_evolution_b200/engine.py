@@ -610,6 +610,26 @@ class Engine:
                                             d_block_idx.data_ptr() if d_block_idx is not None else None, n_agg, d_agg_sig.data_ptr(),
                                             d_agg_status.data_ptr(), d_ok.data_ptr()))
 
+    def votes_group_dev(self, d_vote, d_vote_off, d_members, d_off, d_sigs, c_begin, c_end, d_sigs_out, d_members_out, d_pos_out, d_seg_off,
+                        d_bits_out, d_agg_bits_out, d_seg_off_loc=None):
+        """b2_votes_group_dev on the current stream: group committee order by vote (include/b200pos.h).  d_vote uint32[n_sig], d_vote_off
+        uint32[n_committees+1], d_members / d_off the committees; d_sigs / d_sigs_out uint8[*, 96] the signatures of committees [c_begin,
+        c_end); outputs d_members_out / d_pos_out uint32[n_sig], d_seg_off uint32[n_votes+1], d_bits_out / d_agg_bits_out uint8[n_votes,
+        bits_stride] (n_votes and bits_stride from d_seg_off and d_bits_out), d_seg_off_loc the range's offsets over its own signatures."""
+        n_votes, stride = d_seg_off.numel() - 1, d_bits_out.shape[1]
+        assert d_bits_out.shape[0] >= n_votes and d_agg_bits_out.shape[1] == stride
+        self._ck(self.lib.b2_votes_group_dev(self.h, d_vote.data_ptr(), d_vote_off.data_ptr(), n_votes, d_members.data_ptr(), d_off.data_ptr(),
+                                             d_off.numel() - 1, d_members.numel(), stride, d_sigs.data_ptr(), int(c_begin), int(c_end),
+                                             d_sigs_out.data_ptr(), d_members_out.data_ptr(), d_pos_out.data_ptr(), d_seg_off.data_ptr(),
+                                             d_seg_off_loc.data_ptr() if d_seg_off_loc is not None else None, d_bits_out.data_ptr(),
+                                             d_agg_bits_out.data_ptr(), self._stream()))
+
+    def votes_empty_dev(self, d_bits, d_agg_sig, d_agg_status=None):
+        """b2_votes_empty_dev on the current stream: every vote whose grouped bit row d_bits (uint8[n_votes, bits_stride]) has no attester
+        gets 96 zero bytes in d_agg_sig and, when given, status 2 in d_agg_status"""
+        self._ck(self.lib.b2_votes_empty_dev(self.h, d_bits.data_ptr(), d_bits.shape[1], d_bits.shape[0], d_agg_sig.data_ptr(),
+                                             d_agg_status.data_ptr() if d_agg_status is not None else None, self._stream()))
+
     def epoch_set_pairing_form(self, team: bool):
         self._ck(self.lib.b2_epoch_set_pairing_form(self.h, 1 if team else 0))
 
