@@ -421,6 +421,56 @@ int b2_votes_group_dev(b2_ctx* ctx, const uint32_t* d_vote, const uint32_t* d_vo
                        uint8_t* d_bits_out, uint8_t* d_agg_bits_out, void* stream);
 int b2_votes_empty_dev(b2_ctx* ctx, const uint8_t* d_bits, uint32_t bits_stride, uint32_t n_votes, uint8_t* d_agg_sig96, int32_t* d_agg_status,
                        void* stream);
+/* ---- attestation intake: one epoch of unaggregated Attestations straight off the wire (pos-evolution.md:714-717; each with one member's
+ * AttestationData, one set bit and one signature) checked and turned into the vote form's inputs above.  Target epoch e, committee c of
+ * the epoch = (data.slot - start_slot(e)) * committees_per_slot + data.index with members d_off[c] .. d_off[c+1] (the layout of the
+ * epoch's b2_votes_group_dev call; n_committees = slots_per_epoch * committees_per_slot).  wire / woff are the encodings of
+ * b2_attestations_decode, wire_len the wire's length in bytes.  Every attestation gets exactly one status, the first failing check:
+ *    0  kept
+ *    1  malformed container; also a woff row that is reversed or ends past wire_len
+ *    2  empty Bitlist or no delimiter
+ *    3  more bits than 8 * bits_stride
+ *    4  not exactly one bit set
+ *    5  Bitlist length != the size of its committee (:730); a malformed committee row (device form) matches no length
+ *    6  data.slot outside epoch e, or data.index >= committees_per_slot (:725-727)
+ *    7  data.target.epoch != e
+ *    8  current_slot < data.slot + 1
+ *    9  beacon_block_root is not a block of the device tree
+ *   10  target.root is not a block of the device tree
+ *   11  slot(beacon_block_root) > data.slot
+ *   12  target.root != get_ancestor(beacon_block_root, start_slot(e)); a walk that reaches the tree's root while still above
+ *       start_slot(e) is not the ancestor
+ *   13  duplicate: an earlier attestation in list order that passed checks 1-12 holds the same (committee, position)
+ * Checks 9-12 are validate_on_attestation's (upstream fork-choice spec v1.2.0, :963-979) with store.blocks = the tree on the device:
+ * the blocks since the last b2_tree_prune, with the slots given to b2_tree_load / b2_tree_add.  Checks 5-8 are process_attestation's
+ * (:724-730); validate_target_epoch_against_current_time is made for the whole batch: an epoch e that is neither current_slot's epoch nor
+ * the one before it is B2_EINVAL.  Outputs, the arrays the vote form takes:
+ *   vote u32[n_sig]           vote[d_off[c] + p] = the vote id of the attestation kept at position p, or 0xFFFFFFFF.  A committee's kept
+ *                             attestations are grouped by their 128 data bytes (SSZ serialisation is injective); its vote ids are in the
+ *                             order of each group's smallest position.  A committee with nothing kept has one placeholder id.
+ *   vote_off u32[n_committees + 1]   written on the device;
+ *   sig96 u8[n_sig][96]       the kept signatures in committee order, zero where nothing is kept;
+ *   per vote v < max_votes    data128 u8[128], msg32 = compute_signing_root(data, domain32), source and target epoch (u64), block_idx =
+ *                             the tree id of beacon_block_root; a placeholder has zero data and message and block 0.
+ * An epoch with more than max_votes votes keeps its true counts in vote_off; only the first max_votes rows are written.  domain32 =
+ * get_domain(DOMAIN_BEACON_ATTESTER, e), a host pointer read when the call is made.
+ * b2_attestation_intake_dev is asynchronous on `stream` and self-guarding: a woff row that is reversed or ends past wire_len is status 1,
+ * a committee row that is reversed, ends past n_sig or exceeds 8 * bits_stride gets only its placeholder and its positions are not written
+ * (both B2_GUARD_BAD_ROW); nothing is read or written out of bounds.  The intakes of one context run one after another (they share its
+ * scratch), and the tree must not change while one is in flight.  b2_attestation_intake takes host arrays and returns when done; it
+ * checks woff (starts at 0, never decreases, ends inside the wire) and d_off (the same, no committee larger than 8 * bits_stride) first,
+ * and a rejected call (B2_EINVAL: these, a committee count that does not match, no loaded tree, a bad epoch, bits_stride == 0 or > 256,
+ * n_att or max_votes == 0) writes no output and changes nothing; rows past the epoch's vote count are zero. */
+int b2_attestation_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n_att, const uint32_t* d_off,
+                              uint32_t n_committees, uint64_t n_sig, uint32_t committees_per_slot, uint32_t slots_per_epoch, uint32_t bits_stride,
+                              uint64_t epoch, uint64_t current_slot, const uint8_t* domain32, uint32_t max_votes, int32_t* d_status_out,
+                              uint32_t* d_vote_out, uint32_t* d_vote_off_out, uint8_t* d_sig96_out, uint8_t* d_data128_out, uint8_t* d_msg32_out,
+                              uint64_t* d_source_epoch_out, uint64_t* d_target_epoch_out, uint32_t* d_block_idx_out, void* stream);
+int b2_attestation_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n_att, const uint32_t* off,
+                          uint32_t n_committees, uint32_t committees_per_slot, uint32_t slots_per_epoch, uint32_t bits_stride, uint64_t epoch,
+                          uint64_t current_slot, const uint8_t* domain32, uint32_t max_votes, int32_t* status_out, uint32_t* vote_out,
+                          uint32_t* vote_off_out, uint8_t* sig96_out, uint8_t* data128_out, uint8_t* msg32_out, uint64_t* source_epoch_out,
+                          uint64_t* target_epoch_out, uint32_t* block_idx_out);
 int b2_latest_messages_update_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_off, const uint8_t* d_bits,
                                   uint32_t bits_stride, const uint64_t* d_target_epoch, const uint32_t* d_block_idx,
                                   const uint8_t* d_accept, uint32_t n_agg, void* stream);

@@ -100,6 +100,12 @@ SIGNATURES = {
     "b2_votes_group_dev": (c_int, [c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_uint64, c_uint32, c_void_p, c_uint32,
                                    c_uint32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "b2_votes_empty_dev": (c_int, [c_void_p, c_void_p, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p]),
+    "b2_attestation_intake_dev": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_uint32, c_uint64, c_uint32, c_uint32,
+                                          c_uint32, c_uint64, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b2_attestation_intake": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_uint32, c_uint32, c_uint32, c_uint32, c_uint64,
+                                      c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                      c_void_p]),
     "b2_vote_weights_dev": (c_int, [c_void_p, c_void_p, c_void_p]),
     "b2_vote_weights_range_dev": (c_int, [c_void_p, c_uint64, c_uint64, c_void_p, c_void_p]),
     "b2_guard_flags": (c_int, [c_void_p, c_void_p]),

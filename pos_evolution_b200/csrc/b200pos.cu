@@ -21,6 +21,7 @@
 #include "ssz.cuh"
 #include "tree.cuh"
 #include "votes.cuh"
+#include "intake.cuh"
 
 using namespace b2;
 
@@ -79,7 +80,8 @@ struct tree_tables {
     dbuf prefix, w2;                                  // generic form: u64[n+1] prefix sums, u64 weights
     // per block id, so that b2_tree_add / _prune / _set_viable change the tree on the device (tree.cuh); `pre` above is per id too
     dbuf size, rank_id, parent, root, viable;         // u32 subtree size, u32 rank of (root, id), u32 parent, u8[32] root, u8 viability
-    dbuf pre_b, size_b, rank_b, parent_b, root_b, viable_b;      // the other side of the out-of-place steps (prune, grid insert)
+    dbuf slot;                                        // u64 block slot (read by the attestation intake)
+    dbuf pre_b, size_b, rank_b, parent_b, root_b, viable_b, slot_b;      // the other side of the out-of-place steps (prune, grid insert)
     dbuf scan, scan2, map;                            // u32[n+1] prefix-count scratch, u32[n] prune map
 };
 
@@ -114,6 +116,14 @@ struct ssz_tables {
     dbuf chunks;
 };
 
+// attestation intake (intake.cuh): per attestation, per committee, per bucket entry, per member slot, and the root-sorted block ids
+struct intake_scratch {
+    dbuf comm, pos, fp, grp;
+    dbuf bucket, cursor, nkept;
+    dbuf list, lead, gstat, gblk, gmin, vgrp;
+    dbuf posatt, sorted;
+};
+
 struct vslot {
     dbuf haff, hflag, pkjac, pkst, saff, sflag, f, sumjac;
     dbuf g2aff, g2st;                                      // the slot's own decompressed signatures (pipelined epochs)
@@ -143,6 +153,7 @@ struct b2_ctx {
     unsigned dec_turn = 0;
     cudaEvent_t ev_votes_done = nullptr, ev_lmd_done = nullptr;
     cudaEvent_t ev_equiv_done = nullptr;             // the last equivocation mark enqueued (b2_slasher_discount_dev, b2_equivocating_merge_dev)
+    cudaEvent_t ev_intake = nullptr;                 // the last attestation intake enqueued: the next one re-uses its scratch
     vslot slot[B2_EPOCH_SLOTS];
     char err[512] = {0};
     uint64_t launches = 0;
@@ -195,6 +206,7 @@ struct b2_ctx {
     slasher_tables sl;
     pack_scratch pk;
     ssz_tables ssz;
+    intake_scratch in;
 };
 
 struct nvtx_scope {
@@ -345,6 +357,7 @@ int b2_init(int device, b2_ctx** out) {
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_lmd_done, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_votes_done, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_equiv_done, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_intake, cudaEventDisableTiming);
     for (int i = 0; i < B2_EPOCH_SLOTS && e == cudaSuccess; i++) {
         cudaEvent_t* evs[6] = {&ctx->slot[i].ev_join0, &ctx->slot[i].ev_join1, &ctx->slot[i].ev_seg, &ctx->slot[i].ev_tail_done, &ctx->slot[i].ev_fork,
                                &ctx->slot[i].ev_in};
@@ -415,6 +428,7 @@ void b2_destroy(b2_ctx* ctx) {
     if (ctx->ev_lmd_done) cudaEventDestroy(ctx->ev_lmd_done);
     if (ctx->ev_votes_done) cudaEventDestroy(ctx->ev_votes_done);
     if (ctx->ev_equiv_done) cudaEventDestroy(ctx->ev_equiv_done);
+    if (ctx->ev_intake) cudaEventDestroy(ctx->ev_intake);
     if (ctx->h_head) cudaFreeHost((void*)ctx->h_head);
     delete ctx;      // frees every device buffer
 }
@@ -1264,6 +1278,112 @@ int b2_attestations_decode(b2_ctx* ctx, const uint8_t* wire, const uint32_t* wof
     return st.finish();
 }
 
+// ------------------------------------------------------------------------------------------ attestation intake (intake.cuh)
+// validate_target_epoch_against_current_time for the whole batch: the current slot's epoch or the one before it
+static bool intake_epoch_ok(uint64_t epoch, uint64_t current_slot, uint32_t slots_per_epoch) {
+    const uint64_t cur = current_slot / slots_per_epoch;
+    return epoch == cur || (cur > 0 && epoch == cur - 1);
+}
+
+int b2_attestation_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n_att, const uint32_t* d_off,
+                              uint32_t n_committees, uint64_t n_sig, uint32_t committees_per_slot, uint32_t slots_per_epoch, uint32_t bits_stride,
+                              uint64_t epoch, uint64_t current_slot, const uint8_t* domain32, uint32_t max_votes, int32_t* d_status_out,
+                              uint32_t* d_vote_out, uint32_t* d_vote_off_out, uint8_t* d_sig96_out, uint8_t* d_data128_out, uint8_t* d_msg32_out,
+                              uint64_t* d_source_epoch_out, uint64_t* d_target_epoch_out, uint32_t* d_block_idx_out, void* stream) {
+    B2_NVTX;
+    REQUIRE(ctx && d_wire && d_woff && d_off && domain32 && d_status_out && d_vote_out && d_vote_off_out && d_sig96_out && d_data128_out &&
+                d_msg32_out && d_source_epoch_out && d_target_epoch_out && d_block_idx_out && n_att > 0 && max_votes > 0 && n_sig < (1ull << 32) &&
+                bits_stride > 0 && bits_stride <= 256 && committees_per_slot > 0 && slots_per_epoch > 0,
+            "attestation_intake_dev: bad arguments");
+    REQUIRE((uint64_t)committees_per_slot * slots_per_epoch == n_committees, "attestation_intake: n_committees must be slots_per_epoch * committees_per_slot");
+    REQUIRE(current_slot < (1ull << 63) && intake_epoch_ok(epoch, current_slot, slots_per_epoch),
+            "attestation_intake: the epoch must be the current slot's epoch or the one before it");
+    REQUIRE(ctx->n_blocks > 0, "attestation_intake: no tree loaded (b2_tree_load)");
+    CK(cudaSetDevice(ctx->device));
+    intake_scratch& S = ctx->in;
+    const size_t na = (size_t)n_att * 4, nc = ((size_t)n_committees + 1) * 4;
+    int rc;
+    if ((rc = ensure(ctx, S.comm, na)) || (rc = ensure(ctx, S.pos, na)) || (rc = ensure(ctx, S.fp, na)) || (rc = ensure(ctx, S.grp, na)) ||
+        (rc = ensure(ctx, S.bucket, nc)) || (rc = ensure(ctx, S.cursor, nc)) || (rc = ensure(ctx, S.nkept, nc)) || (rc = ensure(ctx, S.list, na)) ||
+        (rc = ensure(ctx, S.lead, na)) || (rc = ensure(ctx, S.gstat, na)) || (rc = ensure(ctx, S.gblk, na)) || (rc = ensure(ctx, S.gmin, na)) ||
+        (rc = ensure(ctx, S.vgrp, na)) || (rc = ensure(ctx, S.posatt, n_sig * 4)) || (rc = ensure(ctx, S.sorted, (size_t)ctx->n_blocks * 4)))
+        return rc;
+    const tree_tables& t = ctx->tree;
+    intake_args A = {d_wire, wire_len, d_woff, n_att, d_off, n_committees, committees_per_slot, slots_per_epoch, bits_stride, n_sig, epoch, current_slot,
+                     t.root, t.parent, t.slot, S.sorted, ctx->n_blocks, S.comm, S.pos, S.fp, S.grp, S.bucket, S.cursor, S.nkept, S.list, S.lead,
+                     S.gstat, S.gblk, S.gmin, S.vgrp, S.posatt, d_status_out, d_vote_out, d_vote_off_out, d_sig96_out, max_votes, {},
+                     d_data128_out, d_msg32_out, d_source_epoch_out, d_target_epoch_out, d_block_idx_out, ctx->d_guard};
+    memcpy(A.domain.b, domain32, 32);
+    cudaStream_t s = (cudaStream_t)stream;
+    CK(cudaStreamWaitEvent(s, ctx->ev_intake, 0));
+    k_intake_sorted<<<blocks_for(ctx->n_blocks, 256), 256, 0, s>>>(t.rank_id, ctx->n_blocks, S.sorted);
+    CKL(ctx);
+    CK(cudaMemsetAsync(S.bucket, 0, nc, s));
+    k_intake_parse<<<blocks_for((uint64_t)n_att * 32, 128), 128, 0, s>>>(A);
+    CKL(ctx);
+    k_intake_scan<<<1, 1024, 0, s>>>(S.bucket, n_committees + 1, S.cursor);
+    CKL(ctx);
+    k_intake_scatter<<<blocks_for(n_att, 256), 256, 0, s>>>(A);
+    CKL(ctx);
+    k_intake_committee<<<n_committees, INTAKE_THREADS, 0, s>>>(A);
+    CKL(ctx);
+    k_intake_scan<<<1, 1024, 0, s>>>(d_vote_off_out, n_committees + 1, nullptr);
+    CKL(ctx);
+    k_intake_votes<<<blocks_for(max_votes, 64), 64, 0, s>>>(A);
+    CKL(ctx);
+    k_intake_sigs<<<n_committees, INTAKE_THREADS, 0, s>>>(A);
+    CKL(ctx);
+    CK(cudaEventRecord(ctx->ev_intake, s));
+    return B2_OK;
+}
+
+int b2_attestation_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n_att, const uint32_t* off,
+                          uint32_t n_committees, uint32_t committees_per_slot, uint32_t slots_per_epoch, uint32_t bits_stride, uint64_t epoch,
+                          uint64_t current_slot, const uint8_t* domain32, uint32_t max_votes, int32_t* status_out, uint32_t* vote_out,
+                          uint32_t* vote_off_out, uint8_t* sig96_out, uint8_t* data128_out, uint8_t* msg32_out, uint64_t* source_epoch_out,
+                          uint64_t* target_epoch_out, uint32_t* block_idx_out) {
+    B2_NVTX;
+    REQUIRE(ctx && wire && woff && off && domain32 && status_out && vote_out && vote_off_out && sig96_out && data128_out && msg32_out &&
+                source_epoch_out && target_epoch_out && block_idx_out && n_att > 0 && n_committees > 0 && max_votes > 0 && bits_stride > 0 &&
+                bits_stride <= 256 && committees_per_slot > 0 && slots_per_epoch > 0,
+            "attestation_intake: bad arguments");
+    REQUIRE((uint64_t)committees_per_slot * slots_per_epoch == n_committees, "attestation_intake: n_committees must be slots_per_epoch * committees_per_slot");
+    REQUIRE(current_slot < (1ull << 63) && intake_epoch_ok(epoch, current_slot, slots_per_epoch),
+            "attestation_intake: the epoch must be the current slot's epoch or the one before it");
+    REQUIRE(ctx->n_blocks > 0, "attestation_intake: no tree loaded (b2_tree_load)");
+    int rc;
+    if ((rc = check_offsets(ctx, woff, n_att, "attestation_intake: woff"))) return rc;
+    REQUIRE(woff[n_att] <= wire_len, "attestation_intake: woff ends past the wire");
+    if ((rc = check_offsets(ctx, off, n_committees, "attestation_intake: off"))) return rc;
+    for (uint32_t c = 0; c < n_committees; c++) REQUIRE(off[c + 1] - off[c] <= 8 * bits_stride, "attestation_intake: a committee is larger than 8 * bits_stride");
+    const uint64_t n_sig = off[n_committees];
+    CK(cudaSetDevice(ctx->device));
+    staging st(ctx);
+    const uint8_t* dwire = st.in(wire, wire_len, 16);
+    const uint32_t* dwoff = st.in(woff, (size_t)n_att + 1);
+    const uint32_t* doff = st.in(off, (size_t)n_committees + 1);
+    int32_t* dst = st.out(status_out, n_att);
+    uint32_t* dvote = st.out(vote_out, n_sig);
+    uint32_t* dvoff = st.out(vote_off_out, (size_t)n_committees + 1);
+    uint8_t* dsig = st.out(sig96_out, n_sig * 96);
+    uint8_t* ddata = st.out(data128_out, (size_t)max_votes * 128);
+    uint8_t* dmsg = st.out(msg32_out, (size_t)max_votes * 32);
+    uint64_t* dsrc = st.out(source_epoch_out, max_votes);
+    uint64_t* dtgt = st.out(target_epoch_out, max_votes);
+    uint32_t* dblk = st.out(block_idx_out, max_votes);
+    if (st.rc) return st.rc;
+    // rows past the epoch's vote count are zero
+    CK(cudaMemsetAsync(ddata, 0, (size_t)max_votes * 128, ctx->s_main));
+    CK(cudaMemsetAsync(dmsg, 0, (size_t)max_votes * 32, ctx->s_main));
+    CK(cudaMemsetAsync(dsrc, 0, (size_t)max_votes * 8, ctx->s_main));
+    CK(cudaMemsetAsync(dtgt, 0, (size_t)max_votes * 8, ctx->s_main));
+    CK(cudaMemsetAsync(dblk, 0, (size_t)max_votes * 4, ctx->s_main));
+    if ((rc = b2_attestation_intake_dev(ctx, dwire, wire_len, dwoff, n_att, doff, n_committees, n_sig, committees_per_slot, slots_per_epoch, bits_stride,
+                                        epoch, current_slot, domain32, max_votes, dst, dvote, dvoff, dsig, ddata, dmsg, dsrc, dtgt, dblk, ctx->s_main)))
+        return rc;
+    return st.finish();
+}
+
 // ------------------------------------------------------------------------------------------ committee shuffle
 int b2_shuffle_committees_dev(b2_ctx* ctx, const uint8_t* d_seed32, const uint32_t* d_active, uint32_t n_active, uint32_t rounds,
                               uint32_t* d_members_out, void* stream) {
@@ -1919,7 +2039,7 @@ int b2_tree_load(b2_ctx* ctx, const uint32_t* parent, const uint64_t* slot, cons
                   (rc = ensure(ctx, t.prefix, n8 + 8)) || (rc = ensure(ctx, t.w2, n8))))
         return rc;
     if ((rc = ensure(ctx, t.size, n4)) || (rc = ensure(ctx, t.rank_id, n4)) || (rc = ensure(ctx, t.parent, n4)) || (rc = ensure(ctx, t.root, 32ull * n)) ||
-        (rc = ensure(ctx, t.viable, n)))
+        (rc = ensure(ctx, t.viable, n)) || (rc = ensure(ctx, t.slot, n8)))
         return rc;
     cudaStream_t s = ctx->s_main;
     CK(cudaMemcpyAsync(t.size, size.data(), n4, cudaMemcpyHostToDevice, s));
@@ -1927,6 +2047,7 @@ int b2_tree_load(b2_ctx* ctx, const uint32_t* parent, const uint64_t* slot, cons
     CK(cudaMemcpyAsync(t.parent, parent, n4, cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(t.root, root32, 32ull * n, cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(t.viable, leaf_viable, n, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(t.slot, slot, n8, cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(t.pre, pre.data(), n4, cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync(t.inv, inv.data(), n4, cudaMemcpyHostToDevice, s));
     if (smem) {
@@ -1956,8 +2077,8 @@ static int tree_reserve(b2_ctx* ctx, uint32_t n_old, uint32_t n) {
         size_t keep, need;
     };
     const want all[] = {{&t.pre, k4, m4}, {&t.size, k4, m4}, {&t.rank_id, k4, m4}, {&t.parent, k4, m4}, {&t.root, 32 * (size_t)n_old, 32 * m},
-                        {&t.viable, n_old, m}, {&t.pre_b, 0, m4}, {&t.size_b, 0, m4}, {&t.rank_b, 0, m4}, {&t.parent_b, 0, m4},
-                        {&t.root_b, 0, 32 * m}, {&t.viable_b, 0, m}, {&t.scan, 0, m4 + 4}, {&t.scan2, 0, m4 + 4}, {&t.map, 0, m4},
+                        {&t.viable, n_old, m}, {&t.slot, 8 * (size_t)n_old, 8 * m}, {&t.pre_b, 0, m4}, {&t.size_b, 0, m4}, {&t.rank_b, 0, m4},
+                        {&t.parent_b, 0, m4}, {&t.root_b, 0, 32 * m}, {&t.viable_b, 0, m}, {&t.slot_b, 0, 8 * m}, {&t.scan, 0, m4 + 4}, {&t.scan2, 0, m4 + 4}, {&t.map, 0, m4},
                         {&t.inv, k4, n4}, {&t.votes, 8 * (size_t)std::min(n_old, n), n8}, {&t.weight, 0, n8},
                         {&t.packed, k4, smem ? n4 : 0}, {&t.size_keep, k4, smem ? 0 : n4}, {&t.rank, k4, smem ? 0 : n4},
                         {&t.next, 0, smem ? 0 : n4 + 4}, {&t.prefix, 0, smem ? 0 : n8 + 8}, {&t.w2, 0, smem ? 0 : n8}};
@@ -1977,7 +2098,8 @@ static int tree_reserve(b2_ctx* ctx, uint32_t n_old, uint32_t n) {
 }
 
 static tree_ids ids_of(tree_tables& t, bool other) {
-    return other ? tree_ids{t.pre_b, t.size_b, t.rank_b, t.parent_b, t.root_b, t.viable_b} : tree_ids{t.pre, t.size, t.rank_id, t.parent, t.root, t.viable};
+    return other ? tree_ids{t.pre_b, t.size_b, t.rank_b, t.parent_b, t.root_b, t.viable_b, t.slot_b}
+                 : tree_ids{t.pre, t.size, t.rank_id, t.parent, t.root, t.viable, t.slot};
 }
 
 // re-emits the tables of the form of an n-block tree, waits for the change, and makes n the tree's size
@@ -2010,6 +2132,7 @@ int b2_tree_add(b2_ctx* ctx, const uint32_t* parent, const uint64_t* slot, const
     CK(cudaMemcpyAsync((uint32_t*)t.parent + n0, parent, (size_t)k * 4, cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync((uint8_t*)t.root + 32ull * n0, root32, 32ull * k, cudaMemcpyHostToDevice, s));
     CK(cudaMemcpyAsync((uint8_t*)t.viable + n0, leaf_viable, k, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync((uint64_t*)t.slot + n0, slot, (size_t)k * 8, cudaMemcpyHostToDevice, s));
     CK(cudaMemsetAsync((uint64_t*)t.votes + n0, 0, (size_t)k * 8, s));      // the vote accumulator is clean between calls
     if (tree_form_of(n).smem_tree) {
         k_tree_insert_cta<<<1, 1024, 0, s>>>(t.pre, t.size, t.parent, n0, k);
@@ -2048,7 +2171,7 @@ int b2_tree_prune(b2_ctx* ctx, uint32_t new_root, uint32_t* map_out) {
         CKL(ctx);
     }
     std::swap(t.pre, t.pre_b), std::swap(t.size, t.size_b), std::swap(t.rank_id, t.rank_b);
-    std::swap(t.parent, t.parent_b), std::swap(t.root, t.root_b), std::swap(t.viable, t.viable_b);
+    std::swap(t.parent, t.parent_b), std::swap(t.root, t.root_b), std::swap(t.viable, t.viable_b), std::swap(t.slot, t.slot_b);
     CK(cudaMemcpyAsync(map_out, t.map, (size_t)n0 * 4, cudaMemcpyDeviceToHost, s));
     return tree_emit(ctx, n);
 }

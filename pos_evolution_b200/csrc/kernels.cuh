@@ -1157,6 +1157,21 @@ __global__ void __launch_bounds__(64) k_signing_roots(const uint8_t* __restrict_
 // status: 0 ok, 1 malformed container (too short / wrong offset), 2 empty bitlist or missing delimiter, 3 more than max_bits bits.
 namespace b2 {
 #define B2_ATT_FIXED 228u
+// The container and delimiter checks of the encoding w = wire + begin, wire[begin .. end): the status above; nbits = the Bitlist's length
+// in bits once the delimiter is found (statuses 0 and 3).  Shared by k_attestations_decode and the intake (intake.cuh).
+__device__ __forceinline__ int32_t att_wire_parse(const uint8_t* w, uint32_t begin, uint32_t end, uint32_t bits_stride, uint32_t max_bits,
+                                                  uint32_t& nbits) {
+    if (end < begin || end - begin < B2_ATT_FIXED) return 1;
+    const uint32_t o = (uint32_t)w[0] | ((uint32_t)w[1] << 8) | ((uint32_t)w[2] << 16) | ((uint32_t)w[3] << 24);
+    const uint32_t nbytes = end - begin - B2_ATT_FIXED;
+    if (o != B2_ATT_FIXED) return 1;
+    if (nbytes == 0 || w[end - begin - 1] == 0) return 2;
+    const uint32_t last = w[end - begin - 1];
+    const uint32_t top = 31u - (uint32_t)__clz((int)last);          // position of the delimiter bit in the last byte
+    nbits = 8 * (nbytes - 1) + top;
+    return nbits > max_bits || (nbits + 7) / 8 > bits_stride ? 3 : 0;
+}
+
 __global__ void __launch_bounds__(128) k_attestations_decode(const uint8_t* __restrict__ wire, const uint32_t* __restrict__ woff, uint32_t n,
                                                               uint32_t bits_stride, uint32_t max_bits, uint8_t* bits_out, uint32_t* bit_len_out,
                                                               uint8_t* data128_out, uint8_t* sig96_out, int32_t* status_out) {
@@ -1166,24 +1181,8 @@ __global__ void __launch_bounds__(128) k_attestations_decode(const uint8_t* __re
     const uint8_t* w = wire + begin;
     uint8_t* brow = bits_out + (uint64_t)a * bits_stride;
     for (uint32_t k = lane; k < bits_stride; k += 32) brow[k] = 0;
-    int32_t st = 0;
-    uint32_t nbits = 0, nbytes = 0;
-    if (end < begin || end - begin < B2_ATT_FIXED) {
-        st = 1;
-    } else {
-        const uint32_t o = (uint32_t)w[0] | ((uint32_t)w[1] << 8) | ((uint32_t)w[2] << 16) | ((uint32_t)w[3] << 24);
-        nbytes = end - begin - B2_ATT_FIXED;
-        if (o != B2_ATT_FIXED) {
-            st = 1;
-        } else if (nbytes == 0 || w[end - begin - 1] == 0) {
-            st = 2;
-        } else {
-            const uint32_t last = w[end - begin - 1];
-            const uint32_t top = 31u - (uint32_t)__clz((int)last);          // position of the delimiter bit in the last byte
-            nbits = 8 * (nbytes - 1) + top;
-            if (nbits > max_bits || (nbits + 7) / 8 > bits_stride) st = 3;
-        }
-    }
+    uint32_t nbits = 0;
+    const int32_t st = att_wire_parse(w, begin, end, bits_stride, max_bits, nbits);
     if (st == 0) {
         for (uint32_t k = lane; k < 128; k += 32) data128_out[128 * (uint64_t)a + k] = w[4 + k];
         for (uint32_t k = lane; k < 96; k += 32) sig96_out[96 * (uint64_t)a + k] = w[132 + k];

@@ -2,8 +2,8 @@
 // tree pruned to the finalized block (:1033-1036), leaf viability changed (get_filtered_block_tree, :1104), and the latest messages
 // re-mapped through a prune's id map.
 //
-// Per block id the device keeps the parent, the 32-byte root, the viability byte, the pre-order position, the subtree size and the rank
-// of (root, id) among all blocks -- the order b2_tree_load sorts by.  Siblings are in id order in the pre-order, and an appended block
+// Per block id the device keeps the parent, the 32-byte root, the slot, the viability byte, the pre-order position, the subtree size and
+// the rank of (root, id) among all blocks -- the order b2_tree_load sorts by.  The slot is read by the attestation intake (intake.cuh).  Siblings are in id order in the pre-order, and an appended block
 // has the largest id so far, so it becomes the LAST child of its parent: it takes position pos = pre[p] + size[p], every position
 // >= pos moves up by one, and the ancestors of p (p included) are exactly the blocks q with pre[q] <= pre[p] < pre[q] + size[q].
 // After every change k_tree_emit re-writes the tables of the tree's kernel form (kernels.cuh ghost_tree_args) from the per-id state.
@@ -133,6 +133,7 @@ __global__ void __launch_bounds__(1024) k_tree_emit(const uint32_t* pre, const u
 struct tree_ids {
     uint32_t *pre, *size, *rank, *parent;
     uint8_t *root, *viable;
+    uint64_t* slot;
 };
 
 // Prune to the subtree of block r, in one CTA: the kept blocks are those in r's interval of pre-order positions; their new ids are a
@@ -163,6 +164,7 @@ __global__ void __launch_bounds__(1024) k_tree_prune(tree_ids from, tree_ids to,
         to.rank[nb] = krank[from.rank[b]];
         to.parent[nb] = b == r ? 0u : kid[from.parent[b]];
         to.viable[nb] = from.viable[b];
+        to.slot[nb] = from.slot[b];
         const uint4* src = reinterpret_cast<const uint4*>(from.root + 32ull * b);
         uint4* dst = reinterpret_cast<uint4*>(to.root + 32ull * nb);
         dst[0] = src[0];

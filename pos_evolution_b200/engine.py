@@ -15,6 +15,9 @@ from ._lib import B2Error
 # Engine.pack_attestations: per pick (in pick order) committee, data id, union bit row, u64 numerator; constituents src[src_off[o] ..
 # src_off[o+1]) in pool order; signature (bls.Aggregate of the constituents); cand_status per candidate (0 folded, 1 undecodable)
 PackResult = namedtuple("PackResult", "committee data bits numerator src_off src signature cand_status")
+# Engine.attestation_intake: status per attestation; the vote form's inputs: vote per member slot, vote_off per committee, signatures in
+# committee order, and per vote (max_votes rows) the AttestationData, signing root, source and target epoch and block id
+IntakeResult = namedtuple("IntakeResult", "status vote vote_off sigs data128 msgs source_epoch target_epoch block_idx")
 
 
 def _c(a, dtype):
@@ -276,6 +279,24 @@ class Engine:
         st = np.zeros(n, dtype=np.int32)
         self._ck(self.lib.b2_attestations_decode(self.h, _p(w), _p(woff), n, int(bits_stride), int(max_bits), _p(bits), _p(blen), _p(data), _p(sig), _p(st)))
         return bits, blen, data, sig, st
+
+    def attestation_intake(self, wire: bytes, woff, off, epoch: int, current_slot: int, domain32: bytes, committees_per_slot: int,
+                           slots_per_epoch: int, bits_stride: int, max_votes: int) -> IntakeResult:
+        """One epoch of unaggregated Attestations (the wire form of attestations_decode) checked against the device tree and turned into
+        the vote form's inputs (include/b200pos.h, b2_attestation_intake: statuses 0-13); committee c = members off[c] .. off[c+1]."""
+        woff, off = _c(woff, np.uint32), _c(off, np.uint32)
+        n_att, n_c = woff.shape[0] - 1, off.shape[0] - 1
+        w = np.frombuffer(bytes(wire), dtype=np.uint8) if len(wire) else np.zeros(1, dtype=np.uint8)
+        dom = np.frombuffer(bytes(domain32), dtype=np.uint8)
+        assert dom.shape == (32,)
+        n_sig, mv = int(off[-1]), int(max_votes)
+        r = IntakeResult(np.zeros(n_att, np.int32), np.zeros(n_sig, np.uint32), np.zeros(n_c + 1, np.uint32), np.zeros((n_sig, 96), np.uint8),
+                         np.zeros((mv, 128), np.uint8), np.zeros((mv, 32), np.uint8), np.zeros(mv, np.uint64), np.zeros(mv, np.uint64),
+                         np.zeros(mv, np.uint32))
+        self._ck(self.lib.b2_attestation_intake(self.h, _p(w), len(wire), _p(woff), n_att, _p(off), n_c, int(committees_per_slot),
+                                                int(slots_per_epoch), int(bits_stride), int(epoch), int(current_slot), _p(dom), mv,
+                                                *[_p(x) for x in r]))
+        return r
 
     def signing_roots(self, data128, domains32):
         """compute_signing_root for n attestations: data128 uint8[n,128] (SSZ-serialised AttestationData), domains32 uint8[32] or uint8[n,32]."""
@@ -623,6 +644,20 @@ class Engine:
                                              d_sigs_out.data_ptr(), d_members_out.data_ptr(), d_pos_out.data_ptr(), d_seg_off.data_ptr(),
                                              d_seg_off_loc.data_ptr() if d_seg_off_loc is not None else None, d_bits_out.data_ptr(),
                                              d_agg_bits_out.data_ptr(), self._stream()))
+
+    def attestation_intake_dev(self, d_wire, d_woff, d_off, epoch: int, current_slot: int, domain32: bytes, committees_per_slot: int,
+                               slots_per_epoch: int, bits_stride: int, d_status, d_vote, d_vote_off, d_sigs, d_data128, d_msgs, d_source_epoch,
+                               d_target_epoch, d_block_idx):
+        """attestation_intake on device tensors (the wire's length is d_wire.numel(); max_votes = d_msgs.shape[0]), asynchronous on the
+        current stream."""
+        dom = np.frombuffer(bytes(domain32), dtype=np.uint8)
+        assert dom.shape == (32,)
+        self._ck(self.lib.b2_attestation_intake_dev(self.h, d_wire.data_ptr(), d_wire.numel(), d_woff.data_ptr(), d_woff.numel() - 1,
+                                                    d_off.data_ptr(), d_off.numel() - 1, d_vote.numel(), int(committees_per_slot),
+                                                    int(slots_per_epoch), int(bits_stride), int(epoch), int(current_slot), _p(dom),
+                                                    d_msgs.shape[0], d_status.data_ptr(), d_vote.data_ptr(), d_vote_off.data_ptr(),
+                                                    d_sigs.data_ptr(), d_data128.data_ptr(), d_msgs.data_ptr(), d_source_epoch.data_ptr(),
+                                                    d_target_epoch.data_ptr(), d_block_idx.data_ptr(), self._stream()))
 
     def votes_empty_dev(self, d_bits, d_agg_sig, d_agg_status=None):
         """b2_votes_empty_dev on the current stream: every vote whose grouped bit row d_bits (uint8[n_votes, bits_stride]) has no attester

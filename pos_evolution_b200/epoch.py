@@ -42,6 +42,10 @@ on the stream that claimed the slot) and the epoch kernels run unchanged with on
 aggregate_signatures() / aggregation_bits() then hold one row per vote, i.e. one Attestation each.  Sharded, rank g aggregates the votes
 of its committees [vote_off[c0_g], vote_off[c1_g]); the all-gather pads every rank's block to the largest count.
 
+Attestation intake (`intake_dev`): an epoch of unaggregated Attestations straight off the wire is checked against the device tree
+(process_attestation, validate_on_attestation), one kept per committee position, and turned into the vote form's inputs on the device
+(Engine.attestation_intake_dev); the returned tensors go to submit_dev / process_epoch_dev with votes=(r.vote, r.vote_off).
+
 Equivocation discounting (`enable_slasher(..., discount=True)`, pos-evolution.md:1405-1461): right after each epoch's slasher update,
 every validator it flagged joins the device's Store.equivocating_indices, so from the next epoch on its votes neither move its latest
 message nor count in a head (:1411: votes of validators "not viewed to have equivocated at previous slots").  The marks only grow.
@@ -63,6 +67,13 @@ MAX_DEPTH = 16      # == B2_EPOCH_SLOTS (include/b200pos.h)
 # off_loc over its own signatures `sigs`; sharded, `pad` rows per rank in the all-gather of out_loc into out_all and, in the vote form,
 # `ranges` = (first row, count) of every rank.
 _Layout = collections.namedtuple("_Layout", "votes n members off r0 r1 members_loc off_loc sigs pad ranges out_loc out_all")
+
+Intake = collections.namedtuple("Intake", "sigs vote msgs target_epoch block_idx source_epoch data128 status vote_off")
+Intake.__doc__ = """One epoch's attestations after EpochProcessor.intake_dev: fresh device tensors sigs uint8[n_sig, 96] (committee order), vote
+int32[n_sig], and per vote (min(n_votes, max_votes) rows) msgs uint8[., 32], target_epoch / source_epoch int64, block_idx int32, data128
+uint8[., 128];
+status int32[n_att] per attestation (include/b200pos.h, b2_attestation_intake); vote_off int64[n_committees + 1] on the host.  Submit
+with submit_dev(r.sigs, None, r.msgs, r.target_epoch, r.block_idx, votes=(r.vote, r.vote_off), source_epoch=r.source_epoch)."""
 
 Slashings = collections.namedtuple("Slashings", "status aggregate position validator kind surrounded_target surrounding_target")
 Slashings.__doc__ = """What the slasher found in one epoch (numpy arrays).  status: int32[n_agg], B2_SLASHER_* per aggregate.  One entry per
@@ -585,6 +596,36 @@ class EpochProcessor:
                     self._discount(s, L, host)
                 if pipelined:
                     s.ev_sl = self._record()
+
+    # ------------------------------------------------------------------ attestation intake
+    def intake_dev(self, d_wire, d_woff, epoch, current_slot, domain32, committees_per_slot, slots_per_epoch) -> Intake:
+        """One epoch of unaggregated Attestations straight off the wire (d_wire uint8, d_woff int32/uint32[n_att + 1] on the device, the
+        form of Engine.attestations_decode) checked against the device tree and turned into the vote form's inputs for this processor's
+        committees (Engine.attestation_intake_dev, on the current stream).  Returns an Intake of fresh tensors, which follow the input
+        contract of submit_dev once submitted.  Reading vote_off waits for the current stream's work up to the intake: enqueue it under a
+        stream that carries no epoch (torch.cuda.stream(...)) and it waits for the intake alone.  An epoch with more than max_votes votes
+        is then refused by submit_dev.  Not for a sharded processor."""
+        if self.sharded:
+            raise ValueError("intake_dev: a sharded EpochProcessor is not supported")
+        if self.max_votes is None:
+            raise ValueError("intake_dev needs an EpochProcessor constructed with max_votes")
+        if int(committees_per_slot) * int(slots_per_epoch) != self.n_agg:
+            raise ValueError("committees_per_slot * slots_per_epoch must be the processor's n_agg = %d" % self.n_agg)
+        self._check_tree()
+        z, mv = self._zeros, self.max_votes
+        r = Intake(z((self.n_sig, 96), torch.uint8), torch.full((self.n_sig,), -1, dtype=torch.int32, device=self.dev), z((mv, 32), torch.uint8),
+                   z(mv, torch.int64), z(mv, torch.int32), z(mv, torch.int64), z((mv, 128), torch.uint8), z(d_woff.numel() - 1, torch.int32), None)
+        d_vote_off = z(self.n_agg + 1, torch.int32)
+        self.eng.attestation_intake_dev(d_wire, d_woff, self.d_off, epoch, current_slot, domain32, committees_per_slot, slots_per_epoch,
+                                        self.bits_stride, r.status, r.vote, d_vote_off, r.sigs, r.data128, r.msgs, r.source_epoch,
+                                        r.target_epoch, r.block_idx)
+        h = self._pinned(self.n_agg + 1, torch.int32)
+        h.copy_(d_vote_off, non_blocking=True)
+        self._record().synchronize()
+        vote_off = h.numpy().astype(np.int64)
+        n = min(int(vote_off[-1]), mv)                  # the per-vote rows the entry points take: one per vote
+        return r._replace(msgs=r.msgs[:n], target_epoch=r.target_epoch[:n], block_idx=r.block_idx[:n], source_epoch=r.source_epoch[:n],
+                          data128=r.data128[:n], vote_off=vote_off)
 
     # ------------------------------------------------------------------ synchronous form
     def _prepare(self, s, host, sigs, bits, msgs, tgt, blk, src, V):
