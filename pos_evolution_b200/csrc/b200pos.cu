@@ -1321,13 +1321,13 @@ int b2_attestation_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_
     CK(cudaMemsetAsync(S.bucket, 0, nc, s));
     k_intake_parse<<<blocks_for((uint64_t)n_att * 32, 128), 128, 0, s>>>(A);
     CKL(ctx);
-    k_intake_scan<<<1, 1024, 0, s>>>(S.bucket, n_committees + 1, S.cursor);
+    k_intake_scan<<<1, 1024, 0, s>>>(S.bucket, n_committees, S.cursor);      // bucket[n_committees] = the candidates
     CKL(ctx);
     k_intake_scatter<<<blocks_for(n_att, 256), 256, 0, s>>>(A);
     CKL(ctx);
     k_intake_committee<<<n_committees, INTAKE_THREADS, 0, s>>>(A);
     CKL(ctx);
-    k_intake_scan<<<1, 1024, 0, s>>>(d_vote_off_out, n_committees + 1, nullptr);
+    k_intake_scan<<<1, 1024, 0, s>>>(d_vote_off_out, n_committees, nullptr);      // vote_off[n_committees] = the epoch's votes
     CKL(ctx);
     k_intake_votes<<<blocks_for(max_votes, 64), 64, 0, s>>>(A);
     CKL(ctx);

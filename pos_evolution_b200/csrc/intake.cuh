@@ -5,12 +5,12 @@
 //
 //   k_intake_parse      warp per attestation: container and delimiter (att_wire_parse), the single set bit, checks 1-8, committee and
 //                       position; candidates are counted per committee
-//   k_intake_scan       one CTA: bucket starts of the committees (exclusive scan of the counts)
+//   k_intake_scan       one CTA: bucket starts of the committees (exclusive scan of the counts, the total in bucket[n_committees])
 //   k_intake_scatter    thread per candidate: its index into its committee's bucket
 //   k_intake_committee  CTA per committee: the distinct data of its candidates (exact 128-byte comparison, a fingerprint first), the
 //                       tree checks 9-12 once per distinct data, the position claims (smallest list index wins), vote numbering by the
 //                       smallest position of each kept group
-//   k_intake_scan       again: the vote counts into vote_off
+//   k_intake_scan       again: the vote counts into vote_off, the epoch's vote count in vote_off[n_committees]
 //   k_intake_votes      thread per vote: data, signing root, epochs, block id
 //   k_intake_sigs       CTA per committee: global vote ids and the kept signatures in committee order
 #pragma once
@@ -173,7 +173,8 @@ __global__ void __launch_bounds__(128) k_intake_parse(intake_args A) {
     }
 }
 
-// x[0 .. n) -> its exclusive scan, in one CTA of 1024 threads; cursor (may be null) receives a copy
+// x[0 .. n) -> its exclusive scan and x[n] = the total (x holds n + 1 entries), in one CTA of 1024 threads; cursor (may be null)
+// receives a copy of x[0 .. n)
 __global__ void __launch_bounds__(1024) k_intake_scan(uint32_t* x, uint32_t n, uint32_t* cursor) {
     __shared__ uint32_t warp_tot[32];
     block_exclusive_scan(x, n, warp_tot);
@@ -203,7 +204,8 @@ __device__ __forceinline__ uint32_t intake_block_min(uint32_t v, uint32_t* s_red
 // gblk / gmin, and its kept votes l the same range of vgrp (D <= m, kept votes <= D).
 __global__ void __launch_bounds__(INTAKE_THREADS) k_intake_committee(intake_args A) {
     __shared__ uint32_t win[VOTES_MAX_MEMBERS];          // per position: the smallest list index claiming it
-    __shared__ uint32_t first[VOTES_MAX_MEMBERS + 1];    // per position: 1 if it is its group's smallest kept position; then scanned
+    __shared__ uint32_t first[VOTES_MAX_MEMBERS + 1];    // per position: 1 if it is its group's smallest kept position; then scanned,
+                                                         // the total in first[size]
     __shared__ uint8_t ldata[128];
     __shared__ uint32_t s_red[INTAKE_THREADS / 32], warp_tot[32];
     const uint32_t c = blockIdx.x, tid = threadIdx.x;
@@ -261,9 +263,8 @@ __global__ void __launch_bounds__(INTAKE_THREADS) k_intake_committee(intake_args
     __syncthreads();
     // votes: the kept groups in the order of their smallest position
     for (uint32_t p = tid; p < size; p += INTAKE_THREADS) first[p] = win[p] != VOTE_NONE && A.gmin[b0 + A.grp[win[p]]] == p ? 1u : 0u;
-    if (tid == 0) first[size] = 0;
     __syncthreads();
-    block_exclusive_scan(first, size + 1, warp_tot);
+    block_exclusive_scan(first, size, warp_tot);      // first[size] = the kept votes (size <= VOTES_MAX_MEMBERS)
     __syncthreads();
     for (uint32_t p = tid; p < size; p += INTAKE_THREADS) {
         const uint32_t a = win[p];
@@ -279,7 +280,6 @@ __global__ void __launch_bounds__(INTAKE_THREADS) k_intake_committee(intake_args
     if (tid == 0) {
         A.nkept[c] = first[size];
         A.vote_off[c] = max(first[size], 1u);      // a committee without a kept attestation has one placeholder vote
-        if (c == A.n_committees - 1) A.vote_off[A.n_committees] = 0;
     }
 }
 

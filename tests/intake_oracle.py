@@ -4,6 +4,7 @@ against a block store, one kept per committee position, grouped by AttestationDa
 
 intake_plain restates the contract attestation by attestation over oracle.spec containers, a block dict and oracle.spec's get_ancestor
 and hash_tree_root_attestation_data; intake_numpy computes the same for fixed-length records with array operations, for epochs of 2^20."""
+import hashlib
 import types
 
 import numpy as np
@@ -355,5 +356,67 @@ def random_epoch(rng, epoch, spe, cps, csize, tree, n_extra=0, corrupt=0.3, head
         w = bytearray(wires[int(rng.integers(0, len(wires)))])
         if rng.random() < 0.5:
             w[4 + 56] ^= 1                                                      # another source root: other data, same position
+        wires.append(bytes(w))
+    return wires
+
+
+def ragged_layout(sizes):
+    """the committee layout off (uint32[len(sizes) + 1]) of committees of the given sizes"""
+    return np.concatenate([[0], np.cumsum(sizes)]).astype(np.uint32)
+
+
+def ragged_epoch(rng, epoch, spe, cps, sizes, tree, distinct=2, absent=0.0, dup=0.0, corrupt=0.0):
+    """The wires of one epoch whose committee c has sizes[c] members (len(sizes) == spe * cps).  Committee c's attesters sign
+    distinct[c] (or `distinct`) different AttestationData, each used by at least one attester while min(that, attesters) allows; the
+    data differ in their head or source root, so all of them pass the tree checks.  A share `absent` of the members does not attest.
+    A share `corrupt` of the attestations fails one check: two bits (4), a Bitlist one bit longer (5), a foreign target epoch (7), an
+    unknown head (9) or a known block that is not the target's ancestor as target (12).  The wires come in random order; then, for a
+    share `dup` of the attestations, a second one for the same position is appended: with equal data, with other data, or after the
+    earlier copy was made to fail (unknown target, 10), so that the appended one is the position's first passing attestation."""
+    parent, slot, roots = tree
+    start, n_c = epoch * spe, spe * cps
+    assert len(sizes) == n_c
+    distinct = [distinct] * n_c if np.isscalar(distinct) else list(distinct)
+    src_root = bytes(roots[0])
+    wires, meta = [], []
+    for c in range(n_c):
+        size, s = int(sizes[c]), start + c // cps
+        ok = [b for b in range(len(parent)) if int(slot[b]) <= s and ancestor(parent, slot, b, start) is not None] or [0]
+        present = np.nonzero(rng.random(size) >= absent)[0]
+        k = max(1, min(int(distinct[c]), len(present)))
+        group = rng.permutation(np.arange(len(present)) % k)
+        data = []
+        for g in range(k):
+            h = ok[int(rng.integers(0, len(ok)))]
+            t = ancestor(parent, slot, h, start)
+            src = hashlib.sha256(b"ragged-source/%d/%d" % (c, g)).digest() if g else src_root
+            data.append(data128(s, c % cps, bytes(roots[h]), epoch - 1 if epoch else 0, src, epoch, bytes(roots[0 if t is None else t])))
+        for p, g in zip(present.tolist(), group.tolist()):
+            meta.append((size, p, data[g]))
+    sig = lambda: rng.integers(0, 256, size=96, dtype=np.uint8).tobytes()      # noqa: E731
+    for size, p, d in meta:
+        d, bits = bytearray(d), [j == p for j in range(size)]
+        kind = int(rng.integers(0, 5)) if rng.random() < corrupt else -1
+        if kind == 0 and size > 1:
+            bits[(p + 1) % size] = True
+        elif kind == 1:
+            bits.append(False)
+        elif kind == 2:
+            d[88:96] = (epoch + 1).to_bytes(8, "little")
+        elif kind == 3:
+            d[16:48] = bytes([0xAB] * 32)
+        elif kind == 4:
+            d[96:128] = bytes(roots[int(np.argmax(slot))])
+        wires.append(encode(bits, bytes(d), sig()))
+    wires = [wires[i] for i in rng.permutation(len(wires))]
+    for i in np.nonzero(rng.random(len(wires)) < dup)[0].tolist():
+        w, kind = bytearray(wires[i]), int(rng.integers(0, 3))
+        if kind == 1:
+            w[4 + 56] ^= 1                                                      # other data, same position
+        elif kind == 2:
+            bad = bytearray(wires[i])
+            bad[4 + 96:4 + 128] = bytes([0xCD] * 32)                            # the earlier copy fails (10)
+            wires[i] = bytes(bad)
+        w[132:228] = sig()
         wires.append(bytes(w))
     return wires

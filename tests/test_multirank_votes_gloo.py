@@ -2,8 +2,8 @@
 committees' signatures, verifies the votes of its committees [vote_off[c0_g], vote_off[c1_g]) -- a different count per rank --, the
 all-gather pads every rank's block to the largest count and unpacks it by vote, and every rank applies update_latest_messages over ALL
 votes.  The result must equal the unsharded vote form and a sequential oracle.  The GPU kernels are replaced by a numpy stand-in behind
-the same EpochProcessor plumbing (engine interface duck-typed, as test_multirank_gloo.py); its grouping is an independent model of
-b2_votes_group_dev's layout."""
+the same EpochProcessor plumbing (engine interface duck-typed, as test_multirank_gloo.py); its grouping is tests/votes_oracle.py, an
+independent model of b2_votes_group_dev's layout."""
 import os
 import socket
 
@@ -13,6 +13,7 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 import scenarios
+import votes_oracle as VO
 from oracle import fast
 
 N_VAL, N_BLK, CS = 64, 50, 16
@@ -41,21 +42,6 @@ def _inputs():
     return members, off, vote, vote_off, sigs, verdict, epochs, blocks
 
 
-def _group(members, off, vote, vote_off):
-    """numpy model of the grouping: per committee, stable by vote, non-attesters last in the last vote's segment"""
-    n_votes = int(vote_off[-1])
-    order, seg = np.zeros(N_VAL, dtype=np.int64), np.zeros(n_votes + 1, dtype=np.int64)
-    for c in range(N_C):
-        o0, v0, v1 = int(off[c]), int(vote_off[c]), int(vote_off[c + 1])
-        local = vote[o0:off[c + 1]].astype(np.int64)
-        key = np.where((local >= v0) & (local < v1), local - v0, v1 - v0)
-        p = np.argsort(key, kind="stable")
-        order[o0:off[c + 1]] = o0 + p
-        seg[v0:v1] = o0 + np.searchsorted(key[p], np.arange(v1 - v0))
-    seg[n_votes] = off[N_C]
-    return order, seg
-
-
 class _VoteEngine:
     """Stand-in for engine.Engine: grouping in numpy, verdicts from a table keyed by the vote id carried in each message, the
     'aggregate signature' = (vote id, sum of its attesters' signer bytes), the LMD table and the vote scatter by the numpy oracle."""
@@ -73,32 +59,17 @@ class _VoteEngine:
                         d_bits_out, d_agg_bits_out, d_seg_off_loc=None):
         vote, vote_off = d_vote.numpy().view(np.uint32), d_vote_off.numpy().astype(np.int64)
         members, off = d_members.numpy().view(np.uint32), d_off.numpy().astype(np.int64)
-        order, seg = _group(members, off, vote, vote_off)
         n_votes = int(vote_off[-1])
         assert d_seg_off.numel() == n_votes + 1 and d_bits_out.shape[0] == n_votes
-        d_members_out.copy_(torch.from_numpy(members[order].view(np.int32)))
-        d_pos_out.copy_(torch.from_numpy((order - off[np.searchsorted(off, order, side="right") - 1]).astype(np.int32)))
-        d_seg_off.copy_(torch.from_numpy(seg.astype(np.int32)))
-        bits, agg = np.zeros((n_votes, d_bits_out.shape[1]), dtype=np.uint8), np.zeros((n_votes, d_bits_out.shape[1]), dtype=np.uint8)
-        for c in range(N_C):
-            for v in range(int(vote_off[c]), int(vote_off[c + 1])):
-                pos = np.nonzero(vote[off[c]:off[c + 1]] == v)[0]
-                for i in range(len(pos)):
-                    bits[v, i >> 3] |= 1 << (i & 7)
-                for j in pos:
-                    agg[v, j >> 3] |= 1 << (j & 7)
-        d_bits_out.copy_(torch.from_numpy(bits))
-        d_agg_bits_out.copy_(torch.from_numpy(agg))
-        b0, b1 = int(off[c_begin]), int(off[c_end])
-        src = d_sigs.numpy()
-        out = np.zeros((b1 - b0, 96), dtype=np.uint8)
-        for p in range(b0, b1):
-            j = int(order[p])
-            out[p - b0] = src[j - b0] if vote[j] != NONE else np.frombuffer(bytes([0xC0]) + bytes(95), dtype=np.uint8)
-        d_sigs_out.copy_(torch.from_numpy(out))
+        g = VO.group_outputs(members, off, vote, vote_off, d_sigs.numpy(), d_bits_out.shape[1], c_begin, c_end)
+        d_members_out.copy_(torch.from_numpy(g.members_out.view(np.int32)))
+        d_pos_out.copy_(torch.from_numpy(g.pos_out.astype(np.int32)))
+        d_seg_off.copy_(torch.from_numpy(g.seg_off.astype(np.int32)))
+        d_bits_out.copy_(torch.from_numpy(g.bits))
+        d_agg_bits_out.copy_(torch.from_numpy(g.agg_bits))
+        d_sigs_out.copy_(torch.from_numpy(g.sigs_out))
         if d_seg_off_loc is not None:
-            v0, v1 = int(vote_off[c_begin]), int(vote_off[c_end])
-            d_seg_off_loc[:v1 - v0 + 1] = torch.from_numpy((seg[v0:v1 + 1] - b0).astype(np.int32))
+            d_seg_off_loc[:g.seg_off_loc.shape[0]] = torch.from_numpy(g.seg_off_loc.astype(np.int32))
         self.calls.append(("group", c_begin, c_end))
 
     def epoch_dev(self, d_sigs, d_members, d_off, d_bits, d_msgs, d_target_epoch, d_block_idx, d_agg_sig, d_agg_status, d_ok):

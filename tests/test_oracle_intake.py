@@ -94,3 +94,31 @@ def test_numpy_form_equals_plain_form(seed):
     assert set(a.status.tolist()) >= {0, 1, 2, 4, 5, 6, 7, 9, 10, 13}
     for f in ("status", "vote", "vote_off", "sigs", "data128", "msgs", "source_epoch", "target_epoch", "block_idx"):
         assert np.array_equal(getattr(a, f), getattr(b, f)), f
+
+
+def test_ragged_epoch_has_the_requested_groups_and_late_duplicates():
+    """ragged_epoch: the requested number of distinct data per committee, whatever its size; with dup = 1 every attestation has a later
+    copy, and where the earlier one was made to fail (status 10) the later one is the position's kept attestation"""
+    rng = np.random.default_rng(8)
+    sizes, distinct = [1, 2, 9, 64, 64], [1, 2, 3, 64, 5]
+    tree = IO.random_tree(rng, 30, 3 * 5 - 7)
+    wires = IO.ragged_epoch(rng, 3, 5, 1, sizes, tree, distinct=distinct, dup=1.0)
+    r = IO.intake_plain(wires, IO.ragged_layout(sizes), 3, 4 * 5, DOMAIN, 1, 5, 8, *IO.block_store(*tree))
+    n = sum(sizes)
+    assert len(wires) == 2 * n and (r.status[:n] != 13).all() and (r.vote != IO.NONE).all()
+    assert np.diff(r.vote_off).tolist() == distinct
+    late = r.status[n:].tolist()
+    assert 10 in r.status[:n].tolist() and 0 in late and 13 in late and set(late) <= {0, 13}
+
+
+def test_ragged_numpy_form_equals_plain_form():
+    """committees of one size through ragged_epoch, with 2 048 members and every member's own data in one of them"""
+    rng = np.random.default_rng(9)
+    tree = IO.random_tree(rng, 30, 0)
+    wires = IO.ragged_epoch(rng, 3, 2, 1, [2048, 2048], tree, distinct=[2048, 3], absent=0.1, dup=0.05, corrupt=0.1)
+    off = IO.ragged_layout([2048, 2048]).astype(np.int64)
+    a = IO.intake_plain(wires, off, 3, 8, DOMAIN, 1, 2, 256, *IO.block_store(*tree))
+    b = IO.intake_numpy(np.frombuffer(b"".join(wires), dtype=np.uint8).reshape(len(wires), -1), off, 3, 8, DOMAIN, 1, 2, 256, *tree)
+    assert int(a.vote_off[1]) > 1500
+    for f in ("status", "vote", "vote_off", "sigs", "data128", "msgs", "source_epoch", "target_epoch", "block_idx"):
+        assert np.array_equal(getattr(a, f), getattr(b, f)), f

@@ -13,7 +13,7 @@ cd "$(dirname "$0")/.."
 OUT="${OUT:-$(mktemp -d)}"
 mkdir -p "$OUT"
 SAN=/usr/local/cuda/bin/compute-sanitizer
-SMALL="tests/test_gpu_bls.py tests/test_gpu_bls_adversarial.py tests/test_gpu_aggregate_verify.py tests/test_gpu_sync_aggregate.py tests/test_gpu_forkchoice.py tests/test_gpu_gather.py tests/test_gpu_participation.py tests/test_gpu_epoch.py tests/test_gpu_slasher.py tests/test_gpu_epoch_slasher.py tests/test_gpu_epoch_votes.py tests/test_gpu_intake.py::test_every_status_and_output_matches_oracle tests/test_gpu_intake.py::test_device_guards tests/test_gpu_intake.py::test_rejected_host_calls_change_nothing tests/test_gpu_epoch_discount.py tests/test_gpu_pack.py tests/test_gpu_ssz.py::test_validators_load tests/test_gpu_ssz.py::test_incremental_updates tests/test_gpu_tree_update.py::test_random_sequences_match_a_fresh_load tests/test_gpu_tree_update.py::test_root_ties tests/test_gpu_tree_update.py::test_rejected_calls_change_nothing"
+SMALL="tests/test_gpu_bls.py tests/test_gpu_bls_adversarial.py tests/test_gpu_aggregate_verify.py tests/test_gpu_sync_aggregate.py tests/test_gpu_forkchoice.py tests/test_gpu_gather.py tests/test_gpu_participation.py tests/test_gpu_epoch.py tests/test_gpu_slasher.py tests/test_gpu_epoch_slasher.py tests/test_gpu_epoch_votes.py tests/test_gpu_intake.py::test_every_status_and_output_matches_oracle tests/test_gpu_intake.py::test_device_guards tests/test_gpu_intake.py::test_rejected_host_calls_change_nothing tests/test_gpu_intake_shapes.py::test_single_committee_epoch tests/test_gpu_intake_shapes.py::test_more_than_1024_committees tests/test_gpu_intake_shapes.py::test_votes_group_matches_numpy_model tests/test_gpu_epoch_discount.py tests/test_gpu_pack.py tests/test_gpu_ssz.py::test_validators_load tests/test_gpu_ssz.py::test_incremental_updates tests/test_gpu_tree_update.py::test_random_sequences_match_a_fresh_load tests/test_gpu_tree_update.py::test_root_ties tests/test_gpu_tree_update.py::test_rejected_calls_change_nothing"
 RACE="tests/test_gpu_bls.py::test_fast_aggregate_verify_vs_oracle tests/test_gpu_bls.py::test_g1_aggregate_all_minimal_committees tests/test_gpu_forkchoice.py tests/test_gpu_gather.py tests/test_gpu_pack.py::test_pack_matches_oracle tests/test_gpu_ssz.py::test_validators_load"
 run() {  # name, timeout, command...
     local name=$1 tmo=$2; shift 2
