@@ -105,8 +105,8 @@ def _run(eng, epochs, members, off, n_blk, mode, depth, H, discount, n_agg=T.N_A
     return results, (equiv, e_, b_, h_)
 
 
-def _six_epochs(mode, depth, discount, pre_marked=(), n_epochs=T.N_EPOCHS):
-    members, off, tree, eff = T._world()
+def _six_epochs(mode, depth, discount, pre_marked=(), n_epochs=T.N_EPOCHS, n_val=T.N_VAL):
+    members, off, tree, eff = T._world(n_val)
     eng = T._engine(tree, eff)
     epochs = T._inputs(eng, members, off)[:n_epochs]
     if pre_marked:

@@ -29,12 +29,15 @@ def _h(tag):
     return hashlib.sha256(tag).digest()
 
 
-def _world():
+def _world(n_val=N_VAL):
+    """n_val >= N_VAL: the registry's size; validators N_VAL.. are in no committee (32 ETH each), so they change no vote, verdict or
+    finding, only the registry's validator ranges"""
     rng = np.random.default_rng(21)
     members = rng.permutation(N_VAL).astype(np.uint32)
     off = (np.arange(N_AGG + 1) * CSIZE).astype(np.uint32)
     parent, slot, roots, leaf_viable = scenarios.fork_tree(N_BLK, 5)
     eff = (rng.integers(16, 33, size=N_VAL).astype(np.uint64)) * np.uint64(10**9)
+    eff = np.concatenate([eff, np.full(n_val - N_VAL, 32 * 10**9, dtype=np.uint64)])
     return members, off, (parent, slot, roots, leaf_viable), eff
 
 
@@ -103,11 +106,11 @@ def _inputs(eng, members, off):
     return out
 
 
-def _engine(tree, eff):
+def _engine(tree, eff, device=0):
     from pos_evolution_b200.engine import Engine
     parent, slot, roots, leaf_viable = tree
-    eng = Engine(0)
-    pk = eng.sk_to_pk([scenarios.secret_key(v) for v in range(N_VAL)])
+    eng = Engine(device)
+    pk = eng.sk_to_pk([scenarios.secret_key(v) for v in range(len(eff))])
     eng.registry_load(pk, eff)
     eng.tree_load(parent, slot, roots, leaf_viable)
     eng.latest_messages_reset()
@@ -124,10 +127,11 @@ def _full(sl, total):
     return sl.status, kind, conflict, len(slots)
 
 
-def _run(mode, depth, H, slasher):
-    """the six epochs through EpochProcessor in `mode`; -> per epoch (verdicts, head, aggregate signatures, Slashings or None)"""
+def _run(mode, depth, H, slasher, n_val=N_VAL):
+    """the six epochs through EpochProcessor in `mode`, on a registry of n_val; -> per epoch (verdicts, head, aggregate signatures,
+    Slashings or None)"""
     from pos_evolution_b200.epoch import EpochProcessor
-    members, off, tree, eff = _world()
+    members, off, tree, eff = _world(n_val)
     eng = _engine(tree, eff)
     epochs = _inputs(eng, members, off)
     dev = torch.device("cuda", 0)

@@ -21,17 +21,24 @@ PLACEHOLDER, FOREIGN = 4, 1            # the committee where nobody attests; the
 ZERO96 = bytes(96)
 
 
-@pytest.fixture(scope="module")
-def world():
-    from pos_evolution_b200.engine import Engine
-    eng = Engine(0)
-    pks = scenarios.pubkeys(N_VAL)
+def _world(n_val=N_VAL):
+    """(pubkeys, members, off, tree, effective balances) on a registry of n_val >= N_VAL validators; validators N_VAL.. are in no
+    committee (32 ETH each), so they change no vote, verdict or head, only the registry's validator ranges"""
+    pks = scenarios.pubkeys(n_val)
     rng = np.random.default_rng(5)
     members = rng.permutation(N_VAL).astype(np.uint32)
     off = (np.arange(N_C + 1) * CSIZE).astype(np.uint32)
     tree = scenarios.fork_tree(N_BLK, 5)
     eff = rng.integers(16, 33, size=N_VAL).astype(np.uint64) * np.uint64(10**9)
-    yield eng, pks, members, off, tree, eff
+    eff = np.concatenate([eff, np.full(n_val - N_VAL, 32 * 10**9, dtype=np.uint64)])
+    return pks, members, off, tree, eff
+
+
+@pytest.fixture(scope="module")
+def world():
+    from pos_evolution_b200.engine import Engine
+    eng = Engine(0)
+    yield (eng,) + _world()
     eng.close()
 
 
@@ -47,7 +54,7 @@ def _epoch(eng, k, members, off):
     nv[PLACEHOLDER], nv[FOREIGN] = 1, 2
     vote_off = np.concatenate([[0], np.cumsum(nv)]).astype(np.int64)
     n_votes = int(vote_off[-1])
-    vote = np.full(N_VAL, NONE, dtype=np.int64)
+    vote = np.full(len(members), NONE, dtype=np.int64)
     for c in range(N_C):
         if c == PLACEHOLDER:
             continue

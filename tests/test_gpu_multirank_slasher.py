@@ -1,13 +1,18 @@
-"""The slasher in the sharded epoch pipeline on real GPUs (needs >= 2; run with `python -m pytest tests/test_gpu_multirank_slasher.py -m gpu`
-on a machine with two or more H100s).  Every rank runs the sharded EpochProcessor over NCCL with enable_slasher (pipelined, depth 3)
-on the six epochs of test_gpu_epoch_slasher.py, so it holds the history of its validator range only; the union of the ranks' flagged
-member slots must equal a single-process unsharded run on the same epochs, the ranks' slots must be disjoint and every rank must
-report the same per-aggregate statuses."""
-import os
-import socket
+"""The slasher in the sharded epoch pipeline, every rank a process with its own context.  Every rank runs the sharded EpochProcessor
+with enable_slasher on the six epochs of test_gpu_epoch_slasher.py, so it holds the history of its validator range only; the union of
+the ranks' flagged member slots must equal a single-process unsharded run of the same epochs in the same form, the ranks' slots must
+lie in their ranges and every rank must report the same per-aggregate statuses.
 
+Two layouts (tests/rank_group.py):
+  * per_device: world 2, one GPU per rank over NCCL (skipped below 2 GPUs), pipelined (submit_dev, depth 3);
+  * shared_device: the ranks share one GPU over host-staged gloo: pipelined at world 2 and 4, and the synchronous process_epoch_dev and
+    process_epoch_host (sharded) at world 2.
+The shared layout runs every device call of the sharded path -- the tail without the LMD update, the exchange's LMD update on the
+fork-choice stream, the range scatter and the range slasher fed the gathered verdicts -- but not NCCL, NVLink or any multi-GPU timing."""
 import numpy as np
 import pytest
+
+import rank_group
 
 pytestmark = pytest.mark.gpu
 
@@ -20,20 +25,13 @@ def _report(sl):
     return sl.status.tolist(), sorted(rows)
 
 
-def _worker(rank, world, port, q):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world), LOCAL_RANK=str(rank))
+def _worker(rank, world, port, q, shared, mode):
     import torch.distributed as dist
     import test_gpu_epoch_slasher as T
-    from pos_evolution_b200.engine import Engine
     from pos_evolution_b200.epoch import EpochProcessor
-    torch.cuda.set_device(rank)
-    dev = torch.device("cuda", rank)
-    dist.init_process_group("nccl", device_id=dev)
-    members, off, (parent, slot, roots, leaf_viable), eff = T._world()
-    eng = Engine(rank)
-    eng.registry_load(eng.sk_to_pk([T.scenarios.secret_key(v) for v in range(T.N_VAL)]), eff)
-    eng.tree_load(parent, slot, roots, leaf_viable)
-    eng.latest_messages_reset()
+    dev = rank_group.init(rank, world, port, shared)
+    members, off, tree, eff = T._world()
+    eng = T._engine(tree, eff, dev.index)
     epochs = T._inputs(eng, members, off)
     ep = EpochProcessor(eng, T.N_AGG, T.N_AGG * T.CSIZE, 1, T.N_BLK, process_group=dist.group.WORLD, device=dev, depth=3,
                         shard=(rank, world), n_validators=T.N_VAL)
@@ -44,9 +42,18 @@ def _worker(rank, world, port, q):
         d = [torch.as_tensor(ep.local_signatures(e["sigs"]), device=dev)] + [torch.as_tensor(e[x], device=dev) for x in ("bits", "msgs", "tgt", "blk")]
         src = torch.as_tensor(e["src"], device=dev)
         keep.append((d, src))
-        t = ep.submit_dev(*d, last=(k == len(epochs) - 1), source_epoch=src, current_epoch=T.CUR0 + k)
-        if t is not None:
-            out.append(_report(t.slashings()))
+        if mode == "sync":
+            ep.process_epoch_dev(*d, source_epoch=src, current_epoch=T.CUR0 + k)
+            out.append(_report(ep.slashings()))
+        elif mode == "sync_host":
+            h, hs = [x.cpu().pin_memory() for x in d], src.cpu().pin_memory()
+            keep.append((h, hs))
+            ep.process_epoch_host(*h, source_epoch=hs, current_epoch=T.CUR0 + k)
+            out.append(_report(ep.slashings()))
+        else:
+            t = ep.submit_dev(*d, last=(k == len(epochs) - 1), source_epoch=src, current_epoch=T.CUR0 + k)
+            if t is not None:
+                out.append(_report(t.slashings()))
     out += [_report(t.slashings()) for t in ep.drain()]
     q.put((rank, ep.sl_range, out, eng.guard_flags()))
     dist.barrier()
@@ -54,26 +61,15 @@ def _worker(rank, world, port, q):
     eng.close()
 
 
-@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs >= 2 GPUs")
-def test_sharded_slasher_on_two_gpus_equals_unsharded():
-    import torch.multiprocessing as mp
+@pytest.mark.parametrize("layout,world,mode", [("per_device", 2, "pipelined"), ("shared_device", 2, "pipelined"), ("shared_device", 4, "pipelined"),
+                                               ("shared_device", 2, "sync"), ("shared_device", 2, "sync_host")])
+def test_sharded_slasher_equals_unsharded(layout, world, mode):
     import test_gpu_epoch_slasher as T
-    world = 2
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    port = s.getsockname()[1]
-    s.close()
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    results = sorted((q.get(timeout=900) for _ in range(world)), key=lambda r: r[0])
-    for p in procs:
-        p.join(timeout=120)
-        assert p.exitcode == 0
-    whole = [_report(r[3]) for r in T._run("pipelined", 3, 16, True)]
-    assert [r[1] for r in results] == [(0, T.N_VAL // 2), (T.N_VAL // 2, T.N_VAL)]
+    if layout == "per_device" and torch.cuda.device_count() < world:
+        pytest.skip("needs >= %d GPUs" % world)
+    results = rank_group.run(_worker, world, args=(layout == "shared_device", mode))
+    whole = [_report(r[3]) for r in T._run(mode, 3, 16, True)]
+    assert [r[1] for r in results] == [(g * T.N_VAL // world, (g + 1) * T.N_VAL // world) for g in range(world)]
     for k in range(T.N_EPOCHS):
         union = []
         for rank, (v0, v1), out, guard in results:
