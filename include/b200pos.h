@@ -471,6 +471,72 @@ int b2_attestation_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, c
                           uint64_t current_slot, const uint8_t* domain32, uint32_t max_votes, int32_t* status_out, uint32_t* vote_out,
                           uint32_t* vote_off_out, uint8_t* sig96_out, uint8_t* data128_out, uint8_t* msg32_out, uint64_t* source_epoch_out,
                           uint64_t* target_epoch_out, uint32_t* block_idx_out);
+/* ---- aggregated-attestation intake: one target epoch e of SignedAggregateAndProof messages from gossip (the beacon_aggregate_and_proof
+ * topic of the upstream phase 0 p2p spec), checked and verified on the device.  Containers (upstream phase 0):
+ *   AggregateAndProof{aggregator_index u64, aggregate Attestation, selection_proof BLSSignature}
+ *   SignedAggregateAndProof{message AggregateAndProof, signature BLSSignature}
+ * wire / woff = the SSZ encodings back to back and their byte offsets (as b2_attestations_decode takes them), wire_len the wire's bytes.
+ * Committee c of the epoch = (data.slot - start_slot(e)) * committees_per_slot + data.index, members d_members[d_off[c] .. d_off[c+1])
+ * (the layout of b2_attestation_intake; precondition: the committees are pairwise disjoint, as get_beacon_committee makes them).
+ * domains96 (host pointer) = get_domain(., D, e) for D = DOMAIN_BEACON_ATTESTER, DOMAIN_SELECTION_PROOF, DOMAIN_AGGREGATE_AND_PROOF, back to
+ * back.  target_aggregators = TARGET_AGGREGATORS_PER_COMMITTEE, propagation_slot_range = ATTESTATION_PROPAGATION_SLOT_RANGE.
+ * Every item gets exactly one status, the first failing check in this order (the class is what gossip scoring reads):
+ *    0  accept
+ *    1  reject  malformed outer, inner or nested container (offsets, lengths, trailing bytes); also a woff row that is reversed or ends
+ *               past wire_len
+ *    2  reject  empty Bitlist or no delimiter
+ *    3  reject  more bits than 8 * bits_stride
+ *    4  reject  data.index >= committees_per_slot
+ *    5  ignore  not data.slot <= current_slot <= data.slot + propagation_slot_range
+ *    6  reject  data.target.epoch != compute_epoch_at_slot(data.slot)
+ *    7  (other) compute_epoch_at_slot(data.slot) != e: the item belongs to the other epoch's call
+ *    8  reject  Bitlist length != committee size; a malformed committee row (device form) matches no length
+ *    9  reject  no bit set
+ *   10  ignore  an earlier ACCEPTED item of the call has byte-equal AttestationData and bits that cover this item's
+ *   11  ignore  an earlier ACCEPTED item of the call has the same aggregator_index
+ *   12  reject  is_aggregator is false: bytes_to_uint64(hash(selection_proof)[0:8]) % max(1, len(committee) // target_aggregators) != 0
+ *   13  reject  aggregator_index is not in the committee
+ *   14  reject  the selection proof fails Verify(pubkey(aggregator), compute_signing_root(data.slot, selection domain))
+ *   15  reject  the signature fails Verify(pubkey(aggregator), compute_signing_root(AggregateAndProof, aggregate_and_proof domain))
+ *   16  reject  the aggregate fails FastAggregateVerify over the selected members and the attestation signing root
+ *   17  ignore  beacon_block_root is not a block of the device tree
+ *   18  reject  target.root is not a block of the device tree
+ *   19  reject  slot(beacon_block_root) > data.slot
+ *   20  reject  target.root != get_ancestor(beacon_block_root, start_slot(e))
+ * 17-20 are b2_attestation_intake's 9-12 (the same tree walk).  Checks 10 and 11 read only earlier items of the same call that end with
+ * status 0: each item gets the status it would get if the items arrived one by one in list order at a node whose seen-caches were empty
+ * when the call began (the caller keeps the caches across calls).  e must be current_slot's epoch or the one before it.
+ * Outputs per item (n items; zero rows, 0xFFFFFFFF ids for an item that did not decode, statuses 1-3):
+ *   committee u32        c, or 0xFFFFFFFF for statuses 1-7
+ *   data_id u32          the smallest list index with byte-equal AttestationData
+ *   bits u8[bits_stride] the aggregation bits, delimiter removed, zero padded
+ *   sig96, msg32         the aggregate signature as on the wire; compute_signing_root(data, attester domain)
+ *   target_epoch u64, block_idx u32   data.target.epoch; the tree id of beacon_block_root (0xFFFFFFFF when absent)
+ *   members u32[n][8 * bits_stride], item_off u32[n+1]   item a's member row = its committee, zero padded, and item_off[a] = 8 * bits_stride * a:
+ *                        with bits and accept = (status == 0) these are what b2_latest_messages_update_dev (on_attestation of the accepted
+ *                        aggregates) and b2_fast_aggregate_verify_dev take, and the rows the FastAggregateVerify of check 16 consumed.
+ * b2_aggregate_and_proof_intake_dev is asynchronous on `stream` and self-guarding: a woff row that is reversed or ends past wire_len is
+ * status 1 and a committee row that is reversed, ends past n_sig (the members' length) or exceeds 8 * bits_stride is status 8 (both
+ * B2_GUARD_BAD_ROW); an aggregator index that is not a member never reaches the registry (status 13), and a member index >= n_validators
+ * fails the checks that read it (B2_GUARD_BAD_INDEX); nothing is read or written out of bounds.  It shares scratch with the intake (the
+ * two run one after another) and with the synchronous verify entry points: the verify buffers of pipeline slot 0 (b2_fast_aggregate_verify,
+ * _pks, _dev, b2_epoch_dev) and the AggregateVerify buffers (b2_aggregate_verify, _pks, _dev); enqueue those on the same stream.  The
+ * tree and the registry must not change while a call is in flight.  b2_aggregate_and_proof_intake takes host arrays and returns when
+ * done; it checks woff (starts at 0, never decreases, ends inside the wire) and off (the same, no committee larger than 8 * bits_stride)
+ * first, and a rejected call (B2_EINVAL: these, a committee count other than slots_per_epoch * committees_per_slot, no registry or tree,
+ * a bad epoch, bits_stride == 0 or > 256, target_aggregators == 0, n == 0) writes no output and changes nothing. */
+int b2_aggregate_and_proof_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n, const uint32_t* d_members,
+                                      const uint32_t* d_off, uint32_t n_committees, uint64_t n_sig, uint32_t committees_per_slot, uint32_t slots_per_epoch,
+                                      uint32_t bits_stride, uint64_t epoch, uint64_t current_slot, const uint8_t* domains96, uint32_t target_aggregators,
+                                      uint64_t propagation_slot_range, int32_t* d_status_out, uint32_t* d_committee_out, uint32_t* d_data_id_out,
+                                      uint8_t* d_bits_out, uint8_t* d_sig96_out, uint8_t* d_msg32_out, uint64_t* d_target_epoch_out,
+                                      uint32_t* d_block_idx_out, uint32_t* d_members_out, uint32_t* d_item_off_out, void* stream);
+int b2_aggregate_and_proof_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n, const uint32_t* members,
+                                  const uint32_t* off, uint32_t n_committees, uint32_t committees_per_slot, uint32_t slots_per_epoch, uint32_t bits_stride,
+                                  uint64_t epoch, uint64_t current_slot, const uint8_t* domains96, uint32_t target_aggregators,
+                                  uint64_t propagation_slot_range, int32_t* status_out, uint32_t* committee_out, uint32_t* data_id_out, uint8_t* bits_out,
+                                  uint8_t* sig96_out, uint8_t* msg32_out, uint64_t* target_epoch_out, uint32_t* block_idx_out, uint32_t* members_out,
+                                  uint32_t* item_off_out);
 int b2_latest_messages_update_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_off, const uint8_t* d_bits,
                                   uint32_t bits_stride, const uint64_t* d_target_epoch, const uint32_t* d_block_idx,
                                   const uint8_t* d_accept, uint32_t n_agg, void* stream);

@@ -106,6 +106,12 @@ SIGNATURES = {
     "b2_attestation_intake": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_uint32, c_uint32, c_uint32, c_uint32, c_uint64,
                                       c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                       c_void_p]),
+    # ctx, wire, wire_len, woff, n, members, off, n_committees, [n_sig,] committees_per_slot, slots_per_epoch, bits_stride, epoch, current_slot,
+    # domains96, target_aggregators, propagation_slot_range, ten outputs[, stream]
+    "b2_aggregate_and_proof_intake_dev": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_uint64, c_uint32,
+                                                  c_uint32, c_uint32, c_uint64, c_uint64, c_void_p, c_uint32, c_uint64] + [c_void_p] * 11),
+    "b2_aggregate_and_proof_intake": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_uint32, c_uint32,
+                                              c_uint32, c_uint64, c_uint64, c_void_p, c_uint32, c_uint64] + [c_void_p] * 10),
     "b2_vote_weights_dev": (c_int, [c_void_p, c_void_p, c_void_p]),
     "b2_vote_weights_range_dev": (c_int, [c_void_p, c_uint64, c_uint64, c_void_p, c_void_p]),
     "b2_guard_flags": (c_int, [c_void_p, c_void_p]),

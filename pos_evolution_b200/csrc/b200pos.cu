@@ -22,6 +22,7 @@
 #include "tree.cuh"
 #include "votes.cuh"
 #include "intake.cuh"
+#include "aggintake.cuh"
 
 using namespace b2;
 
@@ -124,6 +125,13 @@ struct intake_scratch {
     dbuf posatt, sorted;
 };
 
+// aggregated-attestation intake (aggintake.cuh): per item, per hash-table slot, per committee, per validator, per single-key set
+struct api_scratch {
+    dbuf comm, fp, slot_of, dtab, dmin, list, acc, accepted_by, incomm, tst, fbits, fav_ok;
+    dbuf bucket, cursor, sorted;
+    dbuf av_signer, av_off, av_msg, av_sig, av_ok;
+};
+
 struct vslot {
     dbuf haff, hflag, pkjac, pkst, saff, sflag, f, sumjac;
     dbuf g2aff, g2st;                                      // the slot's own decompressed signatures (pipelined epochs)
@@ -207,6 +215,7 @@ struct b2_ctx {
     pack_scratch pk;
     ssz_tables ssz;
     intake_scratch in;
+    api_scratch api;
 };
 
 struct nvtx_scope {
@@ -1380,6 +1389,186 @@ int b2_attestation_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, c
     CK(cudaMemsetAsync(dblk, 0, (size_t)max_votes * 4, ctx->s_main));
     if ((rc = b2_attestation_intake_dev(ctx, dwire, wire_len, dwoff, n_att, doff, n_committees, n_sig, committees_per_slot, slots_per_epoch, bits_stride,
                                         epoch, current_slot, domain32, max_votes, dst, dvote, dvoff, dsig, ddata, dmsg, dsrc, dtgt, dblk, ctx->s_main)))
+        return rc;
+    return st.finish();
+}
+
+// ------------------------------------------------------------------------------------------ aggregated-attestation intake (aggintake.cuh)
+int b2_aggregate_and_proof_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n, const uint32_t* d_members,
+                                      const uint32_t* d_off, uint32_t n_committees, uint64_t n_sig, uint32_t committees_per_slot, uint32_t slots_per_epoch,
+                                      uint32_t bits_stride, uint64_t epoch, uint64_t current_slot, const uint8_t* domains96, uint32_t target_aggregators,
+                                      uint64_t propagation_slot_range, int32_t* d_status_out, uint32_t* d_committee_out, uint32_t* d_data_id_out,
+                                      uint8_t* d_bits_out, uint8_t* d_sig96_out, uint8_t* d_msg32_out, uint64_t* d_target_epoch_out,
+                                      uint32_t* d_block_idx_out, uint32_t* d_members_out, uint32_t* d_item_off_out, void* stream) {
+    B2_NVTX;
+    REQUIRE(ctx && d_wire && d_woff && d_members && d_off && domains96 && d_status_out && d_committee_out && d_data_id_out && d_bits_out && d_sig96_out &&
+                d_msg32_out && d_target_epoch_out && d_block_idx_out && d_members_out && d_item_off_out && n > 0 && n < (1u << 28) &&
+                n_sig < (1ull << 32) && bits_stride > 0 && bits_stride <= 256 && (uint64_t)n * 8 * bits_stride < (1ull << 32) &&
+                committees_per_slot > 0 && slots_per_epoch > 0 && target_aggregators > 0,
+            "aggregate_and_proof_intake_dev: bad arguments");
+    REQUIRE((uint64_t)committees_per_slot * slots_per_epoch == n_committees,
+            "aggregate_and_proof_intake: n_committees must be slots_per_epoch * committees_per_slot");
+    REQUIRE(current_slot < (1ull << 63) && intake_epoch_ok(epoch, current_slot, slots_per_epoch),
+            "aggregate_and_proof_intake: the epoch must be the current slot's epoch or the one before it");
+    REQUIRE(ctx->n_blocks > 0, "aggregate_and_proof_intake: no tree loaded (b2_tree_load)");
+    REQUIRE(ctx->n_val > 0, "aggregate_and_proof_intake: registry not loaded");
+    CK(cudaSetDevice(ctx->device));
+    api_scratch& S = ctx->api;
+    uint32_t tab = 1;
+    while (tab < 2 * n) tab <<= 1;
+    const size_t na = (size_t)n * 4, nc = ((size_t)n_committees + 1) * 4;
+    int rc;
+    if ((rc = ensure(ctx, S.comm, na)) || (rc = ensure(ctx, S.fp, na)) || (rc = ensure(ctx, S.slot_of, na)) || (rc = ensure(ctx, S.dtab, (size_t)tab * 4)) ||
+        (rc = ensure(ctx, S.dmin, (size_t)tab * 4)) || (rc = ensure(ctx, S.list, na)) || (rc = ensure(ctx, S.acc, na)) ||
+        (rc = ensure(ctx, S.accepted_by, ctx->n_val * 4)) || (rc = ensure(ctx, S.incomm, n)) || (rc = ensure(ctx, S.tst, n)) ||
+        (rc = ensure(ctx, S.fbits, (size_t)n * bits_stride + 16)) || (rc = ensure(ctx, S.fav_ok, n)) || (rc = ensure(ctx, S.bucket, nc)) ||
+        (rc = ensure(ctx, S.cursor, nc)) || (rc = ensure(ctx, S.sorted, (size_t)ctx->n_blocks * 4)) || (rc = ensure(ctx, S.av_signer, 2 * na)) ||
+        (rc = ensure(ctx, S.av_off, 2 * na + 4)) || (rc = ensure(ctx, S.av_msg, (size_t)n * 64)) || (rc = ensure(ctx, S.av_sig, (size_t)n * 192)) ||
+        (rc = ensure(ctx, S.av_ok, 2 * (size_t)n)))
+        return rc;
+    const tree_tables& t = ctx->tree;
+    intake_args T = {};
+    T.n_att = n;
+    T.off = d_off;
+    T.n_committees = n_committees;
+    T.committees_per_slot = committees_per_slot;
+    T.slots_per_epoch = slots_per_epoch;
+    T.bits_stride = bits_stride;
+    T.n_sig = n_sig;
+    T.epoch = epoch;
+    T.current_slot = current_slot;
+    T.root = t.root;
+    T.parent = t.parent;
+    T.slot = t.slot;
+    T.sorted = S.sorted;
+    T.n_blocks = ctx->n_blocks;
+    T.comm = S.comm;
+    T.bucket = S.bucket;
+    T.cursor = S.cursor;
+    T.list = S.list;
+    T.guard = ctx->d_guard;
+    api_args A = {};
+    A.wire = d_wire;
+    A.wire_len = wire_len;
+    A.woff = d_woff;
+    A.n = n;
+    A.members = d_members;
+    A.committees_per_slot = committees_per_slot;
+    A.slots_per_epoch = slots_per_epoch;
+    A.bits_stride = bits_stride;
+    A.target_aggregators = target_aggregators;
+    A.epoch = epoch;
+    A.current_slot = current_slot;
+    A.propagation_range = propagation_slot_range;
+    A.n_val = ctx->n_val;
+    A.T = T;
+    A.fp = S.fp;
+    A.slot_of = S.slot_of;
+    A.dtab = S.dtab;
+    A.dmin = S.dmin;
+    A.acc = S.acc;
+    A.accepted_by = S.accepted_by;
+    A.dtab_mask = tab - 1;
+    A.incomm = S.incomm;
+    A.tst = S.tst;
+    A.fbits = S.fbits;
+    A.av_signer = S.av_signer;
+    A.av_off = S.av_off;
+    A.av_msg = S.av_msg;
+    A.av_sig = S.av_sig;
+    A.fav_ok = S.fav_ok;
+    A.av_ok = S.av_ok;
+    A.status = d_status_out;
+    A.committee = d_committee_out;
+    A.data_id = d_data_id_out;
+    A.bits = d_bits_out;
+    A.sig96 = d_sig96_out;
+    A.msg32 = d_msg32_out;
+    A.target_epoch = d_target_epoch_out;
+    A.block_idx = d_block_idx_out;
+    A.members_out = d_members_out;
+    A.item_off = d_item_off_out;
+    memcpy(A.dom_att.b, domains96, 32);
+    memcpy(A.dom_sel.b, domains96 + 32, 32);
+    memcpy(A.dom_aap.b, domains96 + 64, 32);
+    A.guard = ctx->d_guard;
+    cudaStream_t s = (cudaStream_t)stream;
+    CK(cudaStreamWaitEvent(s, ctx->ev_intake, 0));
+    k_intake_sorted<<<blocks_for(ctx->n_blocks, 256), 256, 0, s>>>(t.rank_id, ctx->n_blocks, S.sorted);
+    CKL(ctx);
+    CK(cudaMemsetAsync(S.bucket, 0, nc, s));
+    CK(cudaMemsetAsync(S.dtab, 0xff, (size_t)tab * 4, s));
+    CK(cudaMemsetAsync(S.dmin, 0xff, (size_t)tab * 4, s));
+    CK(cudaMemsetAsync(S.accepted_by, 0xff, ctx->n_val * 4, s));
+    k_api_parse<<<blocks_for((uint64_t)n * 32, 128), 128, 0, s>>>(A);
+    CKL(ctx);
+    k_api_data<<<blocks_for(n, 128), 128, 0, s>>>(A);
+    CKL(ctx);
+    k_api_roots<<<blocks_for(n, 64), 64, 0, s>>>(A);
+    CKL(ctx);
+    k_api_sets<<<blocks_for(n, 64), 64, 0, s>>>(A);
+    CKL(ctx);
+    // FastAggregateVerify of the aggregates over their member rows, then AggregateVerify of the 2n single-key sets
+    pk_source P = {d_members_out, d_item_off_out, (const uint8_t*)S.fbits, bits_stride, nullptr, 0};
+    if ((rc = verify_fork(ctx, ctx->slot[0], P, d_msg32_out, n, s)) || (rc = verify_main(ctx, ctx->slot[0], d_sig96_out, n, S.fav_ok, s))) return rc;
+    if ((rc = aggregate_verify_enqueue(ctx, S.av_signer, nullptr, S.av_msg, S.av_off, 2ull * n, S.av_sig, 2 * n, S.av_ok, s))) return rc;
+    k_intake_scan<<<1, 1024, 0, s>>>(S.bucket, n_committees, S.cursor);      // bucket[n_committees] = the candidates
+    CKL(ctx);
+    k_intake_scatter<<<blocks_for(n, 256), 256, 0, s>>>(T);
+    CKL(ctx);
+    k_api_committee<<<n_committees, 32, 0, s>>>(A);
+    CKL(ctx);
+    k_api_outsiders<<<blocks_for(n, 128), 128, 0, s>>>(A);
+    CKL(ctx);
+    CK(cudaEventRecord(ctx->ev_intake, s));
+    return B2_OK;
+}
+
+int b2_aggregate_and_proof_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n, const uint32_t* members,
+                                  const uint32_t* off, uint32_t n_committees, uint32_t committees_per_slot, uint32_t slots_per_epoch, uint32_t bits_stride,
+                                  uint64_t epoch, uint64_t current_slot, const uint8_t* domains96, uint32_t target_aggregators,
+                                  uint64_t propagation_slot_range, int32_t* status_out, uint32_t* committee_out, uint32_t* data_id_out, uint8_t* bits_out,
+                                  uint8_t* sig96_out, uint8_t* msg32_out, uint64_t* target_epoch_out, uint32_t* block_idx_out, uint32_t* members_out,
+                                  uint32_t* item_off_out) {
+    B2_NVTX;
+    REQUIRE(ctx && wire && woff && members && off && domains96 && status_out && committee_out && data_id_out && bits_out && sig96_out && msg32_out &&
+                target_epoch_out && block_idx_out && members_out && item_off_out && n > 0 && n < (1u << 28) && n_committees > 0 && bits_stride > 0 &&
+                bits_stride <= 256 && (uint64_t)n * 8 * bits_stride < (1ull << 32) && committees_per_slot > 0 && slots_per_epoch > 0 &&
+                target_aggregators > 0,
+            "aggregate_and_proof_intake: bad arguments");
+    REQUIRE((uint64_t)committees_per_slot * slots_per_epoch == n_committees,
+            "aggregate_and_proof_intake: n_committees must be slots_per_epoch * committees_per_slot");
+    REQUIRE(current_slot < (1ull << 63) && intake_epoch_ok(epoch, current_slot, slots_per_epoch),
+            "aggregate_and_proof_intake: the epoch must be the current slot's epoch or the one before it");
+    REQUIRE(ctx->n_blocks > 0, "aggregate_and_proof_intake: no tree loaded (b2_tree_load)");
+    REQUIRE(ctx->n_val > 0, "aggregate_and_proof_intake: registry not loaded");
+    int rc;
+    if ((rc = check_offsets(ctx, woff, n, "aggregate_and_proof_intake: woff"))) return rc;
+    REQUIRE(woff[n] <= wire_len, "aggregate_and_proof_intake: woff ends past the wire");
+    if ((rc = check_offsets(ctx, off, n_committees, "aggregate_and_proof_intake: off"))) return rc;
+    for (uint32_t c = 0; c < n_committees; c++)
+        REQUIRE(off[c + 1] - off[c] <= 8 * bits_stride, "aggregate_and_proof_intake: a committee is larger than 8 * bits_stride");
+    const uint64_t n_sig = off[n_committees], W = 8ull * bits_stride;
+    CK(cudaSetDevice(ctx->device));
+    staging st(ctx);
+    const uint8_t* dwire = st.in(wire, wire_len, 16);
+    const uint32_t* dwoff = st.in(woff, (size_t)n + 1);
+    const uint32_t* dmem = st.in(members, n_sig, 4);
+    const uint32_t* doff = st.in(off, (size_t)n_committees + 1);
+    int32_t* dst = st.out(status_out, n);
+    uint32_t* dcom = st.out(committee_out, n);
+    uint32_t* ddid = st.out(data_id_out, n);
+    uint8_t* dbits = st.out(bits_out, (size_t)n * bits_stride);
+    uint8_t* dsig = st.out(sig96_out, (size_t)n * 96);
+    uint8_t* dmsg = st.out(msg32_out, (size_t)n * 32);
+    uint64_t* dtgt = st.out(target_epoch_out, n);
+    uint32_t* dblk = st.out(block_idx_out, n);
+    uint32_t* dmo = st.out(members_out, n * W);
+    uint32_t* dio = st.out(item_off_out, (size_t)n + 1);
+    if (st.rc) return st.rc;
+    if ((rc = b2_aggregate_and_proof_intake_dev(ctx, dwire, wire_len, dwoff, n, dmem, doff, n_committees, n_sig, committees_per_slot, slots_per_epoch,
+                                                bits_stride, epoch, current_slot, domains96, target_aggregators, propagation_slot_range, dst, dcom, ddid,
+                                                dbits, dsig, dmsg, dtgt, dblk, dmo, dio, ctx->s_main)))
         return rc;
     return st.finish();
 }

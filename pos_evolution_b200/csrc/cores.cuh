@@ -283,7 +283,8 @@ HD void sha256_pair(const uint8_t* left32, const uint8_t* right32, uint8_t* out3
     sha256_update(c, right32, 32);
     sha256_final(c, out32);
 }
-HD void attestation_signing_root(const uint8_t* data128, const uint8_t* domain32, uint8_t* out32) {
+// hash_tree_root(AttestationData) of its 128-byte serialisation
+HD void attestation_data_root(const uint8_t* data128, uint8_t* root) {
     uint8_t chunk[8][32];
 #pragma unroll 1
     for (int i = 0; i < 8; i++)
@@ -298,12 +299,16 @@ HD void attestation_signing_root(const uint8_t* data128, const uint8_t* domain32
     sha256_pair(ep, data128 + 56, chunk[3]);     // htr(source)
     for (int k = 0; k < 32; k++) ep[k] = k < 8 ? data128[88 + k] : 0;
     sha256_pair(ep, data128 + 96, chunk[4]);     // htr(target)
-    uint8_t l1[4][32], l2[2][32], root[32];
+    uint8_t l1[4][32], l2[2][32];
 #pragma unroll 1
     for (int i = 0; i < 4; i++) sha256_pair(chunk[2 * i], chunk[2 * i + 1], l1[i]);
     sha256_pair(l1[0], l1[1], l2[0]);
     sha256_pair(l1[2], l1[3], l2[1]);
     sha256_pair(l2[0], l2[1], root);
+}
+HD void attestation_signing_root(const uint8_t* data128, const uint8_t* domain32, uint8_t* out32) {
+    uint8_t root[32];
+    attestation_data_root(data128, root);
     sha256_pair(root, domain32, out32);
 }
 

@@ -18,6 +18,10 @@ PackResult = namedtuple("PackResult", "committee data bits numerator src_off src
 # Engine.attestation_intake: status per attestation; the vote form's inputs: vote per member slot, vote_off per committee, signatures in
 # committee order, and per vote (max_votes rows) the AttestationData, signing root, source and target epoch and block id
 IntakeResult = namedtuple("IntakeResult", "status vote vote_off sigs data128 msgs source_epoch target_epoch block_idx")
+# Engine.aggregate_and_proof_intake: per SignedAggregateAndProof its status (0-20), committee, data id, bit row, aggregate signature, attestation
+# signing root, target epoch and block id; the member rows (u32[n][8 * bits_stride]) and their offsets item_off (u32[n+1]), the committee
+# arrays latest_messages_update / fast_aggregate_verify take with the bit rows
+AggregateIntakeResult = namedtuple("AggregateIntakeResult", "status committee data_id bits sigs msgs target_epoch block_idx members item_off")
 
 
 def _c(a, dtype):
@@ -296,6 +300,27 @@ class Engine:
         self._ck(self.lib.b2_attestation_intake(self.h, _p(w), len(wire), _p(woff), n_att, _p(off), n_c, int(committees_per_slot),
                                                 int(slots_per_epoch), int(bits_stride), int(epoch), int(current_slot), _p(dom), mv,
                                                 *[_p(x) for x in r]))
+        return r
+
+    def aggregate_and_proof_intake(self, wire: bytes, woff, members, off, epoch: int, current_slot: int, domains96: bytes,
+                                   committees_per_slot: int, slots_per_epoch: int, bits_stride: int, target_aggregators: int = 16,
+                                   propagation_slot_range: int = 32) -> AggregateIntakeResult:
+        """One target epoch of SignedAggregateAndProof messages (SSZ encodings back to back, woff their offsets) checked and verified on
+        the device (include/b200pos.h, b2_aggregate_and_proof_intake: statuses 0-20); committee c = members[off[c] .. off[c+1]].
+        domains96 = the DOMAIN_BEACON_ATTESTER, DOMAIN_SELECTION_PROOF and DOMAIN_AGGREGATE_AND_PROOF domains of the epoch, back to back."""
+        woff, members, off = _c(woff, np.uint32), _c(members, np.uint32), _c(off, np.uint32)
+        n, n_c = woff.shape[0] - 1, off.shape[0] - 1
+        w = np.frombuffer(bytes(wire), dtype=np.uint8) if len(wire) else np.zeros(1, dtype=np.uint8)
+        mem = members if members.size else np.zeros(1, dtype=np.uint32)
+        dom = np.frombuffer(bytes(domains96), dtype=np.uint8)
+        assert dom.shape == (96,)
+        width = 8 * int(bits_stride)
+        r = AggregateIntakeResult(np.zeros(n, np.int32), np.zeros(n, np.uint32), np.zeros(n, np.uint32), np.zeros((n, bits_stride), np.uint8),
+                                  np.zeros((n, 96), np.uint8), np.zeros((n, 32), np.uint8), np.zeros(n, np.uint64), np.zeros(n, np.uint32),
+                                  np.zeros((n, width), np.uint32), np.zeros(n + 1, np.uint32))
+        self._ck(self.lib.b2_aggregate_and_proof_intake(self.h, _p(w), len(wire), _p(woff), n, _p(mem), _p(off), n_c, int(committees_per_slot),
+                                                        int(slots_per_epoch), int(bits_stride), int(epoch), int(current_slot), _p(dom),
+                                                        int(target_aggregators), int(propagation_slot_range), *[_p(x) for x in r]))
         return r
 
     def signing_roots(self, data128, domains32):
@@ -658,6 +683,27 @@ class Engine:
                                                     d_msgs.shape[0], d_status.data_ptr(), d_vote.data_ptr(), d_vote_off.data_ptr(),
                                                     d_sigs.data_ptr(), d_data128.data_ptr(), d_msgs.data_ptr(), d_source_epoch.data_ptr(),
                                                     d_target_epoch.data_ptr(), d_block_idx.data_ptr(), self._stream()))
+
+    def aggregate_and_proof_intake_dev(self, d_wire, d_woff, d_members, d_off, epoch: int, current_slot: int, domains96: bytes,
+                                       committees_per_slot: int, slots_per_epoch: int, d_status, d_committee, d_data_id, d_bits, d_sigs, d_msgs,
+                                       d_target_epoch, d_block_idx, d_members_out, d_item_off, target_aggregators: int = 16,
+                                       propagation_slot_range: int = 32):
+        """aggregate_and_proof_intake on device tensors, asynchronous on the current stream: n = d_woff.numel() - 1 items, the wire's
+        length is d_wire.numel(), bits_stride = d_bits.shape[1].  Outputs: d_status int32[n], d_committee / d_data_id / d_block_idx
+        uint32[n], d_bits uint8[n, bits_stride], d_sigs uint8[n, 96], d_msgs uint8[n, 32], d_target_epoch uint64[n], d_members_out
+        uint32[n, 8 * bits_stride], d_item_off uint32[n + 1].  on_attestation of the accepted aggregates is then
+        latest_messages_update_dev(d_members_out, d_item_off, d_bits, d_target_epoch, d_block_idx, (d_status == 0).to(torch.uint8))."""
+        dom = np.frombuffer(bytes(domains96), dtype=np.uint8)
+        assert dom.shape == (96,)
+        n, stride = d_woff.numel() - 1, d_bits.shape[1]
+        assert d_members_out.numel() == n * 8 * stride and d_item_off.numel() == n + 1
+        self._ck(self.lib.b2_aggregate_and_proof_intake_dev(self.h, d_wire.data_ptr(), d_wire.numel(), d_woff.data_ptr(), n, d_members.data_ptr(),
+                                                            d_off.data_ptr(), d_off.numel() - 1, d_members.numel(), int(committees_per_slot),
+                                                            int(slots_per_epoch), int(stride), int(epoch), int(current_slot), _p(dom),
+                                                            int(target_aggregators), int(propagation_slot_range), d_status.data_ptr(),
+                                                            d_committee.data_ptr(), d_data_id.data_ptr(), d_bits.data_ptr(), d_sigs.data_ptr(),
+                                                            d_msgs.data_ptr(), d_target_epoch.data_ptr(), d_block_idx.data_ptr(),
+                                                            d_members_out.data_ptr(), d_item_off.data_ptr(), self._stream()))
 
     def votes_empty_dev(self, d_bits, d_agg_sig, d_agg_status=None):
         """b2_votes_empty_dev on the current stream: every vote whose grouped bit row d_bits (uint8[n_votes, bits_stride]) has no attester

@@ -23,6 +23,8 @@ GENESIS_EPOCH = 0
 ZERO32 = bytes(32)
 DOMAIN_BEACON_PROPOSER = bytes.fromhex("00000000")
 DOMAIN_BEACON_ATTESTER = bytes.fromhex("01000000")
+DOMAIN_SELECTION_PROOF = bytes.fromhex("05000000")             # upstream phase 0 validator spec
+DOMAIN_AGGREGATE_AND_PROOF = bytes.fromhex("06000000")
 DOMAIN_SYNC_COMMITTEE = bytes.fromhex("07000000")
 SYNC_REWARD_WEIGHT = 2
 TIMELY_SOURCE_FLAG_INDEX, TIMELY_TARGET_FLAG_INDEX, TIMELY_HEAD_FLAG_INDEX = 0, 1, 2
@@ -55,6 +57,8 @@ class Preset:
     HISTORICAL_ROOTS_LIMIT: int = 2**24
     EPOCHS_PER_SLASHINGS_VECTOR: int = 8192
     EPOCHS_PER_ETH1_VOTING_PERIOD: int = 64
+    TARGET_AGGREGATORS_PER_COMMITTEE: int = 16    # upstream phase 0 validator spec (is_aggregator)
+    ATTESTATION_PROPAGATION_SLOT_RANGE: int = 32  # upstream phase 0 p2p spec (beacon_aggregate_and_proof)
 
 
 MAINNET = Preset("mainnet", 32, 64, 128, 90, 65536, 8192)
@@ -94,6 +98,19 @@ class AttestationData:                 # :689-697
 class Attestation:                     # :714-717
     aggregation_bits: List[bool]
     data: AttestationData
+    signature: bytes
+
+
+@dataclass
+class AggregateAndProof:               # upstream phase 0 validator spec
+    aggregator_index: int
+    aggregate: Attestation
+    selection_proof: bytes
+
+
+@dataclass
+class SignedAggregateAndProof:         # upstream phase 0 validator spec; the beacon_aggregate_and_proof gossip message
+    message: AggregateAndProof
     signature: bytes
 
 
@@ -265,6 +282,16 @@ def serialize_attestation(att: Attestation) -> bytes:
     bl = bytearray(pack_bits([list(att.aggregation_bits)], stride=n // 8 + 1)[0].tobytes())
     bl[n >> 3] |= 1 << (n & 7)
     return (228).to_bytes(4, "little") + serialize_attestation_data(att.data) + bytes(att.signature) + bytes(bl)
+
+
+def serialize_aggregate_and_proof(m: AggregateAndProof) -> bytes:
+    """SSZ: [aggregator_index u64][offset of aggregate = 108][selection_proof][Attestation]"""
+    return int(m.aggregator_index).to_bytes(8, "little") + (108).to_bytes(4, "little") + bytes(m.selection_proof) + serialize_attestation(m.aggregate)
+
+
+def serialize_signed_aggregate_and_proof(s: SignedAggregateAndProof) -> bytes:
+    """SSZ: [offset of message = 100][signature][AggregateAndProof]"""
+    return (100).to_bytes(4, "little") + bytes(s.signature) + serialize_aggregate_and_proof(s.message)
 
 
 def serialize_validators(validators) -> np.ndarray:
@@ -945,6 +972,35 @@ class Spec:
         indexed = self.get_indexed_attestation(target_state, attestation)
         assert self.is_valid_indexed_attestation(target_state, indexed)
         self.update_latest_messages(store, indexed.attesting_indices, attestation)
+
+    def validate_aggregate_and_proofs(self, state, store, items, current_slot=None):
+        """The beacon_aggregate_and_proof gossip checks (upstream phase 0 p2p spec) of a list of SignedAggregateAndProof on the GPU
+        (b2_aggregate_and_proof_intake).  Returns (status per item, the accepted items' Attestations in list order): statuses 0-20 of
+        include/b200pos.h, where an item whose data.slot lies neither in current_slot's epoch nor in the one before it gets 7.  The items
+        are split by the epoch of data.slot, one call per epoch, committees from `state`; each call starts with empty seen-caches.
+        Needs Spec(incremental_tree=True): its device tree is rooted at the finalized block, so "not in the tree" also covers the
+        IGNORE for a finalized checkpoint that is not an ancestor."""
+        if not self.incremental_tree:
+            raise ValueError("validate_aggregate_and_proofs needs Spec(incremental_tree=True): the device tree must be rooted at the finalized block")
+        current_slot = self.get_current_slot(store) if current_slot is None else int(current_slot)
+        self._sync_store(store)
+        self.sync_registry(state)
+        status = [7] * len(items)
+        cur = self.compute_epoch_at_slot(current_slot)
+        for epoch in [cur] + ([cur - 1] if cur > GENESIS_EPOCH else []):
+            sel = [i for i, x in enumerate(items) if self.compute_epoch_at_slot(x.message.aggregate.data.slot) == epoch]
+            if not sel:
+                continue
+            wires = [serialize_signed_aggregate_and_proof(items[i]) for i in sel]
+            woff = np.cumsum([0] + [len(w) for w in wires]).astype(np.uint32)
+            members, off, cps = self.epoch_committees(state, epoch)
+            stride = max(1, (int(np.diff(off.astype(np.int64)).max()) + 7) // 8)      # the bit rows of the epoch's largest committee
+            domains = b"".join(self.get_domain(state, d, epoch) for d in (DOMAIN_BEACON_ATTESTER, DOMAIN_SELECTION_PROOF, DOMAIN_AGGREGATE_AND_PROOF))
+            r = self.engine.aggregate_and_proof_intake(b"".join(wires), woff, members, off, epoch, current_slot, domains, cps, self.p.SLOTS_PER_EPOCH,
+                                                       stride, self.p.TARGET_AGGREGATORS_PER_COMMITTEE, self.p.ATTESTATION_PROPAGATION_SLOT_RANGE)
+            for k, i in enumerate(sel):
+                status[i] = int(r.status[k])
+        return status, [items[i].message.aggregate for i in range(len(items)) if status[i] == 0]
 
     @staticmethod
     def is_slashable_attestation_data(data_1, data_2):                         # :1134-1143
