@@ -537,6 +537,63 @@ int b2_aggregate_and_proof_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wir
                                   uint64_t propagation_slot_range, int32_t* status_out, uint32_t* committee_out, uint32_t* data_id_out, uint8_t* bits_out,
                                   uint8_t* sig96_out, uint8_t* msg32_out, uint64_t* target_epoch_out, uint32_t* block_idx_out, uint32_t* members_out,
                                   uint32_t* item_off_out);
+/* ---- process_attestation (pos-evolution.md:722-754) for the attestations of a run of blocks of one chain in one epoch e, block-atomic as
+ * on_block's state_transition (:1008-1009).  Inputs:
+ *   wire, woff[n_att+1], wire_len   the attestations' SSZ encodings back to back (b2_attestations_decode's form), in block order and list
+ *                                   order within a block
+ *   block_off[n_blocks+1]           block b holds attestations [block_off[b], block_off[b+1])
+ *   block_slot[n_blocks]            the state.slot of each block: strictly increasing, all in epoch e = block_slot[0] / slots_per_epoch
+ *   members, off[n_committees+1]    the committees of e - 1 (cps_prev * slots_per_epoch rows), then those of e (cps_cur * slots_per_epoch
+ *                                   rows; n_committees = their sum): committee (E, slot, index) = (E == e ? cps_prev * slots_per_epoch : 0) + (slot - start(E)) *
+ *                                   cps_E + index.  At e = 0 there is no previous epoch and cps_prev is 0.
+ *   chain_roots u8[2 * slots_per_epoch][32]   the root of slot s at s + slots_per_epoch - start(e), state.block_roots[s %
+ *                                   SLOTS_PER_HISTORICAL_ROOT] as this chain sees it; only slots below the including block's slot are read
+ *   justified80 (host)              previous_justified_checkpoint, then current_justified_checkpoint, 40 SSZ bytes each (epoch u64 LE || root)
+ *   domains64 (host)                get_domain(DOMAIN_BEACON_ATTESTER, e - 1), then the same for e
+ * plus MIN_ATTESTATION_INCLUSION_DELAY (> 0), bits_stride (1..256), EFFECTIVE_BALANCE_INCREMENT and get_base_reward_per_increment;
+ * integer_squareroot(slots_per_epoch) is computed inside.  Each attestation gets the first check it fails, in process_attestation's order:
+ *    0  passes every check
+ *    1  malformed container, or a woff row that is reversed or ends past wire_len, or an attestation in no block's row
+ *    2  empty Bitlist or no delimiter                  3  more bits than 8 * bits_stride
+ *    4  target.epoch is neither e - 1 nor e (:724)     5  target.epoch != compute_epoch_at_slot(data.slot) (:725)
+ *    6  not data.slot + MIN_ATTESTATION_INCLUSION_DELAY <= block slot <= data.slot + SLOTS_PER_EPOCH (:726)
+ *    7  data.index >= committees_per_slot of the target epoch (:727)
+ *    8  Bitlist length != committee size (:730); a malformed committee row matches no length
+ *    9  data.source != the justified checkpoint of the target epoch (:733, is_matching_source)
+ *   10  no bit set (:736, is_valid_indexed_attestation on empty indices)     11  FastAggregateVerify fails (:736)
+ * Outputs per attestation: status; flag_mask (bit f = participation flag f, get_attestation_participation_flag_indices with inclusion_delay =
+ * block slot - data.slot; 0 unless checks 1-9 pass); numerator u64 (proposer_reward_numerator of :745-749, 0 where not applied).  Per block:
+ * block_status (0 applied, 1 invalid: its row is malformed or it holds a nonzero status, 2 valid but after the first invalid block);
+ * block_first, the list index of its first failing attestation or 0xFFFFFFFF; block_reward, the sum over its attestations of numerator //
+ * 448 (:752-754, the proposer's increase_balance).  n_applied: the blocks applied, those before the first invalid one.  They set the flags of
+ * the attestations with target e in participation table 0 and of those with target e - 1 in table 1, order-exact over (block, list) order
+ * (a repeated attestation is valid and earns nothing); rewards read the registry's effective balances; nothing of the first invalid block
+ * or of a later one changes a table.  b2_set_verify_mode applies to the FastAggregateVerify.
+ * b2_block_attestations_dev is asynchronous on `stream` and self-guarding: a woff row that is reversed or ends past wire_len is status 1, a
+ * committee row that is reversed, ends past n_sig or exceeds 8 * bits_stride is status 8, and a block whose block_off row is reversed or
+ * ends past n_att, whose slot is outside e or not above the previous block's, is invalid (all B2_GUARD_BAD_ROW); a member index >=
+ * n_validators fails FastAggregateVerify (B2_GUARD_BAD_INDEX); nothing is read or written out of bounds.  It shares the verify buffers of
+ * pipeline slot 0 with the synchronous verify entry points and the aggregate intake: enqueue those on the same stream.  The registry and
+ * the participation tables must not change while a call is in flight.  b2_block_attestations takes host arrays and returns when done; a
+ * rejected call (B2_EINVAL: no registry or a participation table not loaded, a woff, block_off or off row that does not start at 0 or
+ * decreases, woff ending past the wire, block_off not ending at n_att, a committee larger than 8 * bits_stride, block slots that do not
+ * increase strictly or leave one epoch, cps_prev != 0 exactly when e == 0, a committee count other than slots_per_epoch * (cps_prev +
+ * cps_cur) (the device form refuses that too), bits_stride 0 or > 256, n_att == 0 or n_blocks == 0) writes no
+ * output and changes nothing. */
+int b2_block_attestations_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n_att, const uint32_t* d_block_off,
+                              const uint64_t* d_block_slot, uint32_t n_blocks, const uint32_t* d_members, const uint32_t* d_off, uint32_t n_committees,
+                              uint64_t n_sig,
+                              uint32_t cps_prev, uint32_t cps_cur, const uint8_t* d_chain_roots, const uint8_t* justified80, const uint8_t* domains64,
+                              uint32_t slots_per_epoch, uint32_t min_inclusion_delay, uint32_t bits_stride, uint64_t effective_balance_increment,
+                              uint64_t base_reward_per_increment, int32_t* d_status_out, uint8_t* d_flag_mask_out, uint64_t* d_numerator_out,
+                              int32_t* d_block_status_out, uint32_t* d_block_first_out, uint64_t* d_block_reward_out, uint32_t* d_n_applied_out,
+                              void* stream);
+int b2_block_attestations(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n_att, const uint32_t* block_off,
+                          const uint64_t* block_slot, uint32_t n_blocks, const uint32_t* members, const uint32_t* off, uint32_t n_committees,
+                          uint32_t cps_prev, uint32_t cps_cur, const uint8_t* chain_roots, const uint8_t* justified80, const uint8_t* domains64, uint32_t slots_per_epoch,
+                          uint32_t min_inclusion_delay, uint32_t bits_stride, uint64_t effective_balance_increment, uint64_t base_reward_per_increment,
+                          int32_t* status_out, uint8_t* flag_mask_out, uint64_t* numerator_out, int32_t* block_status_out, uint32_t* block_first_out,
+                          uint64_t* block_reward_out, uint32_t* n_applied_out);
 int b2_latest_messages_update_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_off, const uint8_t* d_bits,
                                   uint32_t bits_stride, const uint64_t* d_target_epoch, const uint32_t* d_block_idx,
                                   const uint8_t* d_accept, uint32_t n_agg, void* stream);

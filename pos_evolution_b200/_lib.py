@@ -112,6 +112,13 @@ SIGNATURES = {
                                                   c_uint32, c_uint32, c_uint64, c_uint64, c_void_p, c_uint32, c_uint64] + [c_void_p] * 11),
     "b2_aggregate_and_proof_intake": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_uint32, c_uint32,
                                               c_uint32, c_uint64, c_uint64, c_void_p, c_uint32, c_uint64] + [c_void_p] * 10),
+    # ctx, wire, wire_len, woff, n_att, block_off, block_slot, n_blocks, members, off, n_committees, [n_sig,] cps_prev, cps_cur, chain_roots, justified80,
+    # domains64, slots_per_epoch, min_inclusion_delay, bits_stride, increment, base_reward_per_increment, seven outputs[, stream]
+    "b2_block_attestations_dev": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32,
+                                          c_uint64, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p, c_uint32, c_uint32, c_uint32, c_uint64,
+                                          c_uint64] + [c_void_p] * 8),
+    "b2_block_attestations": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p,
+                                      c_uint32, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p, c_uint32, c_uint32, c_uint32, c_uint64, c_uint64] + [c_void_p] * 7),
     "b2_vote_weights_dev": (c_int, [c_void_p, c_void_p, c_void_p]),
     "b2_vote_weights_range_dev": (c_int, [c_void_p, c_uint64, c_uint64, c_void_p, c_void_p]),
     "b2_guard_flags": (c_int, [c_void_p, c_void_p]),

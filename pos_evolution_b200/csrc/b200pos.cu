@@ -23,6 +23,7 @@
 #include "votes.cuh"
 #include "intake.cuh"
 #include "aggintake.cuh"
+#include "blockatt.cuh"
 
 using namespace b2;
 
@@ -132,6 +133,11 @@ struct api_scratch {
     dbuf av_signer, av_off, av_msg, av_sig, av_ok;
 };
 
+// block attestations (blockatt.cuh): per attestation, plus its member row u32[8 * bits_stride]
+struct ba_scratch {
+    dbuf blk_of, cur, fav_ok, accept, num1, bits, sig96, data128, dom32, msg32, members, item_off;
+};
+
 struct vslot {
     dbuf haff, hflag, pkjac, pkst, saff, sflag, f, sumjac;
     dbuf g2aff, g2st;                                      // the slot's own decompressed signatures (pipelined epochs)
@@ -216,6 +222,7 @@ struct b2_ctx {
     ssz_tables ssz;
     intake_scratch in;
     api_scratch api;
+    ba_scratch ba;
 };
 
 struct nvtx_scope {
@@ -1569,6 +1576,166 @@ int b2_aggregate_and_proof_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wir
     if ((rc = b2_aggregate_and_proof_intake_dev(ctx, dwire, wire_len, dwoff, n, dmem, doff, n_committees, n_sig, committees_per_slot, slots_per_epoch,
                                                 bits_stride, epoch, current_slot, domains96, target_aggregators, propagation_slot_range, dst, dcom, ddid,
                                                 dbits, dsig, dmsg, dtgt, dblk, dmo, dio, ctx->s_main)))
+        return rc;
+    return st.finish();
+}
+
+// ------------------------------------------------------------------------------------------ block attestations (blockatt.cuh)
+static uint32_t isqrt_u32(uint32_t n) {
+    uint32_t x = 0;
+    while ((uint64_t)(x + 1) * (x + 1) <= n) x++;
+    return x;
+}
+
+int b2_block_attestations_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n_att, const uint32_t* d_block_off,
+                              const uint64_t* d_block_slot, uint32_t n_blocks, const uint32_t* d_members, const uint32_t* d_off, uint32_t n_committees,
+                              uint64_t n_sig,
+                              uint32_t cps_prev, uint32_t cps_cur, const uint8_t* d_chain_roots, const uint8_t* justified80, const uint8_t* domains64,
+                              uint32_t slots_per_epoch, uint32_t min_inclusion_delay, uint32_t bits_stride, uint64_t effective_balance_increment,
+                              uint64_t base_reward_per_increment, int32_t* d_status_out, uint8_t* d_flag_mask_out, uint64_t* d_numerator_out,
+                              int32_t* d_block_status_out, uint32_t* d_block_first_out, uint64_t* d_block_reward_out, uint32_t* d_n_applied_out,
+                              void* stream) {
+    B2_NVTX;
+    REQUIRE(ctx && d_wire && d_woff && d_block_off && d_block_slot && d_members && d_off && d_chain_roots && justified80 && domains64 && d_status_out &&
+                d_flag_mask_out && d_numerator_out && d_block_status_out && d_block_first_out && d_block_reward_out && d_n_applied_out && n_att > 0 &&
+                n_att < (1u << 28) && n_blocks > 0 && n_sig < (1ull << 32) && bits_stride > 0 && bits_stride <= 256 &&
+                (uint64_t)n_att * 8 * bits_stride < (1ull << 32) && slots_per_epoch > 0 && cps_cur > 0 &&
+                ((uint64_t)cps_prev + cps_cur) * slots_per_epoch < (1ull << 31) && min_inclusion_delay > 0 && effective_balance_increment > 0,
+            "block_attestations_dev: bad arguments");
+    REQUIRE(((uint64_t)cps_prev + cps_cur) * slots_per_epoch == n_committees,
+            "block_attestations: n_committees must be slots_per_epoch * (cps_prev + cps_cur)");
+    REQUIRE(ctx->n_val > 0, "block_attestations: registry not loaded");
+    REQUIRE(ctx->reg.part[0] && ctx->reg.part[1], "block_attestations: both participation tables must be loaded (b2_participation_load)");
+    CK(cudaSetDevice(ctx->device));
+    ba_scratch& S = ctx->ba;
+    const size_t n = n_att, W = 8ull * bits_stride;
+    int rc;
+    if ((rc = ensure(ctx, S.blk_of, n * 4)) || (rc = ensure(ctx, S.cur, n)) || (rc = ensure(ctx, S.fav_ok, n)) || (rc = ensure(ctx, S.accept, 2 * n)) ||
+        (rc = ensure(ctx, S.num1, n * 8)) || (rc = ensure(ctx, S.bits, n * bits_stride + 16)) || (rc = ensure(ctx, S.sig96, n * 96)) ||
+        (rc = ensure(ctx, S.data128, n * 128)) || (rc = ensure(ctx, S.dom32, n * 32)) || (rc = ensure(ctx, S.msg32, n * 32)) ||
+        (rc = ensure(ctx, S.members, n * W * 4)) || (rc = ensure(ctx, S.item_off, (n + 1) * 4)))
+        return rc;
+    ba_args A = {};
+    A.wire = d_wire;
+    A.wire_len = wire_len;
+    A.woff = d_woff;
+    A.n = n_att;
+    A.block_off = d_block_off;
+    A.block_slot = d_block_slot;
+    A.n_blocks = n_blocks;
+    A.members = d_members;
+    A.T.off = d_off;
+    A.T.n_sig = n_sig;
+    A.T.bits_stride = bits_stride;
+    A.cps_prev = cps_prev;
+    A.cps_cur = cps_cur;
+    A.slots_per_epoch = slots_per_epoch;
+    A.bits_stride = bits_stride;
+    A.min_delay = min_inclusion_delay;
+    A.isqrt_spe = isqrt_u32(slots_per_epoch);
+    A.chain_roots = d_chain_roots;
+    memcpy(A.justified.b, justified80, 80);
+    memcpy(A.dom[0].b, domains64, 32);
+    memcpy(A.dom[1].b, domains64 + 32, 32);
+    A.blk_of = S.blk_of;
+    A.cur = S.cur;
+    A.fav_ok = S.fav_ok;
+    A.accept = S.accept;
+    A.num1 = S.num1;
+    A.bits = S.bits;
+    A.sig96 = S.sig96;
+    A.data128 = S.data128;
+    A.dom32 = S.dom32;
+    A.members_out = S.members;
+    A.item_off = S.item_off;
+    A.status = d_status_out;
+    A.flag_mask = d_flag_mask_out;
+    A.numerator = (unsigned long long*)d_numerator_out;
+    A.block_status = d_block_status_out;
+    A.block_first = d_block_first_out;
+    A.block_reward = (unsigned long long*)d_block_reward_out;
+    A.n_applied = d_n_applied_out;
+    A.guard = ctx->d_guard;
+    cudaStream_t s = (cudaStream_t)stream;
+    k_ba_parse<<<blocks_for((uint64_t)n_att * 32, 128), 128, 0, s>>>(A);
+    CKL(ctx);
+    k_signing_roots<<<blocks_for(n_att, 64), 64, 0, s>>>(S.data128, S.dom32, 32u, n_att, S.msg32);
+    CKL(ctx);
+    pk_source P = {S.members, S.item_off, (const uint8_t*)S.bits, bits_stride, nullptr, 0};
+    if ((rc = verify_fork(ctx, ctx->slot[0], P, S.msg32, n_att, s)) || (rc = verify_main(ctx, ctx->slot[0], S.sig96, n_att, S.fav_ok, s))) return rc;
+    k_ba_blocks<<<1, BA_BLOCKS_THREADS, 0, s>>>(A);
+    CKL(ctx);
+    // the flag scatter of :745-749, order-exact over (block, list) order: table 0 (target e) writes `numerator`, table 1 (target e - 1) num1
+    const registry_tables& R = ctx->reg;
+    const uint8_t* db = S.bits;
+    for (int which = 0; which < 2; which++) {
+        const uint8_t* acc = (const uint8_t*)S.accept.p + (size_t)which * n;
+        unsigned long long* num = which == 0 ? (unsigned long long*)d_numerator_out : (unsigned long long*)S.num1.p;
+        k_part_phase1<<<n_att, 128, 0, s>>>(S.members, S.item_off, db, bits_stride, d_flag_mask_out, acc, n_att, R.part[which], R.part_first);
+        CKL(ctx);
+        k_part_phase2<<<n_att, 128, 0, s>>>(S.members, S.item_off, db, bits_stride, d_flag_mask_out, acc, n_att, R.part_first, R.eff,
+                                            effective_balance_increment, base_reward_per_increment, num);
+        CKL(ctx);
+        k_part_phase3<<<n_att, 128, 0, s>>>(S.members, S.item_off, db, bits_stride, d_flag_mask_out, acc, n_att, R.part_first, R.part[which]);
+        CKL(ctx);
+    }
+    k_ba_rewards<<<blocks_for((uint64_t)n_blocks * 32, 128), 128, 0, s>>>(A);
+    CKL(ctx);
+    return B2_OK;
+}
+
+int b2_block_attestations(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n_att, const uint32_t* block_off,
+                          const uint64_t* block_slot, uint32_t n_blocks, const uint32_t* members, const uint32_t* off, uint32_t n_committees, uint32_t cps_prev,
+                          uint32_t cps_cur, const uint8_t* chain_roots, const uint8_t* justified80, const uint8_t* domains64, uint32_t slots_per_epoch,
+                          uint32_t min_inclusion_delay, uint32_t bits_stride, uint64_t effective_balance_increment, uint64_t base_reward_per_increment,
+                          int32_t* status_out, uint8_t* flag_mask_out, uint64_t* numerator_out, int32_t* block_status_out, uint32_t* block_first_out,
+                          uint64_t* block_reward_out, uint32_t* n_applied_out) {
+    B2_NVTX;
+    REQUIRE(ctx && wire && woff && block_off && block_slot && members && off && chain_roots && justified80 && domains64 && status_out && flag_mask_out &&
+                numerator_out && block_status_out && block_first_out && block_reward_out && n_applied_out && n_att > 0 && n_att < (1u << 28) &&
+                n_blocks > 0 && bits_stride > 0 && bits_stride <= 256 && (uint64_t)n_att * 8 * bits_stride < (1ull << 32) && slots_per_epoch > 0 &&
+                cps_cur > 0 && ((uint64_t)cps_prev + cps_cur) * slots_per_epoch < (1ull << 31) && min_inclusion_delay > 0 &&
+                effective_balance_increment > 0,
+            "block_attestations: bad arguments");
+    REQUIRE(((uint64_t)cps_prev + cps_cur) * slots_per_epoch == n_committees,
+            "block_attestations: n_committees must be slots_per_epoch * (cps_prev + cps_cur)");
+    REQUIRE(ctx->n_val > 0, "block_attestations: registry not loaded");
+    REQUIRE(ctx->reg.part[0] && ctx->reg.part[1], "block_attestations: both participation tables must be loaded (b2_participation_load)");
+    int rc;
+    if ((rc = check_offsets(ctx, woff, n_att, "block_attestations: woff"))) return rc;
+    REQUIRE(woff[n_att] <= wire_len, "block_attestations: woff ends past the wire");
+    if ((rc = check_offsets(ctx, block_off, n_blocks, "block_attestations: block_off"))) return rc;
+    REQUIRE(block_off[n_blocks] == n_att, "block_attestations: block_off must end at n_att");
+    const uint64_t e = block_slot[0] / slots_per_epoch;
+    REQUIRE(block_slot[0] < (1ull << 63), "block_attestations: block slot out of range");
+    for (uint32_t b = 1; b < n_blocks; b++)
+        REQUIRE(block_slot[b] > block_slot[b - 1] && block_slot[b] / slots_per_epoch == e,
+                "block_attestations: block slots must increase strictly and lie in one epoch");
+    REQUIRE(e > 0 ? cps_prev > 0 : cps_prev == 0, "block_attestations: cps_prev must be 0 exactly at epoch 0");
+    if ((rc = check_offsets(ctx, off, n_committees, "block_attestations: off"))) return rc;
+    for (uint32_t c = 0; c < n_committees; c++)
+        REQUIRE(off[c + 1] - off[c] <= 8 * bits_stride, "block_attestations: a committee is larger than 8 * bits_stride");
+    const uint64_t n_sig = off[n_committees];
+    CK(cudaSetDevice(ctx->device));
+    staging st(ctx);
+    const uint8_t* dwire = st.in(wire, wire_len, 16);
+    const uint32_t* dwoff = st.in(woff, (size_t)n_att + 1);
+    const uint32_t* dboff = st.in(block_off, (size_t)n_blocks + 1);
+    const uint64_t* dbslot = st.in(block_slot, n_blocks);
+    const uint32_t* dmem = st.in(members, n_sig, 4);
+    const uint32_t* doff = st.in(off, (size_t)n_committees + 1);
+    const uint8_t* droots = st.in(chain_roots, 64ull * slots_per_epoch);
+    int32_t* dst = st.out(status_out, n_att);
+    uint8_t* dmask = st.out(flag_mask_out, n_att);
+    uint64_t* dnum = st.out(numerator_out, n_att);
+    int32_t* dbst = st.out(block_status_out, n_blocks);
+    uint32_t* dbfirst = st.out(block_first_out, n_blocks);
+    uint64_t* dbrew = st.out(block_reward_out, n_blocks);
+    uint32_t* dnapp = st.out(n_applied_out, 1);
+    if (st.rc) return st.rc;
+    if ((rc = b2_block_attestations_dev(ctx, dwire, wire_len, dwoff, n_att, dboff, dbslot, n_blocks, dmem, doff, n_committees, n_sig, cps_prev, cps_cur, droots,
+                                        justified80, domains64, slots_per_epoch, min_inclusion_delay, bits_stride, effective_balance_increment,
+                                        base_reward_per_increment, dst, dmask, dnum, dbst, dbfirst, dbrew, dnapp, ctx->s_main)))
         return rc;
     return st.finish();
 }

@@ -22,6 +22,10 @@ IntakeResult = namedtuple("IntakeResult", "status vote vote_off sigs data128 msg
 # signing root, target epoch and block id; the member rows (u32[n][8 * bits_stride]) and their offsets item_off (u32[n+1]), the committee
 # arrays latest_messages_update / fast_aggregate_verify take with the bit rows
 AggregateIntakeResult = namedtuple("AggregateIntakeResult", "status committee data_id bits sigs msgs target_epoch block_idx members item_off")
+# Engine.block_attestations: per attestation its status (0-11), participation flag mask and proposer_reward_numerator; per block its status
+# (0 applied, 1 invalid, 2 after an invalid block), the list index of its first failing attestation (0xFFFFFFFF: none) and proposer reward;
+# the number of blocks applied
+BlockAttestationsResult = namedtuple("BlockAttestationsResult", "status flag_mask numerator block_status block_first block_reward n_applied")
 
 
 def _c(a, dtype):
@@ -322,6 +326,29 @@ class Engine:
                                                         int(slots_per_epoch), int(bits_stride), int(epoch), int(current_slot), _p(dom),
                                                         int(target_aggregators), int(propagation_slot_range), *[_p(x) for x in r]))
         return r
+
+    def block_attestations(self, wire: bytes, woff, block_off, block_slot, members, off, cps_prev: int, cps_cur: int, chain_roots,
+                           justified80: bytes, domains64: bytes, slots_per_epoch: int, min_inclusion_delay: int, bits_stride: int,
+                           increment: int, base_reward_per_increment: int) -> BlockAttestationsResult:
+        """process_attestation for the attestations of a run of blocks of one epoch (include/b200pos.h, b2_block_attestations): the
+        SSZ encodings back to back (woff their offsets), block b = attestations [block_off[b], block_off[b+1]) included at block_slot[b];
+        committee c = members[off[c] .. off[c+1]], those of epoch e - 1 then those of e; chain_roots uint8[2 * slots_per_epoch, 32].
+        Applies the blocks before the first invalid one to the device participation tables (both must be loaded)."""
+        woff, block_off, members, off = _c(woff, np.uint32), _c(block_off, np.uint32), _c(members, np.uint32), _c(off, np.uint32)
+        block_slot = _c(block_slot, np.uint64)
+        roots = _c(chain_roots, np.uint8).reshape(-1)
+        n, n_b = woff.shape[0] - 1, block_off.shape[0] - 1
+        w = np.frombuffer(bytes(wire), dtype=np.uint8) if len(wire) else np.zeros(1, dtype=np.uint8)
+        mem = members if members.size else np.zeros(1, dtype=np.uint32)
+        j, dom = np.frombuffer(bytes(justified80), dtype=np.uint8), np.frombuffer(bytes(domains64), dtype=np.uint8)
+        assert j.shape == (80,) and dom.shape == (64,) and roots.shape == (64 * int(slots_per_epoch),) and block_slot.shape == (max(n_b, 0),)
+        r = BlockAttestationsResult(np.zeros(n, np.int32), np.zeros(n, np.uint8), np.zeros(n, np.uint64), np.zeros(n_b, np.int32),
+                                    np.zeros(n_b, np.uint32), np.zeros(n_b, np.uint64), np.zeros(1, np.uint32))
+        self._ck(self.lib.b2_block_attestations(self.h, _p(w), len(wire), _p(woff), n, _p(block_off), _p(block_slot), n_b, _p(mem), _p(off),
+                                                off.shape[0] - 1, int(cps_prev), int(cps_cur), _p(roots), _p(j), _p(dom), int(slots_per_epoch),
+                                                int(min_inclusion_delay), int(bits_stride), int(increment), int(base_reward_per_increment),
+                                                *[_p(x) for x in r]))
+        return r._replace(n_applied=int(r.n_applied[0]))
 
     def signing_roots(self, data128, domains32):
         """compute_signing_root for n attestations: data128 uint8[n,128] (SSZ-serialised AttestationData), domains32 uint8[32] or uint8[n,32]."""
@@ -704,6 +731,24 @@ class Engine:
                                                             d_committee.data_ptr(), d_data_id.data_ptr(), d_bits.data_ptr(), d_sigs.data_ptr(),
                                                             d_msgs.data_ptr(), d_target_epoch.data_ptr(), d_block_idx.data_ptr(),
                                                             d_members_out.data_ptr(), d_item_off.data_ptr(), self._stream()))
+
+    def block_attestations_dev(self, d_wire, d_woff, d_block_off, d_block_slot, d_members, d_off, cps_prev: int, cps_cur: int, d_chain_roots,
+                               justified80: bytes, domains64: bytes, slots_per_epoch: int, min_inclusion_delay: int, bits_stride: int,
+                               increment: int, base_reward_per_increment: int, d_status, d_flag_mask, d_numerator, d_block_status, d_block_first,
+                               d_block_reward, d_n_applied):
+        """block_attestations on device tensors, asynchronous on the current stream: n_att = d_woff.numel() - 1, n_blocks =
+        d_block_off.numel() - 1, the wire's length is d_wire.numel(), n_sig = d_members.numel().  Outputs: d_status int32[n_att],
+        d_flag_mask uint8[n_att], d_numerator uint64[n_att], d_block_status int32[n_blocks], d_block_first uint32[n_blocks], d_block_reward
+        uint64[n_blocks], d_n_applied uint32[1]."""
+        j, dom = np.frombuffer(bytes(justified80), dtype=np.uint8), np.frombuffer(bytes(domains64), dtype=np.uint8)
+        assert j.shape == (80,) and dom.shape == (64,)
+        self._ck(self.lib.b2_block_attestations_dev(self.h, d_wire.data_ptr(), d_wire.numel(), d_woff.data_ptr(), d_woff.numel() - 1,
+                                                    d_block_off.data_ptr(), d_block_slot.data_ptr(), d_block_off.numel() - 1, d_members.data_ptr(),
+                                                    d_off.data_ptr(), d_off.numel() - 1, d_members.numel(), int(cps_prev), int(cps_cur), d_chain_roots.data_ptr(), _p(j),
+                                                    _p(dom), int(slots_per_epoch), int(min_inclusion_delay), int(bits_stride), int(increment),
+                                                    int(base_reward_per_increment), d_status.data_ptr(), d_flag_mask.data_ptr(),
+                                                    d_numerator.data_ptr(), d_block_status.data_ptr(), d_block_first.data_ptr(),
+                                                    d_block_reward.data_ptr(), d_n_applied.data_ptr(), self._stream()))
 
     def votes_empty_dev(self, d_bits, d_agg_sig, d_agg_status=None):
         """b2_votes_empty_dev on the current stream: every vote whose grouped bit row d_bits (uint8[n_votes, bits_stride]) has no attester

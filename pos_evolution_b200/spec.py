@@ -102,6 +102,14 @@ class Attestation:                     # :714-717
 
 
 @dataclass
+class BlockAttestations:               # the attestations of one block (BeaconBlockBody.attestations, :639) and what processing them needs
+    slot: int                          # the block's slot: state.slot when process_block runs
+    proposer_index: int                # the block's proposer, credited with the proposer rewards (:753-754)
+    root: bytes                        # the block's root: state.block_roots of its slot and of the slots skipped after it
+    attestations: List[Attestation]
+
+
+@dataclass
 class AggregateAndProof:               # upstream phase 0 validator spec
     aggregator_index: int
     aggregate: Attestation
@@ -783,6 +791,63 @@ class Spec:
             tables[which][:] = eng.participation_read(which).tolist()
             for v in num:
                 state.balances[proposer] += int(v) // denominator
+
+    def process_block_attestations(self, state, blocks):
+        """process_attestation (:722-754) for every attestation of a run of consecutive blocks of the state's chain in one epoch, one GPU
+        call (b2_block_attestations): state.slot == blocks[0].slot, the state as process_block sees the first block.  Block-atomic as
+        on_block's state_transition (:1008-1009): the blocks before the first invalid one are applied in order (participation flags, and
+        each block's proposer reward credited to its proposer_index), nothing of that block or of a later one.  The chain's roots below
+        blocks[0].slot come from state.block_roots; block k's root stands for the slots [slot_k, slot_{k+1}).  state.slot and block_roots
+        are left as they are.  Returns (n_applied, statuses): per block, the status (0-11, include/b200pos.h) of each attestation."""
+        assert blocks and state.slot == blocks[0].slot
+        block_off = np.concatenate([[0], np.cumsum([len(b.attestations) for b in blocks])]).astype(np.uint32)
+        if not block_off[-1]:
+            return len(blocks), [np.zeros(0, np.int32) for _ in blocks]
+        args = self.block_attestations_inputs(state, blocks)
+        self.sync_registry(state)              # first: a registry reload drops the device participation tables
+        eng = self.engine
+        eng.participation_load(0, np.asarray(state.current_epoch_participation, dtype=np.uint8))
+        eng.participation_load(1, np.asarray(state.previous_epoch_participation, dtype=np.uint8))
+        res = eng.block_attestations(**args)
+        if res.n_applied:
+            state.current_epoch_participation[:] = eng.participation_read(0).tolist()
+            state.previous_epoch_participation[:] = eng.participation_read(1).tolist()
+            for k in range(res.n_applied):
+                state.balances[blocks[k].proposer_index] += int(res.block_reward[k])
+        return res.n_applied, [res.status[block_off[k]:block_off[k + 1]] for k in range(len(blocks))]
+
+    def block_attestations_inputs(self, state, blocks):
+        """The arguments of Engine.block_attestations for these blocks on this state (as process_block_attestations passes them): the
+        attestations' encodings and offsets, the committees of epochs e - 1 and e, the chain's roots (state.block_roots below
+        blocks[0].slot, block k's root for [slot_k, slot_{k+1})), the justified checkpoints, the attester domains and the scalars."""
+        p = self.p
+        spe = p.SLOTS_PER_EPOCH
+        e = blocks[0].slot // spe
+        mem_c, off_c, cps_c = self.epoch_committees(state, e)
+        if e > 0:
+            mem_p, off_p, cps_p = self.epoch_committees(state, e - 1)
+            members = np.concatenate([mem_p, mem_c]).astype(np.uint32)
+            off = np.concatenate([off_p[:-1], off_c + np.uint32(len(mem_p))]).astype(np.uint32)
+        else:
+            members, off, cps_p = mem_c, off_c, 0
+        start = e * spe
+        roots = []
+        for s in range(start - spe, start + spe):
+            if s < blocks[0].slot:
+                roots.append(bytes(state.block_roots[s % p.SLOTS_PER_HISTORICAL_ROOT]) if s >= 0 else bytes(32))
+            else:
+                roots.append(bytes([b for b in blocks if b.slot <= s][-1].root))
+        cps = lambda c: int(c.epoch).to_bytes(8, "little") + bytes(c.root)      # noqa: E731
+        wires = [serialize_attestation(a) for b in blocks for a in b.attestations]
+        return dict(wire=b"".join(wires), woff=np.concatenate([[0], np.cumsum([len(w) for w in wires])]).astype(np.uint32),
+                    block_off=np.concatenate([[0], np.cumsum([len(b.attestations) for b in blocks])]).astype(np.uint32),
+                    block_slot=np.array([b.slot for b in blocks], dtype=np.uint64), members=members, off=off, cps_prev=cps_p, cps_cur=cps_c,
+                    chain_roots=np.frombuffer(b"".join(roots), dtype=np.uint8),
+                    justified80=cps(state.previous_justified_checkpoint) + cps(state.current_justified_checkpoint),
+                    domains64=self.get_domain(state, DOMAIN_BEACON_ATTESTER, max(e, 1) - 1) + self.get_domain(state, DOMAIN_BEACON_ATTESTER, e),
+                    slots_per_epoch=spe, min_inclusion_delay=p.MIN_ATTESTATION_INCLUSION_DELAY,
+                    bits_stride=max(1, (int(np.diff(off.astype(np.int64)).max()) + 7) // 8), increment=p.EFFECTIVE_BALANCE_INCREMENT,
+                    base_reward_per_increment=self.get_base_reward_per_increment(state))
 
     # ------------------------------------------------------------------ block packing (BeaconBlockBody.attestations :639, :659)
     def get_attestations_for_block(self, state, pool, max_attestations=None) -> List[Attestation]:
