@@ -594,6 +594,48 @@ int b2_block_attestations(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, c
                           uint32_t min_inclusion_delay, uint32_t bits_stride, uint64_t effective_balance_increment, uint64_t base_reward_per_increment,
                           int32_t* status_out, uint8_t* flag_mask_out, uint64_t* numerator_out, int32_t* block_status_out, uint32_t* block_first_out,
                           uint64_t* block_reward_out, uint32_t* n_applied_out);
+/* ---- One slot of sync committee messages from gossip: SyncCommitteeMessage (pos-evolution.md:548-557) checked as the sync_committee_{subnet_id}
+ * topics of the upstream Altair p2p spec require, grouped by beacon_block_root, and summed into each subnet's SyncCommitteeContribution and each
+ * root's SyncAggregate as process_sync_committee_contributions of the upstream Altair validator spec builds them.  Inputs:
+ *   wire, woff[n+1], wire_len     the messages' SSZ encodings back to back: slot u64 | beacon_block_root 32 | validator_index u64 | signature 96
+ *   subnet[n]                     the subnet id of the topic each message arrived on
+ *   position_validator[committee_size]   the registry index of each position of the sync committee (the first registry index of its key, as
+ *                                 process_sync_aggregate maps it); a validator may hold several positions
+ *   committee_size, subnet_count  subcommittee size = committee_size / subnet_count; subnet s holds positions [s * size / count, (s + 1) * ...)
+ *   current_slot, domain32 (host) get_domain(state, DOMAIN_SYNC_COMMITTEE, epoch of current_slot)
+ * Each message gets the first check it fails (IGNORE or REJECT as the p2p spec classes it):
+ *    0  accepted
+ *    1  REJECT  not 144 bytes, or a woff row that is reversed or ends past wire_len
+ *    2  IGNORE  slot != current_slot (clock disparity is the caller's)
+ *    3  REJECT  validator_index >= n_validators
+ *    4  REJECT  subnet_id is not one of the validator's subnets (no position p of it with p / subcommittee size == subnet_id), subnet_id >= count
+ *    5  IGNORE  an earlier message of the list with the same (validator_index, subnet_id) was accepted (checked before the signature)
+ *    6  REJECT  Verify(registry key, sha256(beacon_block_root || domain32), signature) fails, a key that failed KeyValidate included
+ * Outputs: status i32[n]; root_id u32[n], the accepted messages' distinct roots numbered by first occurrence in the list, 0xFFFFFFFF for the
+ * others; roots32 u8[n][32] and n_roots u32[1] (rows >= n_roots are zero).  Per (root r, subnet s), row r * subnet_count + s:
+ * contrib_bits u8[n * subnet_count][ceil(subcommittee size / 8)], a Bitvector with bit i set iff the validator at position s * subcommittee size
+ * + i has an accepted message on subnet s naming root r; contrib_sig96 the sum of those validators' signatures, one term per set bit (a
+ * validator at k positions of the subnet counts k times, as eth_fast_aggregate_verify over the positions needs); contrib_present u8, 0 where no
+ * bit is set (bits and signature then zero).  Per root: agg_bits u8[n][ceil(committee_size / 8)], the subnets' rows concatenated bit by bit,
+ * and agg_sig96, the sum over every set position (bls.Aggregate of the present contributions): the SyncAggregate a proposer includes for that
+ * root, which b2_sync_aggregate_verify accepts.  Rows of roots >= n_roots are zero.
+ * b2_sync_committee_messages_dev is asynchronous on `stream` and self-guarding: a reversed woff row or one past wire_len is status 1
+ * (B2_GUARD_BAD_ROW), a bad subnet is status 4, and a position_validator entry >= n_validators matches nothing (B2_GUARD_BAD_INDEX).  It needs
+ * the registry (not b2_sync_committee_load's tables) and shares the AggregateVerify buffers with b2_aggregate_verify[_pks, _dev] and the
+ * intakes: enqueue those and this call on one stream.  The registry must not change while a call is in flight.
+ * b2_sync_committee_messages takes host arrays and returns when done; a rejected call (B2_EINVAL: a woff that does not start at 0, decreases or
+ * ends past the wire, a position_validator entry >= n_validators, committee_size not a multiple of subnet_count or above 1024, no registry,
+ * n == 0) writes no output and changes nothing. */
+int b2_sync_committee_messages_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n, const uint32_t* d_subnet,
+                                   const uint32_t* d_position_validator, uint32_t committee_size, uint32_t subnet_count, uint64_t current_slot,
+                                   const uint8_t* domain32, int32_t* d_status_out, uint32_t* d_root_id_out, uint8_t* d_roots32_out,
+                                   uint32_t* d_n_roots_out, uint8_t* d_contrib_bits_out, uint8_t* d_contrib_sig96_out, uint8_t* d_contrib_present_out,
+                                   uint8_t* d_agg_bits_out, uint8_t* d_agg_sig96_out, void* stream);
+int b2_sync_committee_messages(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n, const uint32_t* subnet,
+                               const uint32_t* position_validator, uint32_t committee_size, uint32_t subnet_count, uint64_t current_slot,
+                               const uint8_t* domain32, int32_t* status_out, uint32_t* root_id_out, uint8_t* roots32_out, uint32_t* n_roots_out,
+                               uint8_t* contrib_bits_out, uint8_t* contrib_sig96_out, uint8_t* contrib_present_out, uint8_t* agg_bits_out,
+                               uint8_t* agg_sig96_out);
 int b2_latest_messages_update_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_off, const uint8_t* d_bits,
                                   uint32_t bits_stride, const uint64_t* d_target_epoch, const uint32_t* d_block_idx,
                                   const uint8_t* d_accept, uint32_t n_agg, void* stream);

@@ -119,6 +119,11 @@ SIGNATURES = {
                                           c_uint64] + [c_void_p] * 8),
     "b2_block_attestations": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p,
                                       c_uint32, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p, c_uint32, c_uint32, c_uint32, c_uint64, c_uint64] + [c_void_p] * 7),
+    # ctx, wire, wire_len, woff, n, subnet, position_validator, committee_size, subnet_count, current_slot, domain32, nine outputs[, stream]
+    "b2_sync_committee_messages_dev": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_uint32, c_uint64,
+                                               c_void_p] + [c_void_p] * 10),
+    "b2_sync_committee_messages": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_uint32, c_uint64,
+                                           c_void_p] + [c_void_p] * 9),
     "b2_vote_weights_dev": (c_int, [c_void_p, c_void_p, c_void_p]),
     "b2_vote_weights_range_dev": (c_int, [c_void_p, c_uint64, c_uint64, c_void_p, c_void_p]),
     "b2_guard_flags": (c_int, [c_void_p, c_void_p]),

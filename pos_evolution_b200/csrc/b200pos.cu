@@ -24,6 +24,7 @@
 #include "intake.cuh"
 #include "aggintake.cuh"
 #include "blockatt.cuh"
+#include "syncmsg.cuh"
 
 using namespace b2;
 
@@ -138,6 +139,13 @@ struct ba_scratch {
     dbuf blk_of, cur, fav_ok, accept, num1, bits, sig96, data128, dom32, msg32, members, item_off;
 };
 
+// sync committee messages (syncmsg.cuh): per position, per item, per hash-table slot, per (root, subnet) segment; the decompressed item
+// signatures, the gathered ones and the segment sums
+struct scm_scratch {
+    dbuf keys, canon, first, pitem, proot, signer, pair_off, msg, sig, ok, slot_of, rtab, rmin, rid, seg_off, agg_off, gsrc;
+    dbuf aff, st, gaff, gst, sumjac, seg_status;
+};
+
 struct vslot {
     dbuf haff, hflag, pkjac, pkst, saff, sflag, f, sumjac;
     dbuf g2aff, g2st;                                      // the slot's own decompressed signatures (pipelined epochs)
@@ -223,6 +231,7 @@ struct b2_ctx {
     intake_scratch in;
     api_scratch api;
     ba_scratch ba;
+    scm_scratch scm;
 };
 
 struct nvtx_scope {
@@ -1736,6 +1745,165 @@ int b2_block_attestations(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, c
     if ((rc = b2_block_attestations_dev(ctx, dwire, wire_len, dwoff, n_att, dboff, dbslot, n_blocks, dmem, doff, n_committees, n_sig, cps_prev, cps_cur, droots,
                                         justified80, domains64, slots_per_epoch, min_inclusion_delay, bits_stride, effective_balance_increment,
                                         base_reward_per_increment, dst, dmask, dnum, dbst, dbfirst, dbrew, dnapp, ctx->s_main)))
+        return rc;
+    return st.finish();
+}
+
+// ------------------------------------------------------------------------------------------ sync committee messages (syncmsg.cuh)
+// SyncCommitteeMessage (pos-evolution.md:548-557) through the sync_committee_{subnet_id} checks of the upstream Altair p2p spec, and the
+// accepted ones into the SyncCommitteeContributions and SyncAggregates of process_sync_committee_contributions (upstream Altair validator
+// spec).  The signature check shares the AggregateVerify buffers with b2_aggregate_verify[_dev] and the intakes: one stream for all of them.
+int b2_sync_committee_messages_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n, const uint32_t* d_subnet,
+                                   const uint32_t* d_position_validator, uint32_t committee_size, uint32_t subnet_count, uint64_t current_slot,
+                                   const uint8_t* domain32, int32_t* d_status_out, uint32_t* d_root_id_out, uint8_t* d_roots32_out,
+                                   uint32_t* d_n_roots_out, uint8_t* d_contrib_bits_out, uint8_t* d_contrib_sig96_out, uint8_t* d_contrib_present_out,
+                                   uint8_t* d_agg_bits_out, uint8_t* d_agg_sig96_out, void* stream) {
+    B2_NVTX;
+    REQUIRE(ctx && d_wire && d_woff && d_subnet && d_position_validator && domain32 && d_status_out && d_root_id_out && d_roots32_out && d_n_roots_out &&
+                d_contrib_bits_out && d_contrib_sig96_out && d_contrib_present_out && d_agg_bits_out && d_agg_sig96_out && n > 0 && n < (1u << 24) &&
+                committee_size > 0 && subnet_count > 0 && (uint64_t)n * (subnet_count + 1) < (1ull << 31),
+            "sync_committee_messages_dev: bad arguments");
+    REQUIRE(committee_size % subnet_count == 0, "sync_committee_messages: committee_size must be a multiple of subnet_count");
+    REQUIRE(committee_size <= B2_SYNC_MAX_SIZE, "sync_committee_messages: committee_size above the kernels' limit (1024)");
+    REQUIRE(ctx->n_val > 0, "sync_committee_messages: registry not loaded");
+    CK(cudaSetDevice(ctx->device));
+    scm_scratch& S = ctx->scm;
+    const uint32_t sub = committee_size / subnet_count;
+    const uint64_t nc = (uint64_t)n * subnet_count;
+    uint32_t tab = 1;
+    while (tab < 2 * n) tab <<= 1;
+    const size_t na = (size_t)n * 4, np = (size_t)committee_size * 4;
+    int rc;
+    if ((rc = ensure(ctx, S.keys, (size_t)committee_size * 8)) || (rc = ensure(ctx, S.canon, na)) || (rc = ensure(ctx, S.first, np)) ||
+        (rc = ensure(ctx, S.pitem, np)) || (rc = ensure(ctx, S.proot, np)) || (rc = ensure(ctx, S.signer, na)) || (rc = ensure(ctx, S.pair_off, na + 4)) ||
+        (rc = ensure(ctx, S.msg, (size_t)n * 32)) || (rc = ensure(ctx, S.sig, (size_t)n * 96)) || (rc = ensure(ctx, S.ok, n)) ||
+        (rc = ensure(ctx, S.slot_of, na)) || (rc = ensure(ctx, S.rtab, (size_t)tab * 4)) || (rc = ensure(ctx, S.rmin, (size_t)tab * 4)) ||
+        (rc = ensure(ctx, S.rid, na)) || (rc = ensure(ctx, S.seg_off, (nc + 1) * 4)) || (rc = ensure(ctx, S.agg_off, na + 4)) ||
+        (rc = ensure(ctx, S.gsrc, np)) || (rc = ensure(ctx, S.aff, (size_t)n * 192 + 16)) || (rc = ensure(ctx, S.st, n + 16)) ||
+        (rc = ensure(ctx, S.gaff, (size_t)committee_size * 192 + 16)) || (rc = ensure(ctx, S.gst, committee_size + 16)) ||
+        (rc = ensure(ctx, S.sumjac, (nc + n) * 288)) || (rc = ensure(ctx, S.seg_status, (nc + n) * 4)))
+        return rc;
+    scm_args A = {};
+    A.wire = d_wire;
+    A.wire_len = wire_len;
+    A.woff = d_woff;
+    A.n = n;
+    A.subnet = d_subnet;
+    A.pos_val = d_position_validator;
+    A.size = committee_size;
+    A.subnets = subnet_count;
+    A.sub = sub;
+    A.sb = (sub + 7) / 8;
+    A.ab = (committee_size + 7) / 8;
+    A.current_slot = current_slot;
+    A.n_val = ctx->n_val;
+    memcpy(A.dom.b, domain32, 32);
+    A.keys = S.keys;
+    A.canon = S.canon;
+    A.first = S.first;
+    A.pitem = S.pitem;
+    A.proot = S.proot;
+    A.signer = S.signer;
+    A.pair_off = S.pair_off;
+    A.msg = S.msg;
+    A.sig = S.sig;
+    A.ok = S.ok;
+    A.slot_of = S.slot_of;
+    A.rtab = S.rtab;
+    A.rmin = S.rmin;
+    A.rid = S.rid;
+    A.rtab_mask = tab - 1;
+    A.seg_off = S.seg_off;
+    A.agg_off = S.agg_off;
+    A.gsrc = S.gsrc;
+    A.status = d_status_out;
+    A.root_id = d_root_id_out;
+    A.n_roots = d_n_roots_out;
+    A.roots32 = d_roots32_out;
+    A.cbits = d_contrib_bits_out;
+    A.cpresent = d_contrib_present_out;
+    A.abits = d_agg_bits_out;
+    A.guard = ctx->d_guard;
+    cudaStream_t s = (cudaStream_t)stream;
+    CK(cudaMemsetAsync(S.first, 0xff, np, s));
+    CK(cudaMemsetAsync(S.rtab, 0xff, (size_t)tab * 4, s));
+    CK(cudaMemsetAsync(S.rmin, 0xff, (size_t)tab * 4, s));
+    k_scm_index<<<1, 1024, 0, s>>>(A);
+    CKL(ctx);
+    k_scm_parse<<<blocks_for(n, 128), 128, 0, s>>>(A);
+    CKL(ctx);
+    if ((rc = aggregate_verify_enqueue(ctx, S.signer, nullptr, S.msg, S.pair_off, n, S.sig, n, S.ok, s))) return rc;
+    k_scm_first<<<blocks_for(n, 128), 128, 0, s>>>(A);
+    CKL(ctx);
+    k_scm_accept<<<blocks_for(n, 128), 128, 0, s>>>(A);
+    CKL(ctx);
+    k_scm_number<<<1, 1024, 0, s>>>(A);
+    CKL(ctx);
+    k_scm_positions<<<blocks_for(committee_size, 128), 128, 0, s>>>(A);
+    CKL(ctx);
+    k_scm_rows<<<blocks_for(nc + n, 128), 128, 0, s>>>(A);
+    CKL(ctx);
+    k_intake_scan<<<1, 1024, 0, s>>>(S.seg_off, (uint32_t)nc, nullptr);      // seg_off[nc] = the set positions of every root
+    CKL(ctx);
+    k_scm_gather<<<blocks_for(std::max<uint64_t>(committee_size, (uint64_t)n + 1), 128), 128, 0, s>>>(A);
+    CKL(ctx);
+    // bls.Aggregate of each contribution's and each root's signatures: the item signatures decompressed once (an item that was not
+    // accepted holds zero bytes and is never gathered), gathered per set position, one segment per (root, subnet) and one per root
+    k_g2_decompress<<<blocks_for(n, ctx->dec_block), ctx->dec_block, 0, s>>>(S.sig, n, S.aff, S.st);
+    CKL(ctx);
+    k_pack_gather<<<blocks_for(committee_size, 128), 128, 0, s>>>(S.aff, S.st, S.gsrc, (const uint32_t*)S.seg_off + nc, S.gaff, S.gst);
+    CKL(ctx);
+    uint32_t* sumjac = S.sumjac;
+    int32_t* segst = S.seg_status;
+    k_g2_segment_sum<<<(unsigned)nc, 32, 0, s>>>(S.gaff, S.gst, S.seg_off, (uint32_t)nc, sumjac, segst, committee_size, ctx->d_guard);
+    CKL(ctx);
+    k_g2_segment_sum<<<n, 32, 0, s>>>(S.gaff, S.gst, S.agg_off, n, sumjac + 72 * nc, segst + nc, committee_size, ctx->d_guard);
+    CKL(ctx);
+    k_g2_finish<<<blocks_for(nc, 32), 32, 0, s>>>(sumjac, segst, (uint32_t)nc, d_contrib_sig96_out, nullptr, nullptr);
+    CKL(ctx);
+    k_g2_finish<<<blocks_for(n, 32), 32, 0, s>>>(sumjac + 72 * nc, segst + nc, n, d_agg_sig96_out, nullptr, nullptr);
+    CKL(ctx);
+    return B2_OK;
+}
+
+int b2_sync_committee_messages(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n, const uint32_t* subnet,
+                               const uint32_t* position_validator, uint32_t committee_size, uint32_t subnet_count, uint64_t current_slot,
+                               const uint8_t* domain32, int32_t* status_out, uint32_t* root_id_out, uint8_t* roots32_out, uint32_t* n_roots_out,
+                               uint8_t* contrib_bits_out, uint8_t* contrib_sig96_out, uint8_t* contrib_present_out, uint8_t* agg_bits_out,
+                               uint8_t* agg_sig96_out) {
+    B2_NVTX;
+    REQUIRE(ctx && wire && woff && subnet && position_validator && domain32 && status_out && root_id_out && roots32_out && n_roots_out &&
+                contrib_bits_out && contrib_sig96_out && contrib_present_out && agg_bits_out && agg_sig96_out && n > 0 && n < (1u << 24) &&
+                committee_size > 0 && subnet_count > 0 && (uint64_t)n * (subnet_count + 1) < (1ull << 31),
+            "sync_committee_messages: bad arguments");
+    REQUIRE(committee_size % subnet_count == 0, "sync_committee_messages: committee_size must be a multiple of subnet_count");
+    REQUIRE(committee_size <= B2_SYNC_MAX_SIZE, "sync_committee_messages: committee_size above the kernels' limit (1024)");
+    REQUIRE(ctx->n_val > 0, "sync_committee_messages: registry not loaded");
+    int rc;
+    if ((rc = check_offsets(ctx, woff, n, "sync_committee_messages: woff"))) return rc;
+    REQUIRE(woff[n] <= wire_len, "sync_committee_messages: woff ends past the wire");
+    for (uint32_t p = 0; p < committee_size; p++)
+        REQUIRE(position_validator[p] < ctx->n_val, "sync_committee_messages: a position_validator entry is outside the registry");
+    CK(cudaSetDevice(ctx->device));
+    const uint32_t sub = committee_size / subnet_count;
+    const size_t nc = (size_t)n * subnet_count;
+    staging st(ctx);
+    const uint8_t* dwire = st.in(wire, wire_len, 16);
+    const uint32_t* dwoff = st.in(woff, (size_t)n + 1);
+    const uint32_t* dsub = st.in(subnet, n);
+    const uint32_t* dpv = st.in(position_validator, committee_size);
+    int32_t* dst = st.out(status_out, n);
+    uint32_t* drid = st.out(root_id_out, n);
+    uint8_t* droots = st.out(roots32_out, (size_t)n * 32);
+    uint32_t* dnr = st.out(n_roots_out, 1);
+    uint8_t* dcb = st.out(contrib_bits_out, nc * ((sub + 7) / 8));
+    uint8_t* dcs = st.out(contrib_sig96_out, nc * 96);
+    uint8_t* dcp = st.out(contrib_present_out, nc);
+    uint8_t* dab = st.out(agg_bits_out, (size_t)n * ((committee_size + 7) / 8));
+    uint8_t* das = st.out(agg_sig96_out, (size_t)n * 96);
+    if (st.rc) return st.rc;
+    if ((rc = b2_sync_committee_messages_dev(ctx, dwire, wire_len, dwoff, n, dsub, dpv, committee_size, subnet_count, current_slot, domain32, dst, drid,
+                                             droots, dnr, dcb, dcs, dcp, dab, das, ctx->s_main)))
         return rc;
     return st.finish();
 }

@@ -26,6 +26,10 @@ AggregateIntakeResult = namedtuple("AggregateIntakeResult", "status committee da
 # (0 applied, 1 invalid, 2 after an invalid block), the list index of its first failing attestation (0xFFFFFFFF: none) and proposer reward;
 # the number of blocks applied
 BlockAttestationsResult = namedtuple("BlockAttestationsResult", "status flag_mask numerator block_status block_first block_reward n_applied")
+# Engine.sync_committee_messages: per message its status (0-6) and root id (0xFFFFFFFF: not accepted); the n_roots distinct roots; per (root,
+# subnet) the contribution's bit row, signature and present byte (uint8[n_roots, subnet_count, ...]); per root the SyncAggregate's bit row and
+# signature
+SyncMessagesResult = namedtuple("SyncMessagesResult", "status root_id roots contrib_bits contrib_sigs contrib_present agg_bits agg_sigs")
 
 
 def _c(a, dtype):
@@ -349,6 +353,29 @@ class Engine:
                                                 int(min_inclusion_delay), int(bits_stride), int(increment), int(base_reward_per_increment),
                                                 *[_p(x) for x in r]))
         return r._replace(n_applied=int(r.n_applied[0]))
+
+    def sync_committee_messages(self, wire: bytes, woff, subnet, position_validator, subnet_count: int, current_slot: int,
+                                domain32: bytes) -> SyncMessagesResult:
+        """One slot of SyncCommitteeMessages (144-byte SSZ encodings back to back, woff their offsets; subnet[i] the topic's subnet id)
+        checked and verified against the registry, grouped by root and aggregated (include/b200pos.h, b2_sync_committee_messages:
+        statuses 0-6).  position_validator: the registry index of each sync committee position.  Per-root outputs are trimmed to n_roots."""
+        woff, sub, pv = _c(woff, np.uint32), _c(subnet, np.uint32), _c(position_validator, np.uint32)
+        n, size, count = woff.shape[0] - 1, pv.shape[0], int(subnet_count)
+        assert sub.shape == (n,) and count > 0
+        w = np.frombuffer(bytes(wire), dtype=np.uint8) if len(wire) else np.zeros(1, dtype=np.uint8)
+        dom = np.frombuffer(bytes(domain32), dtype=np.uint8)
+        assert dom.shape == (32,)
+        sb, ab = (size // count + 7) // 8, (size + 7) // 8
+        r = SyncMessagesResult(np.zeros(n, np.int32), np.zeros(n, np.uint32), np.zeros((n, 32), np.uint8), np.zeros((n, count, sb), np.uint8),
+                               np.zeros((n, count, 96), np.uint8), np.zeros((n, count), np.uint8), np.zeros((n, ab), np.uint8),
+                               np.zeros((n, 96), np.uint8))
+        n_roots = np.zeros(1, np.uint32)
+        self._ck(self.lib.b2_sync_committee_messages(self.h, _p(w), len(wire), _p(woff), n, _p(sub), _p(pv), size, count, int(current_slot),
+                                                     _p(dom), _p(r.status), _p(r.root_id), _p(r.roots), _p(n_roots), _p(r.contrib_bits),
+                                                     _p(r.contrib_sigs), _p(r.contrib_present), _p(r.agg_bits), _p(r.agg_sigs)))
+        k = int(n_roots[0])
+        return r._replace(roots=r.roots[:k], contrib_bits=r.contrib_bits[:k], contrib_sigs=r.contrib_sigs[:k], contrib_present=r.contrib_present[:k],
+                          agg_bits=r.agg_bits[:k], agg_sigs=r.agg_sigs[:k])
 
     def signing_roots(self, data128, domains32):
         """compute_signing_root for n attestations: data128 uint8[n,128] (SSZ-serialised AttestationData), domains32 uint8[32] or uint8[n,32]."""
@@ -749,6 +776,38 @@ class Engine:
                                                     int(base_reward_per_increment), d_status.data_ptr(), d_flag_mask.data_ptr(),
                                                     d_numerator.data_ptr(), d_block_status.data_ptr(), d_block_first.data_ptr(),
                                                     d_block_reward.data_ptr(), d_n_applied.data_ptr(), self._stream()))
+
+    def sync_committee_messages_dev(self, d_wire, d_woff, d_subnet, d_position_validator, subnet_count: int, current_slot: int, domain32: bytes,
+                                    out=None, trim: bool = True) -> SyncMessagesResult:
+        """sync_committee_messages on device tensors (n = d_woff.numel() - 1, the wire's length is d_wire.numel(), committee_size =
+        d_position_validator.numel()), enqueued on the current stream.  `out`: (SyncMessagesResult of device tensors shaped as the host
+        form's untrimmed outputs, n_roots tensor of 4 bytes), or None to allocate them here (status and root_id int32: a message that was
+        not accepted has root id -1).  With trim (the default) the call waits for n_roots and returns the result with the per-root outputs
+        trimmed to it; with trim=False it stays asynchronous and returns the pair `out` takes."""
+        import torch
+        dom = np.frombuffer(bytes(domain32), dtype=np.uint8)
+        assert dom.shape == (32,)
+        n, size, count = d_woff.numel() - 1, d_position_validator.numel(), int(subnet_count)
+        assert d_subnet.numel() == n and count > 0
+        sb, ab = (size // count + 7) // 8, (size + 7) // 8
+        if out is None:
+            dev, u8 = d_woff.device, torch.uint8
+            out = SyncMessagesResult(torch.empty(n, dtype=torch.int32, device=dev), torch.empty(n, dtype=torch.int32, device=dev),
+                                     torch.empty((n, 32), dtype=u8, device=dev), torch.empty((n, count, sb), dtype=u8, device=dev),
+                                     torch.empty((n, count, 96), dtype=u8, device=dev), torch.empty((n, count), dtype=u8, device=dev),
+                                     torch.empty((n, ab), dtype=u8, device=dev), torch.empty((n, 96), dtype=u8, device=dev))
+            n_roots = torch.empty(1, dtype=torch.int32, device=dev)
+        else:
+            out, n_roots = out
+        self._ck(self.lib.b2_sync_committee_messages_dev(self.h, d_wire.data_ptr(), d_wire.numel(), d_woff.data_ptr(), n, d_subnet.data_ptr(),
+                                                         d_position_validator.data_ptr(), size, count, int(current_slot), _p(dom),
+                                                         *[x.data_ptr() for x in out[:3]], n_roots.data_ptr(),
+                                                         *[x.data_ptr() for x in out[3:]], self._stream()))
+        if not trim:
+            return out, n_roots
+        k = int(n_roots.item())
+        return out._replace(roots=out.roots[:k], contrib_bits=out.contrib_bits[:k], contrib_sigs=out.contrib_sigs[:k],
+                            contrib_present=out.contrib_present[:k], agg_bits=out.agg_bits[:k], agg_sigs=out.agg_sigs[:k])
 
     def votes_empty_dev(self, d_bits, d_agg_sig, d_agg_status=None):
         """b2_votes_empty_dev on the current stream: every vote whose grouped bit row d_bits (uint8[n_votes, bits_stride]) has no attester

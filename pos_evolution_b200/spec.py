@@ -21,6 +21,7 @@ from .engine import Engine
 FAR_FUTURE_EPOCH = 2**64 - 1
 GENESIS_EPOCH = 0
 ZERO32 = bytes(32)
+G2_POINT_AT_INFINITY = bytes([0xC0]) + bytes(95)
 DOMAIN_BEACON_PROPOSER = bytes.fromhex("00000000")
 DOMAIN_BEACON_ATTESTER = bytes.fromhex("01000000")
 DOMAIN_SELECTION_PROOF = bytes.fromhex("05000000")             # upstream phase 0 validator spec
@@ -59,6 +60,7 @@ class Preset:
     EPOCHS_PER_ETH1_VOTING_PERIOD: int = 64
     TARGET_AGGREGATORS_PER_COMMITTEE: int = 16    # upstream phase 0 validator spec (is_aggregator)
     ATTESTATION_PROPAGATION_SLOT_RANGE: int = 32  # upstream phase 0 p2p spec (beacon_aggregate_and_proof)
+    SYNC_COMMITTEE_SUBNET_COUNT: int = 4          # upstream Altair validator spec (sync_committee_{subnet_id})
 
 
 MAINNET = Preset("mainnet", 32, 64, 128, 90, 65536, 8192)
@@ -164,6 +166,35 @@ class SyncCommittee:                   # BeaconState.current_sync_committee / ne
 class SyncAggregate:                   # Altair BeaconBlockBody.sync_aggregate
     sync_committee_bits: List[bool]    # Bitvector[SYNC_COMMITTEE_SIZE]
     sync_committee_signature: bytes
+
+
+@dataclass
+class SyncCommitteeMessage:            # pos-evolution.md:548-557; the sync_committee_{subnet_id} gossip message
+    slot: int
+    beacon_block_root: bytes
+    validator_index: int
+    signature: bytes
+
+
+@dataclass
+class SyncCommitteeContribution:       # upstream Altair validator spec
+    slot: int
+    beacon_block_root: bytes
+    subcommittee_index: int
+    aggregation_bits: List[bool]       # Bitvector[SYNC_COMMITTEE_SIZE // SYNC_COMMITTEE_SUBNET_COUNT]
+    signature: bytes
+
+
+class SyncAggregates(dict):
+    """{beacon_block_root: SyncAggregate} of Spec.validate_sync_committee_messages; a root nobody signed gives the empty aggregate (no bits,
+    the G2 infinity signature), which eth_fast_aggregate_verify accepts"""
+
+    def __init__(self, size, *args):
+        super().__init__(*args)
+        self.size = size
+
+    def __missing__(self, root):
+        return SyncAggregate([False] * self.size, G2_POINT_AT_INFINITY)
 
 
 @dataclass
@@ -302,6 +333,11 @@ def serialize_signed_aggregate_and_proof(s: SignedAggregateAndProof) -> bytes:
     return (100).to_bytes(4, "little") + bytes(s.signature) + serialize_aggregate_and_proof(s.message)
 
 
+def serialize_sync_committee_message(m: SyncCommitteeMessage) -> bytes:
+    """SSZ (:548-557): [slot u64][beacon_block_root][validator_index u64][signature], 144 bytes"""
+    return int(m.slot).to_bytes(8, "little") + bytes(m.beacon_block_root) + int(m.validator_index).to_bytes(8, "little") + bytes(m.signature)
+
+
 def serialize_validators(validators) -> np.ndarray:
     """SSZ serialisation of each Validator (:36-45) -> uint8[n, 121]: pubkey 48, withdrawal_credentials 32, effective_balance u64,
     slashed 1, activation_eligibility_epoch, activation_epoch, exit_epoch, withdrawable_epoch u64, little-endian.  The record format of
@@ -391,6 +427,7 @@ class Spec:
         self.registry_valid = None         # KeyValidate verdict per validator of the registry on the device (uint8[n])
         self._sync_key = None              # (length, hash of the pubkey bytes) of the sync committee on the device
         self.sync_committee_valid = None   # KeyValidate verdict per position of that committee (uint8[SYNC_COMMITTEE_SIZE])
+        self._sync_positions = None        # (registry and committee key, first registry index per position): _position_validators
         self._ssz_records = None           # serialised validators of the device tree of hash_tree_root_state (uint8[n, 121])
         self._ssz_load_id = None           # engine.ssz_loads after this Spec's last load: another load replaced the tree when it differs
         self._slasher = None               # slasher_start: size and current epoch of the device history, accepted attestations by target epoch
@@ -975,6 +1012,62 @@ class Spec:
                 state.balances[proposer] += proposer_reward
             else:
                 state.balances[participant_index] = max(0, state.balances[participant_index] - participant_reward)
+
+    def sync_committee_for_messages(self, state):
+        """The committee compute_subnets_for_sync_committee (upstream Altair validator spec) reads: state.current_sync_committee, or
+        state.next_sync_committee when state.slot + 1 starts the next sync committee period."""
+        next_slot_epoch = self.compute_epoch_at_slot(state.slot + 1)
+        if self.compute_sync_committee_period(self.get_current_epoch(state)) == self.compute_sync_committee_period(next_slot_epoch):
+            return state.current_sync_committee
+        return state.next_sync_committee
+
+    def _position_validators(self, state, committee):
+        """uint32[len(committee.pubkeys)]: the first registry index of each committee key (all_pubkeys.index(pubkey), as
+        process_sync_aggregate maps positions), cached per (registry, committee) content"""
+        pubkeys = [bytes(pk) for pk in committee.pubkeys]
+        key = (self._registry_key, len(pubkeys), hashlib.blake2b(b"".join(pubkeys), digest_size=16).digest())
+        if self._sync_positions is not None and self._sync_positions[0] == key:
+            return self._sync_positions[1]
+        first = {}
+        for i, v in enumerate(state.validators):
+            first.setdefault(bytes(v.pubkey), i)
+        if any(pk not in first for pk in pubkeys):
+            raise ValueError("sync committee pubkey is not in the registry")
+        pv = np.array([first[pk] for pk in pubkeys], dtype=np.uint32)
+        self._sync_positions = (key, pv)
+        return pv
+
+    def validate_sync_committee_messages(self, state, items, current_slot=None):
+        """The sync_committee_{subnet_id} gossip checks (upstream Altair p2p spec) of one slot's list of (subnet_id, SyncCommitteeMessage) on
+        the GPU (b2_sync_committee_messages), and the contributions and SyncAggregates process_sync_committee_contributions (upstream Altair
+        validator spec) builds from the accepted ones.  current_slot defaults to state.slot; the committee is sync_committee_for_messages';
+        the domain is get_domain(DOMAIN_SYNC_COMMITTEE) of current_slot's epoch, the epoch of every message that can be accepted.  Subnet
+        membership compares registry indices, each committee key standing for its first registry index.  Returns (status per item, 0-6 of
+        include/b200pos.h; the present SyncCommitteeContributions in (root, subnet) order, roots by first accepted message; a SyncAggregates
+        {root: SyncAggregate}).  Each call starts with an empty seen-cache."""
+        current_slot = state.slot if current_slot is None else int(current_slot)
+        self.sync_registry(state)
+        committee = self.sync_committee_for_messages(state)
+        size, count = len(committee.pubkeys), self.p.SYNC_COMMITTEE_SUBNET_COUNT
+        aggregates = SyncAggregates(size)
+        if not items:
+            return [], [], aggregates
+        pv = self._position_validators(state, committee)
+        wires = [serialize_sync_committee_message(m) for _, m in items]
+        woff = np.cumsum([0] + [len(w) for w in wires]).astype(np.uint32)
+        subnet = np.array([int(sid) if 0 <= int(sid) < 2**32 else 2**32 - 1 for sid, _ in items], dtype=np.uint32)
+        domain = self.get_domain(state, DOMAIN_SYNC_COMMITTEE, self.compute_epoch_at_slot(current_slot))
+        r = self.engine.sync_committee_messages(b"".join(wires), woff, subnet, pv, count, current_slot, domain)
+        sub = size // count
+        contributions = []
+        for k in range(r.roots.shape[0]):
+            root = r.roots[k].tobytes()
+            for sc in range(count):
+                if r.contrib_present[k, sc]:
+                    bits = np.unpackbits(r.contrib_bits[k, sc], bitorder="little")[:sub]
+                    contributions.append(SyncCommitteeContribution(current_slot, root, sc, [bool(b) for b in bits], r.contrib_sigs[k, sc].tobytes()))
+            aggregates[root] = SyncAggregate([bool(b) for b in np.unpackbits(r.agg_bits[k], bitorder="little")[:size]], r.agg_sigs[k].tobytes())
+        return [int(x) for x in r.status], contributions, aggregates
 
     # ------------------------------------------------------------------ fork choice
     def update_latest_messages(self, store, attesting_indices, attestation):   # :1435-1441
