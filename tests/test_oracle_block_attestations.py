@@ -14,7 +14,6 @@ import scenarios
 from oracle import spec as S
 
 SPE = S.MINIMAL.SLOTS_PER_EPOCH          # 8; integer_squareroot = 2
-H = S.MINIMAL.SLOTS_PER_HISTORICAL_ROOT
 
 
 def _h(b):
@@ -45,21 +44,23 @@ def make_state(slot, late=0):
 
 
 class Run:
-    """A run of blocks on a state: blocks[k] = (slot, root); roots(s) is the chain's block root at slot s as the last block sees it"""
+    """A run of blocks on a state: blocks[k] = (slot, root); roots(s) is the chain's block root at slot s as the last block sees it.  The
+    epoch length and the block-root ring come from the spec's preset."""
 
     def __init__(self, spec, state, slots):
         self.spec, self.state, self.slots = spec, state, list(slots)
+        self.spe, self.H = spec.p.SLOTS_PER_EPOCH, spec.p.SLOTS_PER_HISTORICAL_ROOT
         self.roots = [_h(b"block" + s.to_bytes(8, "little")) for s in self.slots]
         self.atts = [[] for _ in self.slots]
 
     def root(self, s):
         if s < self.slots[0]:
-            return bytes(self.state.block_roots[s % H]) if s >= 0 else bytes(32)
+            return bytes(self.state.block_roots[s % self.H]) if s >= 0 else bytes(32)
         return [r for r, b in zip(self.roots, self.slots) if b <= s][-1]
 
     def add(self, k, slot, index, bits=None, head=None, target_root=None, target_epoch=None, source=None, bad_sig=False):
         """an attestation of (slot, index) in block k, right in every field unless one is given"""
-        sp, st = self.spec, self.state
+        sp, st, SPE = self.spec, self.state, self.spe
         e = slot // SPE
         tepoch = e if target_epoch is None else target_epoch
         cur = self.slots[0] // SPE
@@ -71,13 +72,13 @@ class Run:
                                  S.Checkpoint(tepoch, self.root(tepoch * SPE) if target_root is None else target_root))
         signers = sorted(set(v for v, b in zip(committee, bits) if b))
         msg = sp.compute_signing_root(data, sp.get_domain(st, S.DOMAIN_BEACON_ATTESTER, tepoch))
-        sig = fake_sig([PKS[v] for v in signers], msg)
+        sig = fake_sig([st.validators[v].pubkey for v in signers], msg)
         if bad_sig:
             sig = _h(sig) * 3
         self.atts[k].append(S.Attestation(bits, data, sig))
 
     def inputs(self):
-        sp, st = self.spec, self.state
+        sp, st, SPE = self.spec, self.state, self.spe
         e = self.slots[0] // SPE
         members, off, cps = [], [0], []
         for E in ([e - 1] if e > 0 else []) + [e]:
@@ -96,8 +97,8 @@ class Run:
         domains = sp.get_domain(st, S.DOMAIN_BEACON_ATTESTER, max(e, 1) - 1) + sp.get_domain(st, S.DOMAIN_BEACON_ATTESTER, e)
         return dict(wire=wire, woff=woff, block_off=block_off, block_slot=self.slots, members=np.array(members, np.uint32),
                     off=np.array(off, np.uint32), cps_prev=cps_prev, cps_cur=cps_cur, chain_roots=roots, justified80=justified,
-                    domains64=domains, spe=SPE, min_delay=S.MINIMAL.MIN_ATTESTATION_INCLUSION_DELAY, bits_stride=stride,
-                    eff=[v.effective_balance for v in st.validators], increment=S.MINIMAL.EFFECTIVE_BALANCE_INCREMENT,
+                    domains64=domains, spe=SPE, min_delay=sp.p.MIN_ATTESTATION_INCLUSION_DELAY, bits_stride=stride,
+                    eff=[v.effective_balance for v in st.validators], increment=sp.p.EFFECTIVE_BALANCE_INCREMENT,
                     per_increment=sp.get_base_reward_per_increment(st), part_cur=st.current_epoch_participation,
                     part_prev=st.previous_epoch_participation)
 
@@ -108,7 +109,8 @@ class Run:
                                                      d.target.root), a.signature)
 
     def oracle(self):
-        verify = lambda idx, root, sig: bytes(sig) == fake_sig([PKS[v] for v in idx], root)      # noqa: E731
+        keys = [v.pubkey for v in self.state.validators]
+        verify = lambda idx, root, sig: bytes(sig) == fake_sig([keys[v] for v in idx], root)      # noqa: E731
         return O.run(verify=verify, **self.inputs())
 
     def proposers(self):
@@ -125,7 +127,7 @@ class Run:
         for k, s in enumerate(self.slots):
             if k:
                 for t in range(self.slots[k - 1], s):
-                    st.block_roots[t % H] = self.roots[k - 1]
+                    st.block_roots[t % self.H] = self.roots[k - 1]
             st.slot = s
             before = copy.deepcopy(st)
             for j, a in enumerate(self.atts[k]):
