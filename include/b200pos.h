@@ -17,6 +17,8 @@
  *     host<->device copies.  *_dev functions take DEVICE pointers plus a cudaStream_t (as void*)
  *     and only enqueue work (used by bench.py and by the multi-GPU path, where the u64 vote
  *     weights are all-reduced by NCCL between b2_vote_weights_dev and b2_head_from_votes_dev).
+ *     Both forms of an entry point reject the same arguments with the same b2_last_error text;
+ *     the host form also checks the contents of its host arrays (offsets, indices, epochs).
  *   - a b2_ctx is bound to one GPU and is not thread-safe (pyspec is single-threaded).
  *   - there is no CPU fallback: b2_init fails with B2_ENODEVICE when no sm_90 (H100) GPU is present.
  */

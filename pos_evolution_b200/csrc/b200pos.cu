@@ -332,11 +332,37 @@ struct staging {
     }
 };
 
-// host check of the offsets off[0..n]: they start at 0 and never decrease
-static int check_offsets(b2_ctx* ctx, const uint32_t* off, uint32_t n, const char* what) {
-    if (off[0] == 0 && std::is_sorted(off, off + n + 1)) return B2_OK;
-    snprintf(ctx->err, sizeof(ctx->err), "%s must start at 0 and never decrease", what);
+// Argument checks.  An entry point with a host and a device form has one check_X, called by both, for every condition on the arguments
+// both receive and on the tables it needs; the host form adds only the checks that read its host arrays (check_offsets .. check_batch).
+// `what` names the entry point in the message, which is the same whichever form was called.
+static int reject(b2_ctx* ctx, const char* what, const char* why) {
+    snprintf(ctx->err, sizeof(ctx->err), "%s: %s", what, why);
     return B2_EINVAL;
+}
+// the offsets off[0..n] start at 0 and never decrease
+static int check_offsets(b2_ctx* ctx, const uint32_t* off, uint32_t n, const char* what, const char* name = "off") {
+    if (off[0] == 0 && std::is_sorted(off, off + n + 1)) return B2_OK;
+    snprintf(ctx->err, sizeof(ctx->err), "%s: %s must start at 0 and never decrease", what, name);
+    return B2_EINVAL;
+}
+// a wire batch's item offsets woff[0..n]: check_offsets, and the last item ends within the wire
+static int check_wire(b2_ctx* ctx, const uint32_t* woff, uint32_t n, uint64_t wire_len, const char* what) {
+    if (int rc = check_offsets(ctx, woff, n, what, "woff")) return rc;
+    return woff[n] <= wire_len ? B2_OK : reject(ctx, what, "woff ends past the wire");
+}
+// the member offsets off[0..n] of n committees: check_offsets, and no committee is wider than its 8 * bits_stride bit row
+static int check_committees(b2_ctx* ctx, const uint32_t* off, uint32_t n, uint32_t bits_stride, const char* what) {
+    if (int rc = check_offsets(ctx, off, n, what)) return rc;
+    for (uint32_t c = 0; c < n; c++)
+        if (off[c + 1] - off[c] > 8ull * bits_stride) return reject(ctx, what, "a committee is larger than 8 * bits_stride");
+    return B2_OK;
+}
+// a committee batch: check_committees, and every member addresses one of `limit` validators
+static int check_batch(b2_ctx* ctx, const uint32_t* members, const uint32_t* off, uint32_t bits_stride, uint32_t n_agg, uint64_t limit, const char* what) {
+    if (int rc = check_committees(ctx, off, n_agg, bits_stride, what)) return rc;
+    for (uint32_t i = 0; i < off[n_agg]; i++)
+        if (members[i] >= limit) return reject(ctx, what, "member index outside the registry");
+    return B2_OK;
 }
 #define B2_TEAM_SMEM (B2_TEAMS_PER_WARP * sizeof(team_ws))
 static inline unsigned blocks_for(uint64_t n, unsigned t) { return (unsigned)((n + t - 1) / t); }
@@ -537,16 +563,6 @@ int b2_registry_update_balances(b2_ctx* ctx, const uint64_t* eff, const uint8_t*
     return B2_OK;
 }
 
-// host-side validation of a committee batch (indices must address the registry)
-static int check_batch(b2_ctx* ctx, const uint32_t* members, const uint32_t* off, uint32_t bits_stride, uint32_t n_agg, uint64_t limit) {
-    int rc;
-    if ((rc = check_offsets(ctx, off, n_agg, "off"))) return rc;
-    for (uint32_t a = 0; a < n_agg; a++) REQUIRE((uint64_t)(off[a + 1] - off[a]) <= (uint64_t)bits_stride * 8, "committee larger than bits_stride*8");
-    const uint32_t total = off[n_agg];
-    for (uint32_t i = 0; i < total; i++) REQUIRE(members[i] < limit, "member index outside the registry");
-    return B2_OK;
-}
-
 // K2 launch: one warp per aggregate through the TMA-staged gather (wpb warps = aggregates per block), or the LDG form with
 // `ldg_block` threads per aggregate
 static int launch_k2(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_off, const uint8_t* d_bits, uint32_t bits_stride, uint32_t n_agg,
@@ -575,7 +591,7 @@ int b2_g1_aggregate(b2_ctx* ctx, const uint32_t* members, const uint32_t* off, c
     REQUIRE(ctx && members && off && bits && out48 && status && n_agg > 0 && bits_stride > 0, "g1_aggregate: bad arguments");
     REQUIRE(ctx->n_val > 0, "g1_aggregate: registry not loaded");
     int rc;
-    if ((rc = check_batch(ctx, members, off, bits_stride, n_agg, ctx->n_val))) return rc;
+    if ((rc = check_batch(ctx, members, off, bits_stride, n_agg, ctx->n_val, "g1_aggregate"))) return rc;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->s_main;
     staging st(ctx);
@@ -646,23 +662,28 @@ static int aggregate_finish(b2_ctx* ctx, vslot& V, uint32_t n_seg, uint8_t* d_ou
     return B2_OK;
 }
 
+static int check_aggregate(b2_ctx* ctx, const uint8_t* sig96, const uint32_t* seg_off, uint32_t n_seg, uint64_t n_sig, const uint8_t* out96,
+                           const int32_t* seg_status) {
+    REQUIRE(ctx && seg_off && out96 && seg_status && n_seg > 0, "aggregate: bad arguments");
+    return n_sig == 0 || sig96 ? B2_OK : reject(ctx, "aggregate", "null signatures");
+}
 int b2_aggregate_dev(b2_ctx* ctx, const uint8_t* d_sig96, const uint32_t* d_seg_off, uint32_t n_seg, uint64_t n_sig, uint8_t* d_out96,
                      int32_t* d_seg_status, void* stream) {
     B2_NVTX;
-    REQUIRE(ctx && d_seg_off && d_out96 && d_seg_status && n_seg > 0 && (n_sig == 0 || d_sig96), "aggregate_dev: bad arguments");
-    CK(cudaSetDevice(ctx->device));
     int rc;
+    if ((rc = check_aggregate(ctx, d_sig96, d_seg_off, n_seg, n_sig, d_out96, d_seg_status))) return rc;
+    CK(cudaSetDevice(ctx->device));
     if ((rc = aggregate_front(ctx, ctx->slot[0], d_sig96, d_seg_off, n_seg, n_sig, d_seg_status, (cudaStream_t)stream))) return rc;
     return aggregate_finish(ctx, ctx->slot[0], n_seg, d_out96, d_seg_status, false, (cudaStream_t)stream);
 }
 
 int b2_aggregate(b2_ctx* ctx, const uint8_t* sig96, const uint32_t* seg_off, uint32_t n_seg, uint8_t* out96, int32_t* seg_status) {
     B2_NVTX;
-    REQUIRE(ctx && seg_off && out96 && seg_status && n_seg > 0, "aggregate: bad arguments");
+    REQUIRE(ctx && seg_off, "aggregate: bad arguments");
     int rc;
-    if ((rc = check_offsets(ctx, seg_off, n_seg, "aggregate: seg_off"))) return rc;
+    if ((rc = check_offsets(ctx, seg_off, n_seg, "aggregate", "seg_off"))) return rc;
     const uint64_t n_sig = seg_off[n_seg];
-    REQUIRE(n_sig == 0 || sig96, "aggregate: null signatures");
+    if ((rc = check_aggregate(ctx, sig96, seg_off, n_seg, n_sig, out96, seg_status))) return rc;
     CK(cudaSetDevice(ctx->device));
     staging st(ctx);
     const uint8_t* dsig = st.in(sig96, n_sig * 96, 16);
@@ -815,14 +836,18 @@ static int verify_main(b2_ctx* ctx, vslot& V, const uint8_t* d_sig96, uint32_t n
     return launch_final(ctx, V, n_agg, d_ok, team, s);
 }
 
+static int check_fast_aggregate_verify(b2_ctx* ctx, const void* members, const void* off, const void* bits, uint32_t bits_stride, const void* msg32,
+                                       const void* sig96, uint32_t n_agg, const void* ok_out) {
+    REQUIRE(ctx && members && off && bits && msg32 && sig96 && ok_out && n_agg > 0 && bits_stride > 0, "fast_aggregate_verify: bad arguments");
+    return ctx->n_val > 0 ? B2_OK : reject(ctx, "fast_aggregate_verify", "registry not loaded");
+}
 int b2_fast_aggregate_verify_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_off, const uint8_t* d_bits, uint32_t bits_stride,
                                  const uint8_t* d_msg32, const uint8_t* d_sig96, uint32_t n_agg, uint8_t* d_ok_out, void* stream) {
     B2_NVTX;
-    REQUIRE(ctx && d_members && d_off && d_bits && d_msg32 && d_sig96 && d_ok_out && n_agg > 0 && bits_stride > 0, "fast_aggregate_verify_dev: bad arguments");
-    REQUIRE(ctx->n_val > 0, "fast_aggregate_verify: registry not loaded");
+    int rc;
+    if ((rc = check_fast_aggregate_verify(ctx, d_members, d_off, d_bits, bits_stride, d_msg32, d_sig96, n_agg, d_ok_out))) return rc;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
-    int rc;
     pk_source P = {d_members, d_off, d_bits, bits_stride, nullptr, 0};
     if ((rc = verify_fork(ctx, ctx->slot[0], P, d_msg32, n_agg, s))) return rc;
     return verify_main(ctx, ctx->slot[0], d_sig96, n_agg, d_ok_out, s);
@@ -958,10 +983,10 @@ int b2_epoch_wait_dev(b2_ctx* ctx, int slot, void* stream) {
 int b2_fast_aggregate_verify(b2_ctx* ctx, const uint32_t* members, const uint32_t* off, const uint8_t* bits, uint32_t bits_stride,
                              const uint8_t* msg32, const uint8_t* sig96, uint32_t n_agg, uint8_t* ok_out) {
     B2_NVTX;
-    REQUIRE(ctx && members && off && bits && msg32 && sig96 && ok_out && n_agg > 0 && bits_stride > 0, "fast_aggregate_verify: bad arguments");
-    REQUIRE(ctx->n_val > 0, "fast_aggregate_verify: registry not loaded");
     int rc;
-    if ((rc = check_batch(ctx, members, off, bits_stride, n_agg, ctx->n_val))) return rc;
+    if ((rc = check_fast_aggregate_verify(ctx, members, off, bits, bits_stride, msg32, sig96, n_agg, ok_out)) ||
+        (rc = check_batch(ctx, members, off, bits_stride, n_agg, ctx->n_val, "fast_aggregate_verify")))
+        return rc;
     CK(cudaSetDevice(ctx->device));
     staging st(ctx);
     const uint32_t* dm = st.in(members, off[n_agg], 4);
@@ -979,7 +1004,7 @@ int b2_fast_aggregate_verify_pks(b2_ctx* ctx, const uint8_t* pk48, const uint32_
     B2_NVTX;
     REQUIRE(ctx && pk_off && msg32 && sig96 && ok_out && n_agg > 0, "fast_aggregate_verify_pks: bad arguments");
     int rc;
-    if ((rc = check_offsets(ctx, pk_off, n_agg, "pk_off"))) return rc;
+    if ((rc = check_offsets(ctx, pk_off, n_agg, "fast_aggregate_verify_pks", "pk_off"))) return rc;
     const uint64_t n_pk = pk_off[n_agg];
     REQUIRE(n_pk == 0 || pk48, "null pubkeys");
     CK(cudaSetDevice(ctx->device));
@@ -1047,12 +1072,18 @@ static int aggregate_verify_enqueue(b2_ctx* ctx, const uint32_t* d_signer, const
     return B2_OK;
 }
 
+static int check_aggregate_verify(b2_ctx* ctx, const uint32_t* signer, const uint8_t* msg32, const uint32_t* pair_off, uint64_t n_pairs,
+                                  const uint8_t* sig96, uint32_t n_sets, const uint8_t* ok_out) {
+    REQUIRE(ctx && pair_off && sig96 && ok_out && n_sets > 0, "aggregate_verify: bad arguments");
+    REQUIRE(n_pairs == 0 || (signer && msg32), "aggregate_verify: null signers or messages");
+    REQUIRE(n_pairs + n_sets < (1ull << 32), "aggregate_verify: too many pairs");
+    return ctx->n_val > 0 ? B2_OK : reject(ctx, "aggregate_verify", "registry not loaded");
+}
 int b2_aggregate_verify_dev(b2_ctx* ctx, const uint32_t* d_signer, const uint8_t* d_msg32, const uint32_t* d_pair_off, uint64_t n_pairs, const uint8_t* d_sig96,
                             uint32_t n_sets, uint8_t* d_ok_out, void* stream) {
     B2_NVTX;
-    REQUIRE(ctx && d_pair_off && d_sig96 && d_ok_out && n_sets > 0 && (n_pairs == 0 || (d_signer && d_msg32)) && n_pairs + n_sets < (1ull << 32),
-            "aggregate_verify_dev: bad arguments");
-    REQUIRE(ctx->n_val > 0, "aggregate_verify: registry not loaded");
+    int rc;
+    if ((rc = check_aggregate_verify(ctx, d_signer, d_msg32, d_pair_off, n_pairs, d_sig96, n_sets, d_ok_out))) return rc;
     CK(cudaSetDevice(ctx->device));
     return aggregate_verify_enqueue(ctx, d_signer, nullptr, d_msg32, d_pair_off, n_pairs, d_sig96, n_sets, d_ok_out, (cudaStream_t)stream);
 }
@@ -1060,13 +1091,11 @@ int b2_aggregate_verify_dev(b2_ctx* ctx, const uint32_t* d_signer, const uint8_t
 int b2_aggregate_verify(b2_ctx* ctx, const uint32_t* signer, const uint8_t* msg32, const uint32_t* pair_off, const uint8_t* sig96, uint32_t n_sets,
                         uint8_t* ok_out) {
     B2_NVTX;
-    REQUIRE(ctx && pair_off && sig96 && ok_out && n_sets > 0, "aggregate_verify: bad arguments");
-    REQUIRE(ctx->n_val > 0, "aggregate_verify: registry not loaded");
+    REQUIRE(ctx && pair_off, "aggregate_verify: bad arguments");
     int rc;
-    if ((rc = check_offsets(ctx, pair_off, n_sets, "aggregate_verify: pair_off"))) return rc;
+    if ((rc = check_offsets(ctx, pair_off, n_sets, "aggregate_verify", "pair_off"))) return rc;
     const uint64_t n_pairs = pair_off[n_sets];
-    REQUIRE(n_pairs == 0 || (signer && msg32), "aggregate_verify: null signers or messages");
-    REQUIRE(n_pairs + n_sets < (1ull << 32), "aggregate_verify: too many pairs");
+    if ((rc = check_aggregate_verify(ctx, signer, msg32, pair_off, n_pairs, sig96, n_sets, ok_out))) return rc;
     for (uint64_t i = 0; i < n_pairs; i++) REQUIRE(signer[i] < ctx->n_val, "aggregate_verify: signer index outside the registry");
     CK(cudaSetDevice(ctx->device));
     staging st(ctx);
@@ -1084,7 +1113,7 @@ int b2_aggregate_verify_pks(b2_ctx* ctx, const uint8_t* pk48, const uint8_t* msg
     B2_NVTX;
     REQUIRE(ctx && pair_off && sig96 && ok_out && n_sets > 0, "aggregate_verify_pks: bad arguments");
     int rc;
-    if ((rc = check_offsets(ctx, pair_off, n_sets, "aggregate_verify_pks: pair_off"))) return rc;
+    if ((rc = check_offsets(ctx, pair_off, n_sets, "aggregate_verify_pks", "pair_off"))) return rc;
     const uint64_t n_pairs = pair_off[n_sets];
     REQUIRE(n_pairs == 0 || (pk48 && msg32), "aggregate_verify_pks: null pubkeys or messages");
     REQUIRE(n_pairs + n_sets < (1ull << 32), "aggregate_verify_pks: too many pairs");
@@ -1104,7 +1133,7 @@ int b2_aggregate_pks(b2_ctx* ctx, const uint8_t* pk48, const uint32_t* off, uint
     B2_NVTX;
     REQUIRE(ctx && off && out48 && status && n_seg > 0, "aggregate_pks: bad arguments");
     int rc;
-    if ((rc = check_offsets(ctx, off, n_seg, "aggregate_pks: off"))) return rc;
+    if ((rc = check_offsets(ctx, off, n_seg, "aggregate_pks"))) return rc;
     const uint64_t n_pk = off[n_seg];
     REQUIRE(n_pk == 0 || pk48, "aggregate_pks: null pubkeys");
     CK(cudaSetDevice(ctx->device));
@@ -1162,17 +1191,21 @@ int b2_sync_committee_load(b2_ctx* ctx, const uint8_t* pk48, uint32_t committee_
     return B2_OK;
 }
 
+static int check_sync_aggregate_verify(b2_ctx* ctx, const void* committee_idx, const void* bits, const void* msg32, const void* sig96, uint32_t n,
+                                       const void* ok_out) {
+    REQUIRE(ctx && committee_idx && bits && msg32 && sig96 && ok_out && n > 0, "sync_aggregate_verify: bad arguments");
+    return ctx->sync.n > 0 ? B2_OK : reject(ctx, "sync_aggregate_verify", "no sync committee loaded");
+}
 // eth_fast_aggregate_verify per block: the committee form of verify_fork (k_sync_aggregate_pk), the unchanged pairing half, then the
 // empty-participation rule on the verdicts
 int b2_sync_aggregate_verify_dev(b2_ctx* ctx, const uint32_t* d_committee_idx, const uint8_t* d_bits, const uint8_t* d_msg32, const uint8_t* d_sig96,
                                  uint32_t n, uint8_t* d_ok_out, uint8_t* d_pk48_out, void* stream) {
     B2_NVTX;
-    REQUIRE(ctx && d_committee_idx && d_bits && d_msg32 && d_sig96 && d_ok_out && n > 0, "sync_aggregate_verify_dev: bad arguments");
-    REQUIRE(ctx->sync.n > 0, "sync_aggregate_verify: no sync committee loaded");
+    int rc;
+    if ((rc = check_sync_aggregate_verify(ctx, d_committee_idx, d_bits, d_msg32, d_sig96, n, d_ok_out))) return rc;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
     vslot& V = ctx->slot[0];
-    int rc;
     pk_source P = {nullptr, nullptr, d_bits, 0, nullptr, 0, d_committee_idx, d_pk48_out};
     if ((rc = verify_fork(ctx, V, P, d_msg32, n, s)) || (rc = verify_main(ctx, V, d_sig96, n, d_ok_out, s))) return rc;
     k_sync_empty_verdict<<<blocks_for(n, 128), 128, 0, s>>>(V.pkst, d_sig96, n, d_ok_out);
@@ -1183,8 +1216,8 @@ int b2_sync_aggregate_verify_dev(b2_ctx* ctx, const uint32_t* d_committee_idx, c
 int b2_sync_aggregate_verify(b2_ctx* ctx, const uint32_t* committee_idx, const uint8_t* bits, const uint8_t* msg32, const uint8_t* sig96, uint32_t n,
                              uint8_t* ok_out, uint8_t* pk48_out) {
     B2_NVTX;
-    REQUIRE(ctx && committee_idx && bits && msg32 && sig96 && ok_out && n > 0, "sync_aggregate_verify: bad arguments");
-    REQUIRE(ctx->sync.n > 0, "sync_aggregate_verify: no sync committee loaded");
+    int rc;
+    if ((rc = check_sync_aggregate_verify(ctx, committee_idx, bits, msg32, sig96, n, ok_out))) return rc;
     for (uint32_t i = 0; i < n; i++) REQUIRE(committee_idx[i] < ctx->sync.n, "sync_aggregate_verify: committee index out of range");
     CK(cudaSetDevice(ctx->device));
     const size_t stride = (ctx->sync.size + 7) / 8;
@@ -1195,7 +1228,6 @@ int b2_sync_aggregate_verify(b2_ctx* ctx, const uint32_t* committee_idx, const u
     const uint8_t* dsig = st.in(sig96, (size_t)n * 96);
     uint8_t* dok = st.out(ok_out, n);
     uint8_t* d48 = pk48_out ? st.out(pk48_out, (size_t)n * 48) : nullptr;
-    int rc;
     if ((rc = st.rc) || (rc = b2_sync_aggregate_verify_dev(ctx, dc, db, dmsg, dsig, n, dok, d48, ctx->s_main))) return rc;
     return st.finish();
 }
@@ -1287,7 +1319,7 @@ int b2_attestations_decode(b2_ctx* ctx, const uint8_t* wire, const uint32_t* wof
     REQUIRE(ctx && wire && woff && n > 0 && bits_stride > 0 && bits_out && bit_len_out && data128_out && sig96_out && status_out,
             "attestations_decode: bad arguments");
     int rc;
-    if ((rc = check_offsets(ctx, woff, n, "attestations_decode: woff"))) return rc;
+    if ((rc = check_offsets(ctx, woff, n, "attestations_decode", "woff"))) return rc;
     CK(cudaSetDevice(ctx->device));
     staging st(ctx);
     const uint8_t* dwire = st.in(wire, woff[n], 16);
@@ -1304,30 +1336,45 @@ int b2_attestations_decode(b2_ctx* ctx, const uint8_t* wire, const uint32_t* wof
 }
 
 // ------------------------------------------------------------------------------------------ attestation intake (intake.cuh)
-// validate_target_epoch_against_current_time for the whole batch: the current slot's epoch or the one before it
-static bool intake_epoch_ok(uint64_t epoch, uint64_t current_slot, uint32_t slots_per_epoch) {
+// The batch layout both attestation intakes share: one epoch of slots_per_epoch * committees_per_slot committees, an epoch that
+// validate_target_epoch_against_current_time accepts for the whole batch (the current slot's epoch or the one before it), and a block
+// tree to resolve votes against.  slots_per_epoch > 0.
+static int check_intake(b2_ctx* ctx, uint32_t n_committees, uint32_t committees_per_slot, uint32_t slots_per_epoch, uint64_t epoch,
+                        uint64_t current_slot, const char* what) {
+    if ((uint64_t)committees_per_slot * slots_per_epoch != n_committees)
+        return reject(ctx, what, "n_committees must be slots_per_epoch * committees_per_slot");
     const uint64_t cur = current_slot / slots_per_epoch;
-    return epoch == cur || (cur > 0 && epoch == cur - 1);
+    if (current_slot >= (1ull << 63) || !(epoch == cur || (cur > 0 && epoch == cur - 1)))
+        return reject(ctx, what, "the epoch must be the current slot's epoch or the one before it");
+    if (ctx->n_blocks == 0) return reject(ctx, what, "no tree loaded (b2_tree_load)");
+    return B2_OK;
 }
-
+static int check_attestation_intake(b2_ctx* ctx, const void* wire, const void* woff, uint32_t n_att, const void* off, uint32_t n_committees,
+                                    uint32_t committees_per_slot, uint32_t slots_per_epoch, uint32_t bits_stride, uint64_t epoch, uint64_t current_slot,
+                                    const void* domain32, uint32_t max_votes, const void* status_out, const void* vote_out, const void* vote_off_out,
+                                    const void* sig96_out, const void* data128_out, const void* msg32_out, const void* source_epoch_out,
+                                    const void* target_epoch_out, const void* block_idx_out) {
+    REQUIRE(ctx && wire && woff && off && domain32 && status_out && vote_out && vote_off_out && sig96_out && data128_out && msg32_out &&
+                source_epoch_out && target_epoch_out && block_idx_out && n_att > 0 && max_votes > 0 && bits_stride > 0 && bits_stride <= 256 &&
+                committees_per_slot > 0 && slots_per_epoch > 0,
+            "attestation_intake: bad arguments");
+    return check_intake(ctx, n_committees, committees_per_slot, slots_per_epoch, epoch, current_slot, "attestation_intake");
+}
 int b2_attestation_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n_att, const uint32_t* d_off,
                               uint32_t n_committees, uint64_t n_sig, uint32_t committees_per_slot, uint32_t slots_per_epoch, uint32_t bits_stride,
                               uint64_t epoch, uint64_t current_slot, const uint8_t* domain32, uint32_t max_votes, int32_t* d_status_out,
                               uint32_t* d_vote_out, uint32_t* d_vote_off_out, uint8_t* d_sig96_out, uint8_t* d_data128_out, uint8_t* d_msg32_out,
                               uint64_t* d_source_epoch_out, uint64_t* d_target_epoch_out, uint32_t* d_block_idx_out, void* stream) {
     B2_NVTX;
-    REQUIRE(ctx && d_wire && d_woff && d_off && domain32 && d_status_out && d_vote_out && d_vote_off_out && d_sig96_out && d_data128_out &&
-                d_msg32_out && d_source_epoch_out && d_target_epoch_out && d_block_idx_out && n_att > 0 && max_votes > 0 && n_sig < (1ull << 32) &&
-                bits_stride > 0 && bits_stride <= 256 && committees_per_slot > 0 && slots_per_epoch > 0,
-            "attestation_intake_dev: bad arguments");
-    REQUIRE((uint64_t)committees_per_slot * slots_per_epoch == n_committees, "attestation_intake: n_committees must be slots_per_epoch * committees_per_slot");
-    REQUIRE(current_slot < (1ull << 63) && intake_epoch_ok(epoch, current_slot, slots_per_epoch),
-            "attestation_intake: the epoch must be the current slot's epoch or the one before it");
-    REQUIRE(ctx->n_blocks > 0, "attestation_intake: no tree loaded (b2_tree_load)");
+    int rc;
+    if ((rc = check_attestation_intake(ctx, d_wire, d_woff, n_att, d_off, n_committees, committees_per_slot, slots_per_epoch, bits_stride, epoch, current_slot, domain32,
+                                       max_votes, d_status_out, d_vote_out, d_vote_off_out, d_sig96_out, d_data128_out, d_msg32_out, d_source_epoch_out,
+                                       d_target_epoch_out, d_block_idx_out)))
+        return rc;
+    REQUIRE(n_sig < (1ull << 32), "attestation_intake: n_sig does not fit 32 bits");      // the host form's n_sig is a u32 offset
     CK(cudaSetDevice(ctx->device));
     intake_scratch& S = ctx->in;
     const size_t na = (size_t)n_att * 4, nc = ((size_t)n_committees + 1) * 4;
-    int rc;
     if ((rc = ensure(ctx, S.comm, na)) || (rc = ensure(ctx, S.pos, na)) || (rc = ensure(ctx, S.fp, na)) || (rc = ensure(ctx, S.grp, na)) ||
         (rc = ensure(ctx, S.bucket, nc)) || (rc = ensure(ctx, S.cursor, nc)) || (rc = ensure(ctx, S.nkept, nc)) || (rc = ensure(ctx, S.list, na)) ||
         (rc = ensure(ctx, S.lead, na)) || (rc = ensure(ctx, S.gstat, na)) || (rc = ensure(ctx, S.gblk, na)) || (rc = ensure(ctx, S.gmin, na)) ||
@@ -1368,19 +1415,13 @@ int b2_attestation_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, c
                           uint32_t* vote_off_out, uint8_t* sig96_out, uint8_t* data128_out, uint8_t* msg32_out, uint64_t* source_epoch_out,
                           uint64_t* target_epoch_out, uint32_t* block_idx_out) {
     B2_NVTX;
-    REQUIRE(ctx && wire && woff && off && domain32 && status_out && vote_out && vote_off_out && sig96_out && data128_out && msg32_out &&
-                source_epoch_out && target_epoch_out && block_idx_out && n_att > 0 && n_committees > 0 && max_votes > 0 && bits_stride > 0 &&
-                bits_stride <= 256 && committees_per_slot > 0 && slots_per_epoch > 0,
-            "attestation_intake: bad arguments");
-    REQUIRE((uint64_t)committees_per_slot * slots_per_epoch == n_committees, "attestation_intake: n_committees must be slots_per_epoch * committees_per_slot");
-    REQUIRE(current_slot < (1ull << 63) && intake_epoch_ok(epoch, current_slot, slots_per_epoch),
-            "attestation_intake: the epoch must be the current slot's epoch or the one before it");
-    REQUIRE(ctx->n_blocks > 0, "attestation_intake: no tree loaded (b2_tree_load)");
     int rc;
-    if ((rc = check_offsets(ctx, woff, n_att, "attestation_intake: woff"))) return rc;
-    REQUIRE(woff[n_att] <= wire_len, "attestation_intake: woff ends past the wire");
-    if ((rc = check_offsets(ctx, off, n_committees, "attestation_intake: off"))) return rc;
-    for (uint32_t c = 0; c < n_committees; c++) REQUIRE(off[c + 1] - off[c] <= 8 * bits_stride, "attestation_intake: a committee is larger than 8 * bits_stride");
+    if ((rc = check_attestation_intake(ctx, wire, woff, n_att, off, n_committees, committees_per_slot, slots_per_epoch, bits_stride, epoch, current_slot, domain32, max_votes,
+                                       status_out, vote_out, vote_off_out, sig96_out, data128_out, msg32_out, source_epoch_out, target_epoch_out,
+                                       block_idx_out)) ||
+        (rc = check_wire(ctx, woff, n_att, wire_len, "attestation_intake")) ||
+        (rc = check_committees(ctx, off, n_committees, bits_stride, "attestation_intake")))
+        return rc;
     const uint64_t n_sig = off[n_committees];
     CK(cudaSetDevice(ctx->device));
     staging st(ctx);
@@ -1410,6 +1451,19 @@ int b2_attestation_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, c
 }
 
 // ------------------------------------------------------------------------------------------ aggregated-attestation intake (aggintake.cuh)
+static int check_aggregate_and_proof_intake(b2_ctx* ctx, const void* wire, const void* woff, uint32_t n, const void* members, const void* off,
+                                            uint32_t n_committees, uint32_t committees_per_slot, uint32_t slots_per_epoch, uint32_t bits_stride,
+                                            uint64_t epoch, uint64_t current_slot, const void* domains96, uint32_t target_aggregators, const void* status_out,
+                                            const void* committee_out, const void* data_id_out, const void* bits_out, const void* sig96_out,
+                                            const void* msg32_out, const void* target_epoch_out, const void* block_idx_out, const void* members_out,
+                                            const void* item_off_out) {
+    REQUIRE(ctx && wire && woff && members && off && domains96 && status_out && committee_out && data_id_out && bits_out && sig96_out && msg32_out &&
+                target_epoch_out && block_idx_out && members_out && item_off_out && n > 0 && n < (1u << 28) && bits_stride > 0 && bits_stride <= 256 &&
+                (uint64_t)n * 8 * bits_stride < (1ull << 32) && committees_per_slot > 0 && slots_per_epoch > 0 && target_aggregators > 0,
+            "aggregate_and_proof_intake: bad arguments");
+    if (int rc = check_intake(ctx, n_committees, committees_per_slot, slots_per_epoch, epoch, current_slot, "aggregate_and_proof_intake")) return rc;
+    return ctx->n_val > 0 ? B2_OK : reject(ctx, "aggregate_and_proof_intake", "registry not loaded");
+}
 int b2_aggregate_and_proof_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n, const uint32_t* d_members,
                                       const uint32_t* d_off, uint32_t n_committees, uint64_t n_sig, uint32_t committees_per_slot, uint32_t slots_per_epoch,
                                       uint32_t bits_stride, uint64_t epoch, uint64_t current_slot, const uint8_t* domains96, uint32_t target_aggregators,
@@ -1417,23 +1471,17 @@ int b2_aggregate_and_proof_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64
                                       uint8_t* d_bits_out, uint8_t* d_sig96_out, uint8_t* d_msg32_out, uint64_t* d_target_epoch_out,
                                       uint32_t* d_block_idx_out, uint32_t* d_members_out, uint32_t* d_item_off_out, void* stream) {
     B2_NVTX;
-    REQUIRE(ctx && d_wire && d_woff && d_members && d_off && domains96 && d_status_out && d_committee_out && d_data_id_out && d_bits_out && d_sig96_out &&
-                d_msg32_out && d_target_epoch_out && d_block_idx_out && d_members_out && d_item_off_out && n > 0 && n < (1u << 28) &&
-                n_sig < (1ull << 32) && bits_stride > 0 && bits_stride <= 256 && (uint64_t)n * 8 * bits_stride < (1ull << 32) &&
-                committees_per_slot > 0 && slots_per_epoch > 0 && target_aggregators > 0,
-            "aggregate_and_proof_intake_dev: bad arguments");
-    REQUIRE((uint64_t)committees_per_slot * slots_per_epoch == n_committees,
-            "aggregate_and_proof_intake: n_committees must be slots_per_epoch * committees_per_slot");
-    REQUIRE(current_slot < (1ull << 63) && intake_epoch_ok(epoch, current_slot, slots_per_epoch),
-            "aggregate_and_proof_intake: the epoch must be the current slot's epoch or the one before it");
-    REQUIRE(ctx->n_blocks > 0, "aggregate_and_proof_intake: no tree loaded (b2_tree_load)");
-    REQUIRE(ctx->n_val > 0, "aggregate_and_proof_intake: registry not loaded");
+    int rc;
+    if ((rc = check_aggregate_and_proof_intake(ctx, d_wire, d_woff, n, d_members, d_off, n_committees, committees_per_slot, slots_per_epoch, bits_stride, epoch,
+                                               current_slot, domains96, target_aggregators, d_status_out, d_committee_out, d_data_id_out, d_bits_out,
+                                               d_sig96_out, d_msg32_out, d_target_epoch_out, d_block_idx_out, d_members_out, d_item_off_out)))
+        return rc;
+    REQUIRE(n_sig < (1ull << 32), "aggregate_and_proof_intake: n_sig does not fit 32 bits");      // the host form's n_sig is a u32 offset
     CK(cudaSetDevice(ctx->device));
     api_scratch& S = ctx->api;
     uint32_t tab = 1;
     while (tab < 2 * n) tab <<= 1;
     const size_t na = (size_t)n * 4, nc = ((size_t)n_committees + 1) * 4;
-    int rc;
     if ((rc = ensure(ctx, S.comm, na)) || (rc = ensure(ctx, S.fp, na)) || (rc = ensure(ctx, S.slot_of, na)) || (rc = ensure(ctx, S.dtab, (size_t)tab * 4)) ||
         (rc = ensure(ctx, S.dmin, (size_t)tab * 4)) || (rc = ensure(ctx, S.list, na)) || (rc = ensure(ctx, S.acc, na)) ||
         (rc = ensure(ctx, S.accepted_by, ctx->n_val * 4)) || (rc = ensure(ctx, S.incomm, n)) || (rc = ensure(ctx, S.tst, n)) ||
@@ -1547,23 +1595,13 @@ int b2_aggregate_and_proof_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wir
                                   uint8_t* sig96_out, uint8_t* msg32_out, uint64_t* target_epoch_out, uint32_t* block_idx_out, uint32_t* members_out,
                                   uint32_t* item_off_out) {
     B2_NVTX;
-    REQUIRE(ctx && wire && woff && members && off && domains96 && status_out && committee_out && data_id_out && bits_out && sig96_out && msg32_out &&
-                target_epoch_out && block_idx_out && members_out && item_off_out && n > 0 && n < (1u << 28) && n_committees > 0 && bits_stride > 0 &&
-                bits_stride <= 256 && (uint64_t)n * 8 * bits_stride < (1ull << 32) && committees_per_slot > 0 && slots_per_epoch > 0 &&
-                target_aggregators > 0,
-            "aggregate_and_proof_intake: bad arguments");
-    REQUIRE((uint64_t)committees_per_slot * slots_per_epoch == n_committees,
-            "aggregate_and_proof_intake: n_committees must be slots_per_epoch * committees_per_slot");
-    REQUIRE(current_slot < (1ull << 63) && intake_epoch_ok(epoch, current_slot, slots_per_epoch),
-            "aggregate_and_proof_intake: the epoch must be the current slot's epoch or the one before it");
-    REQUIRE(ctx->n_blocks > 0, "aggregate_and_proof_intake: no tree loaded (b2_tree_load)");
-    REQUIRE(ctx->n_val > 0, "aggregate_and_proof_intake: registry not loaded");
     int rc;
-    if ((rc = check_offsets(ctx, woff, n, "aggregate_and_proof_intake: woff"))) return rc;
-    REQUIRE(woff[n] <= wire_len, "aggregate_and_proof_intake: woff ends past the wire");
-    if ((rc = check_offsets(ctx, off, n_committees, "aggregate_and_proof_intake: off"))) return rc;
-    for (uint32_t c = 0; c < n_committees; c++)
-        REQUIRE(off[c + 1] - off[c] <= 8 * bits_stride, "aggregate_and_proof_intake: a committee is larger than 8 * bits_stride");
+    if ((rc = check_aggregate_and_proof_intake(ctx, wire, woff, n, members, off, n_committees, committees_per_slot, slots_per_epoch, bits_stride, epoch, current_slot,
+                                               domains96, target_aggregators, status_out, committee_out, data_id_out, bits_out, sig96_out, msg32_out,
+                                               target_epoch_out, block_idx_out, members_out, item_off_out)) ||
+        (rc = check_wire(ctx, woff, n, wire_len, "aggregate_and_proof_intake")) ||
+        (rc = check_committees(ctx, off, n_committees, bits_stride, "aggregate_and_proof_intake")))
+        return rc;
     const uint64_t n_sig = off[n_committees], W = 8ull * bits_stride;
     CK(cudaSetDevice(ctx->device));
     staging st(ctx);
@@ -1596,6 +1634,24 @@ static uint32_t isqrt_u32(uint32_t n) {
     return x;
 }
 
+static int check_block_attestations(b2_ctx* ctx, const void* wire, const void* woff, uint32_t n_att, const void* block_off, const void* block_slot,
+                                    uint32_t n_blocks, const void* members, const void* off, uint32_t n_committees, uint32_t cps_prev, uint32_t cps_cur,
+                                    const void* chain_roots, const void* justified80, const void* domains64, uint32_t slots_per_epoch,
+                                    uint32_t min_inclusion_delay, uint32_t bits_stride, uint64_t effective_balance_increment, const void* status_out,
+                                    const void* flag_mask_out, const void* numerator_out, const void* block_status_out, const void* block_first_out,
+                                    const void* block_reward_out, const void* n_applied_out) {
+    REQUIRE(ctx && wire && woff && block_off && block_slot && members && off && chain_roots && justified80 && domains64 && status_out && flag_mask_out &&
+                numerator_out && block_status_out && block_first_out && block_reward_out && n_applied_out && n_att > 0 && n_att < (1u << 28) &&
+                n_blocks > 0 && bits_stride > 0 && bits_stride <= 256 && (uint64_t)n_att * 8 * bits_stride < (1ull << 32) && slots_per_epoch > 0 &&
+                cps_cur > 0 && ((uint64_t)cps_prev + cps_cur) * slots_per_epoch < (1ull << 31) && min_inclusion_delay > 0 &&
+                effective_balance_increment > 0,
+            "block_attestations: bad arguments");
+    REQUIRE(((uint64_t)cps_prev + cps_cur) * slots_per_epoch == n_committees,
+            "block_attestations: n_committees must be slots_per_epoch * (cps_prev + cps_cur)");
+    REQUIRE(ctx->n_val > 0, "block_attestations: registry not loaded");
+    return ctx->reg.part[0] && ctx->reg.part[1] ? B2_OK
+                                                : reject(ctx, "block_attestations", "both participation tables must be loaded (b2_participation_load)");
+}
 int b2_block_attestations_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n_att, const uint32_t* d_block_off,
                               const uint64_t* d_block_slot, uint32_t n_blocks, const uint32_t* d_members, const uint32_t* d_off, uint32_t n_committees,
                               uint64_t n_sig,
@@ -1605,20 +1661,15 @@ int b2_block_attestations_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_
                               int32_t* d_block_status_out, uint32_t* d_block_first_out, uint64_t* d_block_reward_out, uint32_t* d_n_applied_out,
                               void* stream) {
     B2_NVTX;
-    REQUIRE(ctx && d_wire && d_woff && d_block_off && d_block_slot && d_members && d_off && d_chain_roots && justified80 && domains64 && d_status_out &&
-                d_flag_mask_out && d_numerator_out && d_block_status_out && d_block_first_out && d_block_reward_out && d_n_applied_out && n_att > 0 &&
-                n_att < (1u << 28) && n_blocks > 0 && n_sig < (1ull << 32) && bits_stride > 0 && bits_stride <= 256 &&
-                (uint64_t)n_att * 8 * bits_stride < (1ull << 32) && slots_per_epoch > 0 && cps_cur > 0 &&
-                ((uint64_t)cps_prev + cps_cur) * slots_per_epoch < (1ull << 31) && min_inclusion_delay > 0 && effective_balance_increment > 0,
-            "block_attestations_dev: bad arguments");
-    REQUIRE(((uint64_t)cps_prev + cps_cur) * slots_per_epoch == n_committees,
-            "block_attestations: n_committees must be slots_per_epoch * (cps_prev + cps_cur)");
-    REQUIRE(ctx->n_val > 0, "block_attestations: registry not loaded");
-    REQUIRE(ctx->reg.part[0] && ctx->reg.part[1], "block_attestations: both participation tables must be loaded (b2_participation_load)");
+    int rc;
+    if ((rc = check_block_attestations(ctx, d_wire, d_woff, n_att, d_block_off, d_block_slot, n_blocks, d_members, d_off, n_committees, cps_prev, cps_cur, d_chain_roots,
+                                       justified80, domains64, slots_per_epoch, min_inclusion_delay, bits_stride, effective_balance_increment, d_status_out,
+                                       d_flag_mask_out, d_numerator_out, d_block_status_out, d_block_first_out, d_block_reward_out, d_n_applied_out)))
+        return rc;
+    REQUIRE(n_sig < (1ull << 32), "block_attestations: n_sig does not fit 32 bits");      // the host form's n_sig is a u32 offset
     CK(cudaSetDevice(ctx->device));
     ba_scratch& S = ctx->ba;
     const size_t n = n_att, W = 8ull * bits_stride;
-    int rc;
     if ((rc = ensure(ctx, S.blk_of, n * 4)) || (rc = ensure(ctx, S.cur, n)) || (rc = ensure(ctx, S.fav_ok, n)) || (rc = ensure(ctx, S.accept, 2 * n)) ||
         (rc = ensure(ctx, S.num1, n * 8)) || (rc = ensure(ctx, S.bits, n * bits_stride + 16)) || (rc = ensure(ctx, S.sig96, n * 96)) ||
         (rc = ensure(ctx, S.data128, n * 128)) || (rc = ensure(ctx, S.dom32, n * 32)) || (rc = ensure(ctx, S.msg32, n * 32)) ||
@@ -1700,20 +1751,13 @@ int b2_block_attestations(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, c
                           int32_t* status_out, uint8_t* flag_mask_out, uint64_t* numerator_out, int32_t* block_status_out, uint32_t* block_first_out,
                           uint64_t* block_reward_out, uint32_t* n_applied_out) {
     B2_NVTX;
-    REQUIRE(ctx && wire && woff && block_off && block_slot && members && off && chain_roots && justified80 && domains64 && status_out && flag_mask_out &&
-                numerator_out && block_status_out && block_first_out && block_reward_out && n_applied_out && n_att > 0 && n_att < (1u << 28) &&
-                n_blocks > 0 && bits_stride > 0 && bits_stride <= 256 && (uint64_t)n_att * 8 * bits_stride < (1ull << 32) && slots_per_epoch > 0 &&
-                cps_cur > 0 && ((uint64_t)cps_prev + cps_cur) * slots_per_epoch < (1ull << 31) && min_inclusion_delay > 0 &&
-                effective_balance_increment > 0,
-            "block_attestations: bad arguments");
-    REQUIRE(((uint64_t)cps_prev + cps_cur) * slots_per_epoch == n_committees,
-            "block_attestations: n_committees must be slots_per_epoch * (cps_prev + cps_cur)");
-    REQUIRE(ctx->n_val > 0, "block_attestations: registry not loaded");
-    REQUIRE(ctx->reg.part[0] && ctx->reg.part[1], "block_attestations: both participation tables must be loaded (b2_participation_load)");
     int rc;
-    if ((rc = check_offsets(ctx, woff, n_att, "block_attestations: woff"))) return rc;
-    REQUIRE(woff[n_att] <= wire_len, "block_attestations: woff ends past the wire");
-    if ((rc = check_offsets(ctx, block_off, n_blocks, "block_attestations: block_off"))) return rc;
+    if ((rc = check_block_attestations(ctx, wire, woff, n_att, block_off, block_slot, n_blocks, members, off, n_committees, cps_prev, cps_cur, chain_roots, justified80,
+                                       domains64, slots_per_epoch, min_inclusion_delay, bits_stride, effective_balance_increment, status_out, flag_mask_out,
+                                       numerator_out, block_status_out, block_first_out, block_reward_out, n_applied_out)) ||
+        (rc = check_wire(ctx, woff, n_att, wire_len, "block_attestations")) ||
+        (rc = check_offsets(ctx, block_off, n_blocks, "block_attestations", "block_off")))
+        return rc;
     REQUIRE(block_off[n_blocks] == n_att, "block_attestations: block_off must end at n_att");
     const uint64_t e = block_slot[0] / slots_per_epoch;
     REQUIRE(block_slot[0] < (1ull << 63), "block_attestations: block slot out of range");
@@ -1721,9 +1765,7 @@ int b2_block_attestations(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, c
         REQUIRE(block_slot[b] > block_slot[b - 1] && block_slot[b] / slots_per_epoch == e,
                 "block_attestations: block slots must increase strictly and lie in one epoch");
     REQUIRE(e > 0 ? cps_prev > 0 : cps_prev == 0, "block_attestations: cps_prev must be 0 exactly at epoch 0");
-    if ((rc = check_offsets(ctx, off, n_committees, "block_attestations: off"))) return rc;
-    for (uint32_t c = 0; c < n_committees; c++)
-        REQUIRE(off[c + 1] - off[c] <= 8 * bits_stride, "block_attestations: a committee is larger than 8 * bits_stride");
+    if ((rc = check_committees(ctx, off, n_committees, bits_stride, "block_attestations"))) return rc;
     const uint64_t n_sig = off[n_committees];
     CK(cudaSetDevice(ctx->device));
     staging st(ctx);
@@ -1753,19 +1795,29 @@ int b2_block_attestations(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, c
 // SyncCommitteeMessage (pos-evolution.md:548-557) through the sync_committee_{subnet_id} checks of the upstream Altair p2p spec, and the
 // accepted ones into the SyncCommitteeContributions and SyncAggregates of process_sync_committee_contributions (upstream Altair validator
 // spec).  The signature check shares the AggregateVerify buffers with b2_aggregate_verify[_dev] and the intakes: one stream for all of them.
+static int check_sync_committee_messages(b2_ctx* ctx, const void* wire, const void* woff, uint32_t n, const void* subnet, const void* position_validator,
+                                         uint32_t committee_size, uint32_t subnet_count, const void* domain32, const void* status_out, const void* root_id_out,
+                                         const void* roots32_out, const void* n_roots_out, const void* contrib_bits_out, const void* contrib_sig96_out,
+                                         const void* contrib_present_out, const void* agg_bits_out, const void* agg_sig96_out) {
+    REQUIRE(ctx && wire && woff && subnet && position_validator && domain32 && status_out && root_id_out && roots32_out && n_roots_out &&
+                contrib_bits_out && contrib_sig96_out && contrib_present_out && agg_bits_out && agg_sig96_out && n > 0 && n < (1u << 24) &&
+                committee_size > 0 && subnet_count > 0 && (uint64_t)n * (subnet_count + 1) < (1ull << 31),
+            "sync_committee_messages: bad arguments");
+    REQUIRE(committee_size % subnet_count == 0, "sync_committee_messages: committee_size must be a multiple of subnet_count");
+    REQUIRE(committee_size <= B2_SYNC_MAX_SIZE, "sync_committee_messages: committee_size above the kernels' limit (1024)");
+    return ctx->n_val > 0 ? B2_OK : reject(ctx, "sync_committee_messages", "registry not loaded");
+}
 int b2_sync_committee_messages_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n, const uint32_t* d_subnet,
                                    const uint32_t* d_position_validator, uint32_t committee_size, uint32_t subnet_count, uint64_t current_slot,
                                    const uint8_t* domain32, int32_t* d_status_out, uint32_t* d_root_id_out, uint8_t* d_roots32_out,
                                    uint32_t* d_n_roots_out, uint8_t* d_contrib_bits_out, uint8_t* d_contrib_sig96_out, uint8_t* d_contrib_present_out,
                                    uint8_t* d_agg_bits_out, uint8_t* d_agg_sig96_out, void* stream) {
     B2_NVTX;
-    REQUIRE(ctx && d_wire && d_woff && d_subnet && d_position_validator && domain32 && d_status_out && d_root_id_out && d_roots32_out && d_n_roots_out &&
-                d_contrib_bits_out && d_contrib_sig96_out && d_contrib_present_out && d_agg_bits_out && d_agg_sig96_out && n > 0 && n < (1u << 24) &&
-                committee_size > 0 && subnet_count > 0 && (uint64_t)n * (subnet_count + 1) < (1ull << 31),
-            "sync_committee_messages_dev: bad arguments");
-    REQUIRE(committee_size % subnet_count == 0, "sync_committee_messages: committee_size must be a multiple of subnet_count");
-    REQUIRE(committee_size <= B2_SYNC_MAX_SIZE, "sync_committee_messages: committee_size above the kernels' limit (1024)");
-    REQUIRE(ctx->n_val > 0, "sync_committee_messages: registry not loaded");
+    int rc;
+    if ((rc = check_sync_committee_messages(ctx, d_wire, d_woff, n, d_subnet, d_position_validator, committee_size, subnet_count, domain32, d_status_out, d_root_id_out,
+                                            d_roots32_out, d_n_roots_out, d_contrib_bits_out, d_contrib_sig96_out, d_contrib_present_out, d_agg_bits_out,
+                                            d_agg_sig96_out)))
+        return rc;
     CK(cudaSetDevice(ctx->device));
     scm_scratch& S = ctx->scm;
     const uint32_t sub = committee_size / subnet_count;
@@ -1773,7 +1825,6 @@ int b2_sync_committee_messages_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t 
     uint32_t tab = 1;
     while (tab < 2 * n) tab <<= 1;
     const size_t na = (size_t)n * 4, np = (size_t)committee_size * 4;
-    int rc;
     if ((rc = ensure(ctx, S.keys, (size_t)committee_size * 8)) || (rc = ensure(ctx, S.canon, na)) || (rc = ensure(ctx, S.first, np)) ||
         (rc = ensure(ctx, S.pitem, np)) || (rc = ensure(ctx, S.proot, np)) || (rc = ensure(ctx, S.signer, na)) || (rc = ensure(ctx, S.pair_off, na + 4)) ||
         (rc = ensure(ctx, S.msg, (size_t)n * 32)) || (rc = ensure(ctx, S.sig, (size_t)n * 96)) || (rc = ensure(ctx, S.ok, n)) ||
@@ -1872,16 +1923,11 @@ int b2_sync_committee_messages(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_l
                                uint8_t* contrib_bits_out, uint8_t* contrib_sig96_out, uint8_t* contrib_present_out, uint8_t* agg_bits_out,
                                uint8_t* agg_sig96_out) {
     B2_NVTX;
-    REQUIRE(ctx && wire && woff && subnet && position_validator && domain32 && status_out && root_id_out && roots32_out && n_roots_out &&
-                contrib_bits_out && contrib_sig96_out && contrib_present_out && agg_bits_out && agg_sig96_out && n > 0 && n < (1u << 24) &&
-                committee_size > 0 && subnet_count > 0 && (uint64_t)n * (subnet_count + 1) < (1ull << 31),
-            "sync_committee_messages: bad arguments");
-    REQUIRE(committee_size % subnet_count == 0, "sync_committee_messages: committee_size must be a multiple of subnet_count");
-    REQUIRE(committee_size <= B2_SYNC_MAX_SIZE, "sync_committee_messages: committee_size above the kernels' limit (1024)");
-    REQUIRE(ctx->n_val > 0, "sync_committee_messages: registry not loaded");
     int rc;
-    if ((rc = check_offsets(ctx, woff, n, "sync_committee_messages: woff"))) return rc;
-    REQUIRE(woff[n] <= wire_len, "sync_committee_messages: woff ends past the wire");
+    if ((rc = check_sync_committee_messages(ctx, wire, woff, n, subnet, position_validator, committee_size, subnet_count, domain32, status_out, root_id_out, roots32_out,
+                                            n_roots_out, contrib_bits_out, contrib_sig96_out, contrib_present_out, agg_bits_out, agg_sig96_out)) ||
+        (rc = check_wire(ctx, woff, n, wire_len, "sync_committee_messages")))
+        return rc;
     for (uint32_t p = 0; p < committee_size; p++)
         REQUIRE(position_validator[p] < ctx->n_val, "sync_committee_messages: a position_validator entry is outside the registry");
     CK(cudaSetDevice(ctx->device));
@@ -1909,15 +1955,19 @@ int b2_sync_committee_messages(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_l
 }
 
 // ------------------------------------------------------------------------------------------ committee shuffle
+static int check_shuffle_committees(b2_ctx* ctx, const uint8_t* seed32, const uint32_t* members_out, uint32_t rounds) {
+    REQUIRE(ctx && seed32 && members_out && rounds <= 255, "shuffle_committees: bad arguments");
+    return B2_OK;
+}
 int b2_shuffle_committees_dev(b2_ctx* ctx, const uint8_t* d_seed32, const uint32_t* d_active, uint32_t n_active, uint32_t rounds,
                               uint32_t* d_members_out, void* stream) {
     B2_NVTX;
-    REQUIRE(ctx && d_seed32 && d_members_out && rounds <= 255, "shuffle_committees_dev: bad arguments");
+    int rc;
+    if ((rc = check_shuffle_committees(ctx, d_seed32, d_members_out, rounds))) return rc;
     if (n_active == 0) return B2_OK;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
     const uint32_t nblk = (n_active + 255) / 256;
-    int rc;
     if ((rc = ensure(ctx, ctx->sc_shuf, (size_t)rounds * nblk * 32 + 16)) || (rc = ensure(ctx, ctx->sc_pivot, (size_t)rounds * 8 + 16))) return rc;
     if (rounds) {
         k_shuffle_sources<<<blocks_for((uint64_t)rounds * (nblk + 1), 128), 128, 0, s>>>(d_seed32, n_active, rounds, nblk, (uint8_t*)ctx->sc_shuf.p,
@@ -1932,14 +1982,14 @@ int b2_shuffle_committees_dev(b2_ctx* ctx, const uint8_t* d_seed32, const uint32
 
 int b2_shuffle_committees(b2_ctx* ctx, const uint8_t* seed32, const uint32_t* active, uint32_t n_active, uint32_t rounds, uint32_t* members_out) {
     B2_NVTX;
-    REQUIRE(ctx && seed32 && members_out && rounds <= 255, "shuffle_committees: bad arguments");
+    int rc;
+    if ((rc = check_shuffle_committees(ctx, seed32, members_out, rounds))) return rc;
     if (n_active == 0) return B2_OK;
     CK(cudaSetDevice(ctx->device));
     staging st(ctx);
     const uint8_t* dseed = st.in(seed32, 32);
     const uint32_t* dact = active ? st.in(active, n_active) : nullptr;
     uint32_t* dm = st.out(members_out, n_active);
-    int rc;
     if ((rc = st.rc) || (rc = b2_shuffle_committees_dev(ctx, dseed, dact, n_active, rounds, dm, ctx->s_main))) return rc;
     return st.finish();
 }
@@ -1992,11 +2042,16 @@ int b2_latest_messages_read(b2_ctx* ctx, uint64_t* epoch, uint32_t* block_idx, u
     return B2_OK;
 }
 
+static int check_latest_messages_update(b2_ctx* ctx, const void* members, const void* off, const void* bits, uint32_t bits_stride, const void* target_epoch,
+                                        const void* block_idx, uint32_t n_agg) {
+    REQUIRE(ctx && members && off && bits && target_epoch && block_idx && n_agg > 0 && bits_stride > 0, "latest_messages_update: bad arguments");
+    return ctx->n_val > 0 ? B2_OK : reject(ctx, "latest_messages_update", "registry not loaded");
+}
 int b2_latest_messages_update_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_off, const uint8_t* d_bits, uint32_t bits_stride,
                                   const uint64_t* d_target_epoch, const uint32_t* d_block_idx, const uint8_t* d_accept, uint32_t n_agg, void* stream) {
     B2_NVTX;
-    REQUIRE(ctx && d_members && d_off && d_bits && d_target_epoch && d_block_idx && n_agg > 0 && bits_stride > 0, "latest_messages_update_dev: bad arguments");
-    REQUIRE(ctx->n_val > 0, "latest_messages_update: registry not loaded");
+    int rc;
+    if ((rc = check_latest_messages_update(ctx, d_members, d_off, d_bits, bits_stride, d_target_epoch, d_block_idx, n_agg))) return rc;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
     k_lmd_phase1<<<n_agg, 128, 0, s>>>(d_members, d_off, d_bits, bits_stride, d_target_epoch, d_accept, ctx->reg.equiv, n_agg, ctx->reg.lmd_key,
@@ -2011,10 +2066,10 @@ int b2_latest_messages_update_dev(b2_ctx* ctx, const uint32_t* d_members, const 
 int b2_latest_messages_update(b2_ctx* ctx, const uint32_t* members, const uint32_t* off, const uint8_t* bits, uint32_t bits_stride,
                               const uint64_t* target_epoch, const uint32_t* block_idx, const uint8_t* accept, uint32_t n_agg) {
     B2_NVTX;
-    REQUIRE(ctx && members && off && bits && target_epoch && block_idx && n_agg > 0 && bits_stride > 0, "latest_messages_update: bad arguments");
-    REQUIRE(ctx->n_val > 0, "latest_messages_update: registry not loaded");
     int rc;
-    if ((rc = check_batch(ctx, members, off, bits_stride, n_agg, ctx->n_val))) return rc;
+    if ((rc = check_latest_messages_update(ctx, members, off, bits, bits_stride, target_epoch, block_idx, n_agg)) ||
+        (rc = check_batch(ctx, members, off, bits_stride, n_agg, ctx->n_val, "latest_messages_update")))
+        return rc;
     for (uint32_t a = 0; a < n_agg; a++) REQUIRE(target_epoch[a] < 0xffffffffull, "latest_messages_update: epoch does not fit 32 bits");
     CK(cudaSetDevice(ctx->device));
     staging st(ctx);
@@ -2066,7 +2121,7 @@ int b2_participation_update(b2_ctx* ctx, int which, const uint32_t* members, con
                 effective_balance_increment > 0, "participation_update: bad arguments");
     REQUIRE(ctx->n_val > 0 && ctx->reg.part[which], "participation_update: registry / participation table not loaded");
     int rc;
-    if ((rc = check_batch(ctx, members, off, bits_stride, n_agg, ctx->n_val))) return rc;
+    if ((rc = check_batch(ctx, members, off, bits_stride, n_agg, ctx->n_val, "participation_update"))) return rc;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = ctx->s_main;
     staging st(ctx);
@@ -2202,17 +2257,21 @@ int b2_slasher_free(b2_ctx* ctx) {
     return B2_OK;
 }
 
+static int check_slasher_advance(b2_ctx* ctx, uint64_t current_epoch) {
+    REQUIRE(ctx && ctx->sl.H, "slasher_advance: no slasher (b2_slasher_init)");
+    return current_epoch >= ctx->sl.cur && current_epoch < 0xffffffffull ? B2_OK
+                                                                         : reject(ctx, "slasher_advance", "the current epoch only moves forward and fits 32 bits");
+}
 int b2_slasher_advance_dev(b2_ctx* ctx, uint64_t current_epoch, void* stream) {
     B2_NVTX;
-    REQUIRE(ctx && ctx->sl.H, "slasher_advance: no slasher (b2_slasher_init)");
+    int rc;
+    if ((rc = check_slasher_advance(ctx, current_epoch))) return rc;
     slasher_tables& t = ctx->sl;
-    REQUIRE(current_epoch >= t.cur && current_epoch < 0xffffffffull, "slasher_advance: the current epoch only moves forward and fits 32 bits");
     if (current_epoch == t.cur) return B2_OK;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
     const uint64_t n_cols = current_epoch - t.cur;
     if (n_cols >= t.H) {
-        int rc;
         if ((rc = slasher_clear(ctx, t, s))) return rc;
     } else {
         const unsigned blocks = (unsigned)std::min<uint64_t>((t.n_rows * n_cols + 255) / 256, (uint64_t)ctx->n_sm * 16);
@@ -2225,28 +2284,35 @@ int b2_slasher_advance_dev(b2_ctx* ctx, uint64_t current_epoch, void* stream) {
 
 int b2_slasher_advance(b2_ctx* ctx, uint64_t current_epoch) {
     B2_NVTX;
-    REQUIRE(ctx && ctx->sl.H, "slasher_advance: no slasher (b2_slasher_init)");
-    REQUIRE(current_epoch >= ctx->sl.cur && current_epoch < 0xffffffffull, "slasher_advance: the current epoch only moves forward and fits 32 bits");
-    if (current_epoch == ctx->sl.cur) return B2_OK;
+    int rc;
+    if ((rc = check_slasher_advance(ctx, current_epoch))) return rc;
+    if (current_epoch == ctx->sl.cur) return B2_OK;      // nothing to wait for
     CK(cudaSetDevice(ctx->device));
     CK(cudaDeviceSynchronize());      // updates enqueued on the caller's streams see the window they were enqueued with
-    int rc;
     if ((rc = b2_slasher_advance_dev(ctx, current_epoch, ctx->s_main))) return rc;
     CK(cudaStreamSynchronize(ctx->s_main));
     return B2_OK;
 }
 
+static int check_slasher_update(b2_ctx* ctx, const void* members, const void* off, const void* bits, uint32_t bits_stride, const void* source_epoch,
+                                const void* target_epoch, const void* data_root32, uint32_t n_agg, const void* att_status_out, const void* kind_out,
+                                const void* n_flagged_out) {
+    REQUIRE(ctx && members && off && bits && source_epoch && target_epoch && data_root32 && att_status_out && kind_out && n_flagged_out && n_agg > 0 &&
+                bits_stride > 0,
+            "slasher_update: bad arguments");
+    return ctx->sl.H ? B2_OK : reject(ctx, "slasher_update", "no slasher (b2_slasher_init)");
+}
 int b2_slasher_update_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_off, const uint8_t* d_bits, uint32_t bits_stride,
                           const uint64_t* d_source_epoch, const uint64_t* d_target_epoch, const uint8_t* d_data_root32, const uint8_t* d_accept,
                           uint32_t n_agg, int32_t* d_att_status_out, uint8_t* d_kind_out, uint32_t* d_conflict_target_out, uint32_t* d_n_flagged_out,
                           void* stream) {
     B2_NVTX;
-    REQUIRE(ctx && d_members && d_off && d_bits && d_source_epoch && d_target_epoch && d_data_root32 && d_att_status_out && d_kind_out &&
-                d_n_flagged_out && n_agg > 0 && bits_stride > 0, "slasher_update_dev: bad arguments");
-    REQUIRE(ctx->sl.H, "slasher_update: no slasher (b2_slasher_init)");
+    int rc;
+    if ((rc = check_slasher_update(ctx, d_members, d_off, d_bits, bits_stride, d_source_epoch, d_target_epoch, d_data_root32, n_agg, d_att_status_out, d_kind_out,
+                                   d_n_flagged_out)))
+        return rc;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
-    int rc;
     if ((rc = ensure(ctx, ctx->sl.agg_id, (size_t)n_agg * 4))) return rc;
     const slasher_view S = slasher_view_of(ctx->sl);
     uint32_t* ids = ctx->sl.agg_id;
@@ -2266,11 +2332,10 @@ int b2_slasher_update(b2_ctx* ctx, const uint32_t* members, const uint32_t* off,
                       const uint64_t* source_epoch, const uint64_t* target_epoch, const uint8_t* data_root32, const uint8_t* accept, uint32_t n_agg,
                       int32_t* att_status_out, uint8_t* kind_out, uint32_t* conflict_target_out, uint32_t* n_flagged_out) {
     B2_NVTX;
-    REQUIRE(ctx && members && off && bits && source_epoch && target_epoch && data_root32 && att_status_out && kind_out && n_flagged_out &&
-                n_agg > 0 && bits_stride > 0, "slasher_update: bad arguments");
-    REQUIRE(ctx->sl.H, "slasher_update: no slasher (b2_slasher_init)");
     int rc;
-    if ((rc = check_batch(ctx, members, off, bits_stride, n_agg, ctx->sl.n_val))) return rc;
+    if ((rc = check_slasher_update(ctx, members, off, bits, bits_stride, source_epoch, target_epoch, data_root32, n_agg, att_status_out, kind_out, n_flagged_out)) ||
+        (rc = check_batch(ctx, members, off, bits_stride, n_agg, ctx->sl.n_val, "slasher_update")))
+        return rc;
     for (uint32_t a = 0; a < n_agg; a++)
         REQUIRE(source_epoch[a] < 0xffffffffull && target_epoch[a] < 0xffffffffull, "slasher_update: epoch does not fit 32 bits");
     CK(cudaSetDevice(ctx->device));
@@ -2294,12 +2359,16 @@ int b2_slasher_update(b2_ctx* ctx, const uint32_t* members, const uint32_t* off,
 }
 
 // ------------------------------------------------------------------------------------------ equivocation discounting (:1405-1461)
+static int check_slasher_discount(b2_ctx* ctx, const void* members, const void* kind, uint64_t n_slots, const void* new_out, const void* n_new_out) {
+    REQUIRE(ctx && members && kind && new_out && n_new_out && n_slots > 0 && n_slots < (1ull << 32), "slasher_discount: bad arguments");
+    REQUIRE(ctx->n_val > 0, "slasher_discount: registry not loaded");
+    return ctx->sl.H ? B2_OK : reject(ctx, "slasher_discount", "no slasher (b2_slasher_init)");
+}
 int b2_slasher_discount_dev(b2_ctx* ctx, const uint32_t* d_members, const uint8_t* d_kind, uint64_t n_slots, uint8_t* d_new_out,
                             uint32_t* d_n_new_out, void* stream) {
     B2_NVTX;
-    REQUIRE(ctx && d_members && d_kind && d_new_out && d_n_new_out && n_slots > 0 && n_slots < (1ull << 32), "slasher_discount_dev: bad arguments");
-    REQUIRE(ctx->n_val > 0, "slasher_discount: registry not loaded");
-    REQUIRE(ctx->sl.H, "slasher_discount: no slasher (b2_slasher_init)");
+    int rc;
+    if ((rc = check_slasher_discount(ctx, d_members, d_kind, n_slots, d_new_out, d_n_new_out))) return rc;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
     const slasher_tables& t = ctx->sl;
@@ -2313,16 +2382,14 @@ int b2_slasher_discount_dev(b2_ctx* ctx, const uint32_t* d_members, const uint8_
 
 int b2_slasher_discount(b2_ctx* ctx, const uint32_t* members, const uint8_t* kind, uint64_t n_slots, uint8_t* new_out, uint32_t* n_new_out) {
     B2_NVTX;
-    REQUIRE(ctx && members && kind && new_out && n_new_out && n_slots > 0 && n_slots < (1ull << 32), "slasher_discount: bad arguments");
-    REQUIRE(ctx->n_val > 0, "slasher_discount: registry not loaded");
-    REQUIRE(ctx->sl.H, "slasher_discount: no slasher (b2_slasher_init)");
+    int rc;
+    if ((rc = check_slasher_discount(ctx, members, kind, n_slots, new_out, n_new_out))) return rc;
     CK(cudaSetDevice(ctx->device));
     staging st(ctx);
     const uint32_t* dm = st.in(members, n_slots);
     const uint8_t* dk = st.in(kind, n_slots);
     uint8_t* dnew = st.out(new_out, n_slots);
     uint32_t* dn = st.out(n_new_out, 1);
-    int rc;
     if ((rc = st.rc) || (rc = b2_slasher_discount_dev(ctx, dm, dk, n_slots, dnew, dn, ctx->s_main))) return rc;
     return st.finish();
 }
@@ -2357,6 +2424,18 @@ int b2_equivocating_merge_dev(b2_ctx* ctx, uint64_t v_begin, uint64_t v_end, con
 }
 
 // ------------------------------------------------------------------------------------------ block packing (pack.cuh)
+static int check_pack_attestations(b2_ctx* ctx, const void* members, const void* committee_off, const void* committee_table, uint32_t n_committees,
+                                   const void* cand_committee, const void* cand_data, const void* cand_flag_mask, const void* bits, uint32_t bits_stride,
+                                   const void* sig96, uint32_t n_cand, uint32_t max_out, uint64_t effective_balance_increment, const void* n_out,
+                                   const void* out_committee, const void* out_data, const void* out_bits, const void* out_sig96, const void* out_numerator,
+                                   const void* out_src_off, const void* out_src, const void* cand_status) {
+    REQUIRE(ctx && committee_off && (n_committees == 0 || (members && committee_table)) &&
+                (n_cand == 0 || (cand_committee && cand_data && cand_flag_mask && bits && sig96 && out_src && cand_status)) && n_out && out_committee &&
+                out_data && out_bits && out_sig96 && out_numerator && out_src_off && max_out > 0 && bits_stride > 0 && bits_stride <= PACK_MAX_WORDS * 4 &&
+                effective_balance_increment > 0,
+            "pack_attestations: bad arguments (max_out > 0, 0 < bits_stride <= 256, increment > 0)");
+    return ctx->n_val > 0 ? B2_OK : reject(ctx, "pack_attestations", "registry not loaded");
+}
 int b2_pack_attestations_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_committee_off, const uint8_t* d_committee_table,
                              uint32_t n_committees, const uint32_t* d_cand_committee, const uint32_t* d_cand_data, const uint8_t* d_cand_flag_mask,
                              const uint8_t* d_bits, uint32_t bits_stride, const uint8_t* d_sig96, uint32_t n_cand, uint32_t max_out,
@@ -2364,18 +2443,16 @@ int b2_pack_attestations_dev(b2_ctx* ctx, const uint32_t* d_members, const uint3
                              uint32_t* d_out_data, uint8_t* d_out_bits, uint8_t* d_out_sig96, uint64_t* d_out_numerator, uint32_t* d_out_src_off,
                              uint32_t* d_out_src, uint8_t* d_cand_status, void* stream) {
     B2_NVTX;
-    REQUIRE(ctx && d_committee_off && (n_committees == 0 || (d_members && d_committee_table)) &&
-                (n_cand == 0 || (d_cand_committee && d_cand_data && d_cand_flag_mask && d_bits && d_sig96 && d_out_src && d_cand_status)) && d_n_out &&
-                d_out_committee && d_out_data && d_out_bits && d_out_sig96 && d_out_numerator && d_out_src_off && max_out > 0 && bits_stride > 0 &&
-                bits_stride <= PACK_MAX_WORDS * 4 && effective_balance_increment > 0,
-            "pack_attestations_dev: bad arguments (max_out > 0, 0 < bits_stride <= 256, increment > 0)");
-    REQUIRE(ctx->n_val > 0, "pack_attestations: registry not loaded");
+    int rc;
+    if ((rc = check_pack_attestations(ctx, d_members, d_committee_off, d_committee_table, n_committees, d_cand_committee, d_cand_data, d_cand_flag_mask, d_bits,
+                                      bits_stride, d_sig96, n_cand, max_out, effective_balance_increment, d_n_out, d_out_committee, d_out_data, d_out_bits,
+                                      d_out_sig96, d_out_numerator, d_out_src_off, d_out_src, d_cand_status)))
+        return rc;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
     pack_scratch& S = ctx->pk;
     const size_t C = std::max<uint32_t>(n_cand, 1), K = n_committees, M = max_out, wstride = (bits_stride + 3) / 4;
     const size_t claim_words = 2 * ((ctx->n_val + 31) / 32);
-    int rc;
     if ((rc = ensure(ctx, S.cnt, K * 4)) || (rc = ensure(ctx, S.off, (K + 1) * 4)) || (rc = ensure(ctx, S.list, C * 4)) || (rc = ensure(ctx, S.fold_of, C * 4)) ||
         (rc = ensure(ctx, S.fdata, C * 4)) || (rc = ensure(ctx, S.fcnt, C * 4)) || (rc = ensure(ctx, S.frow, C * wstride * 4)) || (rc = ensure(ctx, S.fmask, C)) ||
         (rc = ensure(ctx, S.egain, C * 8)) || (rc = ensure(ctx, S.eslot, C * 4)) || (rc = ensure(ctx, S.claim, claim_words * 4)) ||
@@ -2445,14 +2522,12 @@ int b2_pack_attestations(b2_ctx* ctx, const uint32_t* members, const uint32_t* c
                          uint32_t* n_out, uint32_t* out_committee, uint32_t* out_data, uint8_t* out_bits, uint8_t* out_sig96, uint64_t* out_numerator,
                          uint32_t* out_src_off, uint32_t* out_src, uint8_t* cand_status) {
     B2_NVTX;
-    REQUIRE(ctx && committee_off && (n_committees == 0 || (members && committee_table)) &&
-                (n_cand == 0 || (cand_committee && cand_data && cand_flag_mask && bits && sig96 && out_src && cand_status)) && n_out && out_committee &&
-                out_data && out_bits && out_sig96 && out_numerator && out_src_off && max_out > 0 && bits_stride > 0 && bits_stride <= PACK_MAX_WORDS * 4 &&
-                effective_balance_increment > 0,
-            "pack_attestations: bad arguments (max_out > 0, 0 < bits_stride <= 256, increment > 0)");
-    REQUIRE(ctx->n_val > 0, "pack_attestations: registry not loaded");
     int rc;
-    if ((rc = check_batch(ctx, members, committee_off, bits_stride, n_committees, ctx->n_val))) return rc;
+    if ((rc = check_pack_attestations(ctx, members, committee_off, committee_table, n_committees, cand_committee, cand_data, cand_flag_mask, bits, bits_stride, sig96,
+                                      n_cand, max_out, effective_balance_increment, n_out, out_committee, out_data, out_bits, out_sig96, out_numerator,
+                                      out_src_off, out_src, cand_status)) ||
+        (rc = check_batch(ctx, members, committee_off, bits_stride, n_committees, ctx->n_val, "pack_attestations")))
+        return rc;
     // the committees of one table are pairwise disjoint and repeat no member
     std::vector<uint8_t> claimed(2 * ctx->n_val, 0);
     for (uint32_t k = 0; k < n_committees; k++) {

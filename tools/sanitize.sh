@@ -8,7 +8,8 @@
 #      (ldata, win, first) on colliding data
 #   3. compute-sanitizer --tool synccheck  on the same subset (illegal barrier use)
 #   4. the host side of the C ABI under AddressSanitizer + UBSan (pos_evolution_b200/libb200pos_asan.so, built by
-#      `python -m pos_evolution_b200.build --asan`) over the BLS / fork-choice / guard / error-contract tests
+#      `python -m pos_evolution_b200.build --asan`) over the BLS / fork-choice / guard / error-contract tests and the argument checks both
+#      forms of each entry point share
 set -u
 cd "$(dirname "$0")/.."
 OUT="${OUT:-$(mktemp -d)}"
@@ -29,7 +30,7 @@ if [ -f pos_evolution_b200/libb200pos_asan.so ]; then
     ASAN_LIB=$(gcc -print-file-name=libasan.so)
     B2_LIB=$PWD/pos_evolution_b200/libb200pos_asan.so LD_PRELOAD=$ASAN_LIB ASAN_OPTIONS=protect_shadow_gap=0:detect_leaks=0:halt_on_error=1 UBSAN_OPTIONS=print_stacktrace=1 \
         run asan_host 300 python -m pytest tests/test_gpu_bls.py tests/test_gpu_forkchoice.py tests/test_gpu_gather.py tests/test_gpu_participation.py \
-        tests/test_gpu_abi_contract.py -x -q -m gpu
+        tests/test_gpu_abi_contract.py tests/test_gpu_abi_pairs.py -x -q -m gpu
 else
     echo "no ASan build (python -m pos_evolution_b200.build --asan)"
 fi
