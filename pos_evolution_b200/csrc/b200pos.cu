@@ -104,46 +104,12 @@ struct slasher_tables {
     uint32_t H = 0, K = 0, cur = 0;      // H == 0: not initialised
 };
 
-// block packing (b2_pack_attestations_dev): the scratch of pack_view (pack.cuh), the decompressed candidate signatures, the gathered
-// constituents and their segment sums
-struct pack_scratch {
-    dbuf cnt, off, list, fold_of, fdata, fcnt, frow, fmask, egain, eslot, claim, dcomm, dmask, ctl, sel, ord;
-    dbuf aff, st, gaff, gst, sumjac, seg_status;
-};
-
 // hash_tree_root (ssz.cuh): the validators tree's node cache over C leaves (heap layout, 2C nodes of 8 words) and the scratch tree of
 // b2_ssz_chunks_root
 struct ssz_tables {
     dbuf cache;
     uint64_t n = 0, C = 0;      // C == 0: no cache
     dbuf chunks;
-};
-
-// attestation intake (intake.cuh): per attestation, per committee, per bucket entry, per member slot, and the root-sorted block ids
-struct intake_scratch {
-    dbuf comm, pos, fp, grp;
-    dbuf bucket, cursor, nkept;
-    dbuf list, lead, gstat, gblk, gmin, vgrp;
-    dbuf posatt, sorted;
-};
-
-// aggregated-attestation intake (aggintake.cuh): per item, per hash-table slot, per committee, per validator, per single-key set
-struct api_scratch {
-    dbuf comm, fp, slot_of, dtab, dmin, list, acc, accepted_by, incomm, tst, fbits, fav_ok;
-    dbuf bucket, cursor, sorted;
-    dbuf av_signer, av_off, av_msg, av_sig, av_ok;
-};
-
-// block attestations (blockatt.cuh): per attestation, plus its member row u32[8 * bits_stride]
-struct ba_scratch {
-    dbuf blk_of, cur, fav_ok, accept, num1, bits, sig96, data128, dom32, msg32, members, item_off;
-};
-
-// sync committee messages (syncmsg.cuh): per position, per item, per hash-table slot, per (root, subnet) segment; the decompressed item
-// signatures, the gathered ones and the segment sums
-struct scm_scratch {
-    dbuf keys, canon, first, pitem, proot, signer, pair_off, msg, sig, ok, slot_of, rtab, rmin, rid, seg_off, agg_off, gsrc;
-    dbuf aff, st, gaff, gst, sumjac, seg_status;
 };
 
 struct vslot {
@@ -226,12 +192,10 @@ struct b2_ctx {
     std::vector<dbuf> stage;                          // the synchronous entry points' host inputs and outputs (struct staging)
     sync_tables sync;
     slasher_tables sl;
-    pack_scratch pk;
     ssz_tables ssz;
-    intake_scratch in;
-    api_scratch api;
-    ba_scratch ba;
-    scm_scratch scm;
+    // per-call scratch (struct scratch) of the attestation and aggregated-attestation intakes, block attestations, sync committee
+    // messages and block packing
+    std::vector<dbuf> in, api, ba, scm, pk;
 };
 
 struct nvtx_scope {
@@ -275,28 +239,38 @@ static int ensure(b2_ctx* ctx, dbuf& b, size_t bytes) {
     return B2_OK;
 }
 
-// One synchronous call's host traffic on s_main.  in() uploads a host array into the call's next staging buffer (grow-only, as ensure);
+// One call's device buffers from a grow-only list: the i-th request gets bufs[i], grown as ensure grows it, so a call that makes its
+// requests in a fixed order finds each buffer where it left it.  The first error is kept in rc and makes every later request a no-op
+// (a null pointer), so a caller checks rc once after its requests and before its first memset or launch.
+struct scratch {
+    b2_ctx* ctx;
+    std::vector<dbuf>& bufs;
+    size_t used = 0;
+    int rc = B2_OK;
+    scratch(b2_ctx* c, std::vector<dbuf>& b) : ctx(c), bufs(b) {}
+    void* buf(size_t bytes) {
+        if (rc) return nullptr;
+        if (used == bufs.size()) bufs.emplace_back();
+        dbuf& b = bufs[used++];
+        rc = ensure(ctx, b, bytes);
+        return rc ? nullptr : b.p;
+    }
+    // p = a buffer of `count` T and `pad` bytes past them
+    template <class T> void operator()(T*& p, size_t count, size_t pad = 0) { p = static_cast<T*>(buf(count * sizeof(T) + pad)); }
+};
+
+// One synchronous call's host traffic on s_main.  in() uploads a host array into the call's next staging buffer (ctx->stage);
 // out() registers a host output with the device buffer that holds it (by default a staging buffer of its own); finish() copies every
-// output to host memory, synchronises, and only if all of that succeeded writes the caller's buffers.  The first error is kept in rc
-// and makes every later step a no-op, so a caller checks rc once before its launches and returns finish().
-struct staging {
+// output to host memory, synchronises, and only if all of that succeeded writes the caller's buffers.  As in scratch, the first error
+// makes every later step a no-op, so a caller checks rc once before its launches and returns finish().
+struct staging : scratch {
     struct output {
         void* host;
         const void* dev;
         size_t bytes;
     };
-    b2_ctx* ctx;
-    int rc = B2_OK;
-    size_t used = 0;
     std::vector<output> outs;
-    explicit staging(b2_ctx* c) : ctx(c) {}
-    void* buf(size_t bytes) {
-        if (rc) return nullptr;
-        if (used == ctx->stage.size()) ctx->stage.emplace_back();
-        dbuf& b = ctx->stage[used++];
-        rc = ensure(ctx, b, bytes);
-        return rc ? nullptr : b.p;
-    }
+    explicit staging(b2_ctx* c) : scratch(c, c->stage) {}
     // `pad` bytes past the end are allocated but not copied
     template <class T> const T* in(const T* host, size_t count, size_t pad = 0) {
         void* d = buf(count * sizeof(T) + pad);
@@ -1373,27 +1347,53 @@ int b2_attestation_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_
         return rc;
     REQUIRE(n_sig < (1ull << 32), "attestation_intake: n_sig does not fit 32 bits");      // the host form's n_sig is a u32 offset
     CK(cudaSetDevice(ctx->device));
-    intake_scratch& S = ctx->in;
-    const size_t na = (size_t)n_att * 4, nc = ((size_t)n_committees + 1) * 4;
-    if ((rc = ensure(ctx, S.comm, na)) || (rc = ensure(ctx, S.pos, na)) || (rc = ensure(ctx, S.fp, na)) || (rc = ensure(ctx, S.grp, na)) ||
-        (rc = ensure(ctx, S.bucket, nc)) || (rc = ensure(ctx, S.cursor, nc)) || (rc = ensure(ctx, S.nkept, nc)) || (rc = ensure(ctx, S.list, na)) ||
-        (rc = ensure(ctx, S.lead, na)) || (rc = ensure(ctx, S.gstat, na)) || (rc = ensure(ctx, S.gblk, na)) || (rc = ensure(ctx, S.gmin, na)) ||
-        (rc = ensure(ctx, S.vgrp, na)) || (rc = ensure(ctx, S.posatt, n_sig * 4)) || (rc = ensure(ctx, S.sorted, (size_t)ctx->n_blocks * 4)))
-        return rc;
     const tree_tables& t = ctx->tree;
-    intake_args A = {d_wire, wire_len, d_woff, n_att, d_off, n_committees, committees_per_slot, slots_per_epoch, bits_stride, n_sig, epoch, current_slot,
-                     t.root, t.parent, t.slot, S.sorted, ctx->n_blocks, S.comm, S.pos, S.fp, S.grp, S.bucket, S.cursor, S.nkept, S.list, S.lead,
-                     S.gstat, S.gblk, S.gmin, S.vgrp, S.posatt, d_status_out, d_vote_out, d_vote_off_out, d_sig96_out, max_votes, {},
-                     d_data128_out, d_msg32_out, d_source_epoch_out, d_target_epoch_out, d_block_idx_out, ctx->d_guard};
+    intake_args A = {};
+    A.wire = d_wire;
+    A.wire_len = wire_len;
+    A.woff = d_woff;
+    A.n_att = n_att;
+    A.off = d_off;
+    A.n_committees = n_committees;
+    A.committees_per_slot = committees_per_slot;
+    A.slots_per_epoch = slots_per_epoch;
+    A.bits_stride = bits_stride;
+    A.n_sig = n_sig;
+    A.epoch = epoch;
+    A.current_slot = current_slot;
+    A.root = t.root;
+    A.parent = t.parent;
+    A.slot = t.slot;
+    A.n_blocks = ctx->n_blocks;
+    A.status = d_status_out;
+    A.vote = d_vote_out;
+    A.vote_off = d_vote_off_out;
+    A.sig96 = d_sig96_out;
+    A.max_votes = max_votes;
     memcpy(A.domain.b, domain32, 32);
+    A.data128 = d_data128_out;
+    A.msg32 = d_msg32_out;
+    A.source_epoch = d_source_epoch_out;
+    A.target_epoch = d_target_epoch_out;
+    A.block_idx = d_block_idx_out;
+    A.guard = ctx->d_guard;
+    const size_t nc = (size_t)n_committees + 1;
+    uint32_t* sorted;      // written by k_intake_sorted, read by the kernels through A.sorted
+    scratch sc(ctx, ctx->in);
+    sc(A.comm, n_att); sc(A.pos, n_att); sc(A.fp, n_att); sc(A.grp, n_att);
+    sc(A.bucket, nc); sc(A.cursor, nc); sc(A.nkept, nc);
+    sc(A.list, n_att); sc(A.lead, n_att); sc(A.gstat, n_att); sc(A.gblk, n_att); sc(A.gmin, n_att); sc(A.vgrp, n_att);
+    sc(A.posatt, n_sig); sc(sorted, ctx->n_blocks);
+    if (sc.rc) return sc.rc;
+    A.sorted = sorted;
     cudaStream_t s = (cudaStream_t)stream;
     CK(cudaStreamWaitEvent(s, ctx->ev_intake, 0));
-    k_intake_sorted<<<blocks_for(ctx->n_blocks, 256), 256, 0, s>>>(t.rank_id, ctx->n_blocks, S.sorted);
+    k_intake_sorted<<<blocks_for(ctx->n_blocks, 256), 256, 0, s>>>(t.rank_id, ctx->n_blocks, sorted);
     CKL(ctx);
-    CK(cudaMemsetAsync(S.bucket, 0, nc, s));
+    CK(cudaMemsetAsync(A.bucket, 0, nc * 4, s));
     k_intake_parse<<<blocks_for((uint64_t)n_att * 32, 128), 128, 0, s>>>(A);
     CKL(ctx);
-    k_intake_scan<<<1, 1024, 0, s>>>(S.bucket, n_committees, S.cursor);      // bucket[n_committees] = the candidates
+    k_intake_scan<<<1, 1024, 0, s>>>(A.bucket, n_committees, A.cursor);      // bucket[n_committees] = the candidates
     CKL(ctx);
     k_intake_scatter<<<blocks_for(n_att, 256), 256, 0, s>>>(A);
     CKL(ctx);
@@ -1478,20 +1478,11 @@ int b2_aggregate_and_proof_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64
         return rc;
     REQUIRE(n_sig < (1ull << 32), "aggregate_and_proof_intake: n_sig does not fit 32 bits");      // the host form's n_sig is a u32 offset
     CK(cudaSetDevice(ctx->device));
-    api_scratch& S = ctx->api;
     uint32_t tab = 1;
     while (tab < 2 * n) tab <<= 1;
-    const size_t na = (size_t)n * 4, nc = ((size_t)n_committees + 1) * 4;
-    if ((rc = ensure(ctx, S.comm, na)) || (rc = ensure(ctx, S.fp, na)) || (rc = ensure(ctx, S.slot_of, na)) || (rc = ensure(ctx, S.dtab, (size_t)tab * 4)) ||
-        (rc = ensure(ctx, S.dmin, (size_t)tab * 4)) || (rc = ensure(ctx, S.list, na)) || (rc = ensure(ctx, S.acc, na)) ||
-        (rc = ensure(ctx, S.accepted_by, ctx->n_val * 4)) || (rc = ensure(ctx, S.incomm, n)) || (rc = ensure(ctx, S.tst, n)) ||
-        (rc = ensure(ctx, S.fbits, (size_t)n * bits_stride + 16)) || (rc = ensure(ctx, S.fav_ok, n)) || (rc = ensure(ctx, S.bucket, nc)) ||
-        (rc = ensure(ctx, S.cursor, nc)) || (rc = ensure(ctx, S.sorted, (size_t)ctx->n_blocks * 4)) || (rc = ensure(ctx, S.av_signer, 2 * na)) ||
-        (rc = ensure(ctx, S.av_off, 2 * na + 4)) || (rc = ensure(ctx, S.av_msg, (size_t)n * 64)) || (rc = ensure(ctx, S.av_sig, (size_t)n * 192)) ||
-        (rc = ensure(ctx, S.av_ok, 2 * (size_t)n)))
-        return rc;
     const tree_tables& t = ctx->tree;
-    intake_args T = {};
+    api_args A = {};
+    intake_args& T = A.T;
     T.n_att = n;
     T.off = d_off;
     T.n_committees = n_committees;
@@ -1504,14 +1495,8 @@ int b2_aggregate_and_proof_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64
     T.root = t.root;
     T.parent = t.parent;
     T.slot = t.slot;
-    T.sorted = S.sorted;
     T.n_blocks = ctx->n_blocks;
-    T.comm = S.comm;
-    T.bucket = S.bucket;
-    T.cursor = S.cursor;
-    T.list = S.list;
     T.guard = ctx->d_guard;
-    api_args A = {};
     A.wire = d_wire;
     A.wire_len = wire_len;
     A.woff = d_woff;
@@ -1525,23 +1510,7 @@ int b2_aggregate_and_proof_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64
     A.current_slot = current_slot;
     A.propagation_range = propagation_slot_range;
     A.n_val = ctx->n_val;
-    A.T = T;
-    A.fp = S.fp;
-    A.slot_of = S.slot_of;
-    A.dtab = S.dtab;
-    A.dmin = S.dmin;
-    A.acc = S.acc;
-    A.accepted_by = S.accepted_by;
     A.dtab_mask = tab - 1;
-    A.incomm = S.incomm;
-    A.tst = S.tst;
-    A.fbits = S.fbits;
-    A.av_signer = S.av_signer;
-    A.av_off = S.av_off;
-    A.av_msg = S.av_msg;
-    A.av_sig = S.av_sig;
-    A.fav_ok = S.fav_ok;
-    A.av_ok = S.av_ok;
     A.status = d_status_out;
     A.committee = d_committee_out;
     A.data_id = d_data_id_out;
@@ -1556,14 +1525,26 @@ int b2_aggregate_and_proof_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64
     memcpy(A.dom_sel.b, domains96 + 32, 32);
     memcpy(A.dom_aap.b, domains96 + 64, 32);
     A.guard = ctx->d_guard;
+    const size_t nc = (size_t)n_committees + 1;
+    uint8_t *fav_ok, *av_ok;      // written by the verify helpers, read by the kernels through A
+    uint32_t* sorted;             // written by k_intake_sorted, read through T.sorted
+    scratch sc(ctx, ctx->api);
+    sc(T.comm, n); sc(A.fp, n); sc(A.slot_of, n); sc(A.dtab, tab); sc(A.dmin, tab); sc(T.list, n); sc(A.acc, n); sc(A.accepted_by, ctx->n_val);
+    sc(A.incomm, n); sc(A.tst, n); sc(A.fbits, (size_t)n * bits_stride, 16); sc(fav_ok, n);
+    sc(T.bucket, nc); sc(T.cursor, nc); sc(sorted, ctx->n_blocks);
+    sc(A.av_signer, 2 * (size_t)n); sc(A.av_off, 2 * (size_t)n + 1); sc(A.av_msg, (size_t)n * 64); sc(A.av_sig, (size_t)n * 192); sc(av_ok, 2 * (size_t)n);
+    if (sc.rc) return sc.rc;
+    A.fav_ok = fav_ok;
+    A.av_ok = av_ok;
+    T.sorted = sorted;
     cudaStream_t s = (cudaStream_t)stream;
     CK(cudaStreamWaitEvent(s, ctx->ev_intake, 0));
-    k_intake_sorted<<<blocks_for(ctx->n_blocks, 256), 256, 0, s>>>(t.rank_id, ctx->n_blocks, S.sorted);
+    k_intake_sorted<<<blocks_for(ctx->n_blocks, 256), 256, 0, s>>>(t.rank_id, ctx->n_blocks, sorted);
     CKL(ctx);
-    CK(cudaMemsetAsync(S.bucket, 0, nc, s));
-    CK(cudaMemsetAsync(S.dtab, 0xff, (size_t)tab * 4, s));
-    CK(cudaMemsetAsync(S.dmin, 0xff, (size_t)tab * 4, s));
-    CK(cudaMemsetAsync(S.accepted_by, 0xff, ctx->n_val * 4, s));
+    CK(cudaMemsetAsync(T.bucket, 0, nc * 4, s));
+    CK(cudaMemsetAsync(A.dtab, 0xff, (size_t)tab * 4, s));
+    CK(cudaMemsetAsync(A.dmin, 0xff, (size_t)tab * 4, s));
+    CK(cudaMemsetAsync(A.accepted_by, 0xff, ctx->n_val * 4, s));
     k_api_parse<<<blocks_for((uint64_t)n * 32, 128), 128, 0, s>>>(A);
     CKL(ctx);
     k_api_data<<<blocks_for(n, 128), 128, 0, s>>>(A);
@@ -1573,10 +1554,10 @@ int b2_aggregate_and_proof_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64
     k_api_sets<<<blocks_for(n, 64), 64, 0, s>>>(A);
     CKL(ctx);
     // FastAggregateVerify of the aggregates over their member rows, then AggregateVerify of the 2n single-key sets
-    pk_source P = {d_members_out, d_item_off_out, (const uint8_t*)S.fbits, bits_stride, nullptr, 0};
-    if ((rc = verify_fork(ctx, ctx->slot[0], P, d_msg32_out, n, s)) || (rc = verify_main(ctx, ctx->slot[0], d_sig96_out, n, S.fav_ok, s))) return rc;
-    if ((rc = aggregate_verify_enqueue(ctx, S.av_signer, nullptr, S.av_msg, S.av_off, 2ull * n, S.av_sig, 2 * n, S.av_ok, s))) return rc;
-    k_intake_scan<<<1, 1024, 0, s>>>(S.bucket, n_committees, S.cursor);      // bucket[n_committees] = the candidates
+    pk_source P = {d_members_out, d_item_off_out, A.fbits, bits_stride, nullptr, 0};
+    if ((rc = verify_fork(ctx, ctx->slot[0], P, d_msg32_out, n, s)) || (rc = verify_main(ctx, ctx->slot[0], d_sig96_out, n, fav_ok, s))) return rc;
+    if ((rc = aggregate_verify_enqueue(ctx, A.av_signer, nullptr, A.av_msg, A.av_off, 2ull * n, A.av_sig, 2 * n, av_ok, s))) return rc;
+    k_intake_scan<<<1, 1024, 0, s>>>(T.bucket, n_committees, T.cursor);      // bucket[n_committees] = the candidates
     CKL(ctx);
     k_intake_scatter<<<blocks_for(n, 256), 256, 0, s>>>(T);
     CKL(ctx);
@@ -1668,13 +1649,7 @@ int b2_block_attestations_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_
         return rc;
     REQUIRE(n_sig < (1ull << 32), "block_attestations: n_sig does not fit 32 bits");      // the host form's n_sig is a u32 offset
     CK(cudaSetDevice(ctx->device));
-    ba_scratch& S = ctx->ba;
     const size_t n = n_att, W = 8ull * bits_stride;
-    if ((rc = ensure(ctx, S.blk_of, n * 4)) || (rc = ensure(ctx, S.cur, n)) || (rc = ensure(ctx, S.fav_ok, n)) || (rc = ensure(ctx, S.accept, 2 * n)) ||
-        (rc = ensure(ctx, S.num1, n * 8)) || (rc = ensure(ctx, S.bits, n * bits_stride + 16)) || (rc = ensure(ctx, S.sig96, n * 96)) ||
-        (rc = ensure(ctx, S.data128, n * 128)) || (rc = ensure(ctx, S.dom32, n * 32)) || (rc = ensure(ctx, S.msg32, n * 32)) ||
-        (rc = ensure(ctx, S.members, n * W * 4)) || (rc = ensure(ctx, S.item_off, (n + 1) * 4)))
-        return rc;
     ba_args A = {};
     A.wire = d_wire;
     A.wire_len = wire_len;
@@ -1697,17 +1672,6 @@ int b2_block_attestations_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_
     memcpy(A.justified.b, justified80, 80);
     memcpy(A.dom[0].b, domains64, 32);
     memcpy(A.dom[1].b, domains64 + 32, 32);
-    A.blk_of = S.blk_of;
-    A.cur = S.cur;
-    A.fav_ok = S.fav_ok;
-    A.accept = S.accept;
-    A.num1 = S.num1;
-    A.bits = S.bits;
-    A.sig96 = S.sig96;
-    A.data128 = S.data128;
-    A.dom32 = S.dom32;
-    A.members_out = S.members;
-    A.item_off = S.item_off;
     A.status = d_status_out;
     A.flag_mask = d_flag_mask_out;
     A.numerator = (unsigned long long*)d_numerator_out;
@@ -1716,27 +1680,32 @@ int b2_block_attestations_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_
     A.block_reward = (unsigned long long*)d_block_reward_out;
     A.n_applied = d_n_applied_out;
     A.guard = ctx->d_guard;
+    uint8_t* msg32;
+    scratch sc(ctx, ctx->ba);
+    sc(A.blk_of, n); sc(A.cur, n); sc(A.fav_ok, n); sc(A.accept, 2 * n); sc(A.num1, n); sc(A.bits, n * bits_stride, 16);
+    sc(A.sig96, n * 96); sc(A.data128, n * 128); sc(A.dom32, n * 32); sc(msg32, n * 32); sc(A.members_out, n * W); sc(A.item_off, n + 1);
+    if (sc.rc) return sc.rc;
     cudaStream_t s = (cudaStream_t)stream;
     k_ba_parse<<<blocks_for((uint64_t)n_att * 32, 128), 128, 0, s>>>(A);
     CKL(ctx);
-    k_signing_roots<<<blocks_for(n_att, 64), 64, 0, s>>>(S.data128, S.dom32, 32u, n_att, S.msg32);
+    k_signing_roots<<<blocks_for(n_att, 64), 64, 0, s>>>(A.data128, A.dom32, 32u, n_att, msg32);
     CKL(ctx);
-    pk_source P = {S.members, S.item_off, (const uint8_t*)S.bits, bits_stride, nullptr, 0};
-    if ((rc = verify_fork(ctx, ctx->slot[0], P, S.msg32, n_att, s)) || (rc = verify_main(ctx, ctx->slot[0], S.sig96, n_att, S.fav_ok, s))) return rc;
+    pk_source P = {A.members_out, A.item_off, A.bits, bits_stride, nullptr, 0};
+    if ((rc = verify_fork(ctx, ctx->slot[0], P, msg32, n_att, s)) || (rc = verify_main(ctx, ctx->slot[0], A.sig96, n_att, A.fav_ok, s))) return rc;
     k_ba_blocks<<<1, BA_BLOCKS_THREADS, 0, s>>>(A);
     CKL(ctx);
     // the flag scatter of :745-749, order-exact over (block, list) order: table 0 (target e) writes `numerator`, table 1 (target e - 1) num1
     const registry_tables& R = ctx->reg;
-    const uint8_t* db = S.bits;
+    const uint8_t* db = A.bits;
     for (int which = 0; which < 2; which++) {
-        const uint8_t* acc = (const uint8_t*)S.accept.p + (size_t)which * n;
-        unsigned long long* num = which == 0 ? (unsigned long long*)d_numerator_out : (unsigned long long*)S.num1.p;
-        k_part_phase1<<<n_att, 128, 0, s>>>(S.members, S.item_off, db, bits_stride, d_flag_mask_out, acc, n_att, R.part[which], R.part_first);
+        const uint8_t* acc = A.accept + (size_t)which * n;
+        unsigned long long* num = which == 0 ? (unsigned long long*)d_numerator_out : A.num1;
+        k_part_phase1<<<n_att, 128, 0, s>>>(A.members_out, A.item_off, db, bits_stride, d_flag_mask_out, acc, n_att, R.part[which], R.part_first);
         CKL(ctx);
-        k_part_phase2<<<n_att, 128, 0, s>>>(S.members, S.item_off, db, bits_stride, d_flag_mask_out, acc, n_att, R.part_first, R.eff,
+        k_part_phase2<<<n_att, 128, 0, s>>>(A.members_out, A.item_off, db, bits_stride, d_flag_mask_out, acc, n_att, R.part_first, R.eff,
                                             effective_balance_increment, base_reward_per_increment, num);
         CKL(ctx);
-        k_part_phase3<<<n_att, 128, 0, s>>>(S.members, S.item_off, db, bits_stride, d_flag_mask_out, acc, n_att, R.part_first, R.part[which]);
+        k_part_phase3<<<n_att, 128, 0, s>>>(A.members_out, A.item_off, db, bits_stride, d_flag_mask_out, acc, n_att, R.part_first, R.part[which]);
         CKL(ctx);
     }
     k_ba_rewards<<<blocks_for((uint64_t)n_blocks * 32, 128), 128, 0, s>>>(A);
@@ -1819,21 +1788,10 @@ int b2_sync_committee_messages_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t 
                                             d_agg_sig96_out)))
         return rc;
     CK(cudaSetDevice(ctx->device));
-    scm_scratch& S = ctx->scm;
     const uint32_t sub = committee_size / subnet_count;
     const uint64_t nc = (uint64_t)n * subnet_count;
     uint32_t tab = 1;
     while (tab < 2 * n) tab <<= 1;
-    const size_t na = (size_t)n * 4, np = (size_t)committee_size * 4;
-    if ((rc = ensure(ctx, S.keys, (size_t)committee_size * 8)) || (rc = ensure(ctx, S.canon, na)) || (rc = ensure(ctx, S.first, np)) ||
-        (rc = ensure(ctx, S.pitem, np)) || (rc = ensure(ctx, S.proot, np)) || (rc = ensure(ctx, S.signer, na)) || (rc = ensure(ctx, S.pair_off, na + 4)) ||
-        (rc = ensure(ctx, S.msg, (size_t)n * 32)) || (rc = ensure(ctx, S.sig, (size_t)n * 96)) || (rc = ensure(ctx, S.ok, n)) ||
-        (rc = ensure(ctx, S.slot_of, na)) || (rc = ensure(ctx, S.rtab, (size_t)tab * 4)) || (rc = ensure(ctx, S.rmin, (size_t)tab * 4)) ||
-        (rc = ensure(ctx, S.rid, na)) || (rc = ensure(ctx, S.seg_off, (nc + 1) * 4)) || (rc = ensure(ctx, S.agg_off, na + 4)) ||
-        (rc = ensure(ctx, S.gsrc, np)) || (rc = ensure(ctx, S.aff, (size_t)n * 192 + 16)) || (rc = ensure(ctx, S.st, n + 16)) ||
-        (rc = ensure(ctx, S.gaff, (size_t)committee_size * 192 + 16)) || (rc = ensure(ctx, S.gst, committee_size + 16)) ||
-        (rc = ensure(ctx, S.sumjac, (nc + n) * 288)) || (rc = ensure(ctx, S.seg_status, (nc + n) * 4)))
-        return rc;
     scm_args A = {};
     A.wire = d_wire;
     A.wire_len = wire_len;
@@ -1849,24 +1807,7 @@ int b2_sync_committee_messages_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t 
     A.current_slot = current_slot;
     A.n_val = ctx->n_val;
     memcpy(A.dom.b, domain32, 32);
-    A.keys = S.keys;
-    A.canon = S.canon;
-    A.first = S.first;
-    A.pitem = S.pitem;
-    A.proot = S.proot;
-    A.signer = S.signer;
-    A.pair_off = S.pair_off;
-    A.msg = S.msg;
-    A.sig = S.sig;
-    A.ok = S.ok;
-    A.slot_of = S.slot_of;
-    A.rtab = S.rtab;
-    A.rmin = S.rmin;
-    A.rid = S.rid;
     A.rtab_mask = tab - 1;
-    A.seg_off = S.seg_off;
-    A.agg_off = S.agg_off;
-    A.gsrc = S.gsrc;
     A.status = d_status_out;
     A.root_id = d_root_id_out;
     A.n_roots = d_n_roots_out;
@@ -1875,15 +1816,27 @@ int b2_sync_committee_messages_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t 
     A.cpresent = d_contrib_present_out;
     A.abits = d_agg_bits_out;
     A.guard = ctx->d_guard;
+    // the AggregateVerify verdicts (read by the kernels through A.ok); the decompressed item signatures, the gathered ones and the segment sums
+    uint8_t *ok, *st, *gst;
+    uint32_t *aff, *gaff, *sumjac;
+    int32_t* segst;
+    scratch sc(ctx, ctx->scm);
+    sc(A.keys, committee_size); sc(A.canon, n); sc(A.first, committee_size); sc(A.pitem, committee_size); sc(A.proot, committee_size);
+    sc(A.signer, n); sc(A.pair_off, (size_t)n + 1); sc(A.msg, (size_t)n * 32); sc(A.sig, (size_t)n * 96); sc(ok, n);
+    sc(A.slot_of, n); sc(A.rtab, tab); sc(A.rmin, tab); sc(A.rid, n); sc(A.seg_off, nc + 1); sc(A.agg_off, (size_t)n + 1); sc(A.gsrc, committee_size);
+    sc(aff, (size_t)n * 48, 16); sc(st, n, 16); sc(gaff, (size_t)committee_size * 48, 16); sc(gst, committee_size, 16);
+    sc(sumjac, (nc + n) * 72); sc(segst, nc + n);
+    if (sc.rc) return sc.rc;
+    A.ok = ok;
     cudaStream_t s = (cudaStream_t)stream;
-    CK(cudaMemsetAsync(S.first, 0xff, np, s));
-    CK(cudaMemsetAsync(S.rtab, 0xff, (size_t)tab * 4, s));
-    CK(cudaMemsetAsync(S.rmin, 0xff, (size_t)tab * 4, s));
+    CK(cudaMemsetAsync(A.first, 0xff, (size_t)committee_size * 4, s));
+    CK(cudaMemsetAsync(A.rtab, 0xff, (size_t)tab * 4, s));
+    CK(cudaMemsetAsync(A.rmin, 0xff, (size_t)tab * 4, s));
     k_scm_index<<<1, 1024, 0, s>>>(A);
     CKL(ctx);
     k_scm_parse<<<blocks_for(n, 128), 128, 0, s>>>(A);
     CKL(ctx);
-    if ((rc = aggregate_verify_enqueue(ctx, S.signer, nullptr, S.msg, S.pair_off, n, S.sig, n, S.ok, s))) return rc;
+    if ((rc = aggregate_verify_enqueue(ctx, A.signer, nullptr, A.msg, A.pair_off, n, A.sig, n, ok, s))) return rc;
     k_scm_first<<<blocks_for(n, 128), 128, 0, s>>>(A);
     CKL(ctx);
     k_scm_accept<<<blocks_for(n, 128), 128, 0, s>>>(A);
@@ -1894,21 +1847,19 @@ int b2_sync_committee_messages_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t 
     CKL(ctx);
     k_scm_rows<<<blocks_for(nc + n, 128), 128, 0, s>>>(A);
     CKL(ctx);
-    k_intake_scan<<<1, 1024, 0, s>>>(S.seg_off, (uint32_t)nc, nullptr);      // seg_off[nc] = the set positions of every root
+    k_intake_scan<<<1, 1024, 0, s>>>(A.seg_off, (uint32_t)nc, nullptr);     // seg_off[nc] = the set positions of every root
     CKL(ctx);
     k_scm_gather<<<blocks_for(std::max<uint64_t>(committee_size, (uint64_t)n + 1), 128), 128, 0, s>>>(A);
     CKL(ctx);
     // bls.Aggregate of each contribution's and each root's signatures: the item signatures decompressed once (an item that was not
     // accepted holds zero bytes and is never gathered), gathered per set position, one segment per (root, subnet) and one per root
-    k_g2_decompress<<<blocks_for(n, ctx->dec_block), ctx->dec_block, 0, s>>>(S.sig, n, S.aff, S.st);
+    k_g2_decompress<<<blocks_for(n, ctx->dec_block), ctx->dec_block, 0, s>>>(A.sig, n, aff, st);
     CKL(ctx);
-    k_pack_gather<<<blocks_for(committee_size, 128), 128, 0, s>>>(S.aff, S.st, S.gsrc, (const uint32_t*)S.seg_off + nc, S.gaff, S.gst);
+    k_pack_gather<<<blocks_for(committee_size, 128), 128, 0, s>>>(aff, st, A.gsrc, A.seg_off + nc, gaff, gst);
     CKL(ctx);
-    uint32_t* sumjac = S.sumjac;
-    int32_t* segst = S.seg_status;
-    k_g2_segment_sum<<<(unsigned)nc, 32, 0, s>>>(S.gaff, S.gst, S.seg_off, (uint32_t)nc, sumjac, segst, committee_size, ctx->d_guard);
+    k_g2_segment_sum<<<(unsigned)nc, 32, 0, s>>>(gaff, gst, A.seg_off, (uint32_t)nc, sumjac, segst, committee_size, ctx->d_guard);
     CKL(ctx);
-    k_g2_segment_sum<<<n, 32, 0, s>>>(S.gaff, S.gst, S.agg_off, n, sumjac + 72 * nc, segst + nc, committee_size, ctx->d_guard);
+    k_g2_segment_sum<<<n, 32, 0, s>>>(gaff, gst, A.agg_off, n, sumjac + 72 * nc, segst + nc, committee_size, ctx->d_guard);
     CKL(ctx);
     k_g2_finish<<<blocks_for(nc, 32), 32, 0, s>>>(sumjac, segst, (uint32_t)nc, d_contrib_sig96_out, nullptr, nullptr);
     CKL(ctx);
@@ -2450,29 +2401,48 @@ int b2_pack_attestations_dev(b2_ctx* ctx, const uint32_t* d_members, const uint3
         return rc;
     CK(cudaSetDevice(ctx->device));
     cudaStream_t s = (cudaStream_t)stream;
-    pack_scratch& S = ctx->pk;
     const size_t C = std::max<uint32_t>(n_cand, 1), K = n_committees, M = max_out, wstride = (bits_stride + 3) / 4;
     const size_t claim_words = 2 * ((ctx->n_val + 31) / 32);
-    if ((rc = ensure(ctx, S.cnt, K * 4)) || (rc = ensure(ctx, S.off, (K + 1) * 4)) || (rc = ensure(ctx, S.list, C * 4)) || (rc = ensure(ctx, S.fold_of, C * 4)) ||
-        (rc = ensure(ctx, S.fdata, C * 4)) || (rc = ensure(ctx, S.fcnt, C * 4)) || (rc = ensure(ctx, S.frow, C * wstride * 4)) || (rc = ensure(ctx, S.fmask, C)) ||
-        (rc = ensure(ctx, S.egain, C * 8)) || (rc = ensure(ctx, S.eslot, C * 4)) || (rc = ensure(ctx, S.claim, claim_words * 4)) ||
-        (rc = ensure(ctx, S.dcomm, C * 4)) || (rc = ensure(ctx, S.dmask, C * 4)) || (rc = ensure(ctx, S.ctl, 16)) || (rc = ensure(ctx, S.sel, M * 4)) ||
-        (rc = ensure(ctx, S.ord, M * 4)) || (rc = ensure(ctx, S.aff, C * 192 + 16)) || (rc = ensure(ctx, S.st, C + 16)) || (rc = ensure(ctx, S.gaff, C * 192 + 16)) ||
-        (rc = ensure(ctx, S.gst, C + 16)) || (rc = ensure(ctx, S.sumjac, M * 288)) || (rc = ensure(ctx, S.seg_status, M * 4)))
-        return rc;
     const registry_tables& R = ctx->reg;
-    pack_view P = {d_members, d_committee_off, d_committee_table, d_cand_committee, d_cand_data, d_cand_flag_mask, d_bits, S.st, R.eff,
-                   {R.part[0], R.part[1]}, n_committees, n_cand, bits_stride, (uint32_t)wstride, max_out, ctx->n_val, effective_balance_increment,
-                   base_reward_per_increment, S.cnt, S.off, S.list, S.fold_of, S.fdata, S.fcnt, S.frow, S.fmask, S.egain, S.eslot, S.claim, S.dcomm,
-                   S.dmask, S.ctl, S.sel, S.ord, d_cand_status, ctx->d_guard};
-    CK(cudaMemsetAsync(S.ctl, 0, 16, s));
-    CK(cudaMemsetAsync(S.claim, 0, claim_words * 4, s));
-    if (K) CK(cudaMemsetAsync(S.cnt, 0, K * 4, s));
+    pack_view P = {};
+    P.members = d_members;
+    P.coff = d_committee_off;
+    P.ctable = d_committee_table;
+    P.cand_comm = d_cand_committee;
+    P.cand_data = d_cand_data;
+    P.cand_mask = d_cand_flag_mask;
+    P.bits = d_bits;
+    P.eff = R.eff;
+    P.part[0] = R.part[0];
+    P.part[1] = R.part[1];
+    P.n_comm = n_committees;
+    P.n_cand = n_cand;
+    P.stride = bits_stride;
+    P.wstride = (uint32_t)wstride;
+    P.max_out = max_out;
+    P.n_val = ctx->n_val;
+    P.inc = effective_balance_increment;
+    P.per_inc = base_reward_per_increment;
+    P.cand_status = d_cand_status;
+    P.guard = ctx->d_guard;
+    // the decompressed candidate signatures (read by the kernels through P.dec_st), the gathered constituents and their segment sums
+    uint8_t *st, *gst;
+    uint32_t *aff, *gaff, *sumjac;
+    int32_t* segst;
+    scratch sc(ctx, ctx->pk);
+    sc(P.cnt, K); sc(P.off, K + 1); sc(P.list, C); sc(P.fold_of, C); sc(P.fdata, C); sc(P.fcnt, C); sc(P.frow, C * wstride); sc(P.fmask, C);
+    sc(P.egain, C); sc(P.eslot, C); sc(P.claim, claim_words); sc(P.dcomm, C); sc(P.dmask, C); sc(P.ctl, 4); sc(P.sel, M); sc(P.ord, M);
+    sc(aff, C * 48, 16); sc(st, C, 16); sc(gaff, C * 48, 16); sc(gst, C, 16); sc(sumjac, M * 72); sc(segst, M);
+    if (sc.rc) return sc.rc;
+    P.dec_st = st;
+    CK(cudaMemsetAsync(P.ctl, 0, 16, s));
+    CK(cudaMemsetAsync(P.claim, 0, claim_words * 4, s));
+    if (K) CK(cudaMemsetAsync(P.cnt, 0, K * 4, s));
     if (n_cand) {
-        CK(cudaMemsetAsync(S.dcomm, 0xff, (size_t)n_cand * 4, s));
-        CK(cudaMemsetAsync(S.dmask, 0xff, (size_t)n_cand * 4, s));
+        CK(cudaMemsetAsync(P.dcomm, 0xff, (size_t)n_cand * 4, s));
+        CK(cudaMemsetAsync(P.dmask, 0xff, (size_t)n_cand * 4, s));
         CK(cudaMemsetAsync(d_out_src, 0, (size_t)n_cand * 4, s));
-        k_g2_decompress<<<blocks_for(n_cand, ctx->dec_block), ctx->dec_block, 0, s>>>(d_sig96, n_cand, S.aff, S.st);
+        k_g2_decompress<<<blocks_for(n_cand, ctx->dec_block), ctx->dec_block, 0, s>>>(d_sig96, n_cand, aff, st);
         CKL(ctx);
     }
     if (K) {
@@ -2502,12 +2472,12 @@ int b2_pack_attestations_dev(b2_ctx* ctx, const uint32_t* d_members, const uint3
     k_pack_emit<<<max_out, 128, 0, s>>>(P, d_out_src_off, d_out_committee, d_out_data, d_out_bits, (unsigned long long*)d_out_numerator, d_out_src);
     CKL(ctx);
     if (n_cand) {
-        k_pack_gather<<<blocks_for(n_cand, 128), 128, 0, s>>>(S.aff, S.st, d_out_src, d_out_src_off + max_out, S.gaff, S.gst);
+        k_pack_gather<<<blocks_for(n_cand, 128), 128, 0, s>>>(aff, st, d_out_src, d_out_src_off + max_out, gaff, gst);
         CKL(ctx);
     }
-    k_g2_segment_sum<<<max_out, 32, 0, s>>>(S.gaff, S.gst, d_out_src_off, max_out, S.sumjac, S.seg_status, n_cand, ctx->d_guard);
+    k_g2_segment_sum<<<max_out, 32, 0, s>>>(gaff, gst, d_out_src_off, max_out, sumjac, segst, n_cand, ctx->d_guard);
     CKL(ctx);
-    k_g2_finish<<<blocks_for(max_out, 32), 32, 0, s>>>(S.sumjac, S.seg_status, max_out, d_out_sig96, nullptr, nullptr);
+    k_g2_finish<<<blocks_for(max_out, 32), 32, 0, s>>>(sumjac, segst, max_out, d_out_sig96, nullptr, nullptr);
     CKL(ctx);
     if (n_cand) {
         k_pack_single<<<blocks_for(max_out, 128), 128, 0, s>>>(d_sig96, d_out_src_off, d_out_src, max_out, d_out_sig96);

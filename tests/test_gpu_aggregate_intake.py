@@ -179,10 +179,14 @@ def test_every_status_against_oracle(env):
     wires, ok = _scenario(env)
     o = _oracle(members, off, wires, ok)
     assert set(o.status.tolist()) == set(range(21)), sorted(set(range(21)) - set(o.status.tolist()))
+    few = _oracle(members, off, wires[:3], ok[:3])
+    _same(_dev_call(eng, members, off, wires[:3])[0], few)
     r = _host_call(eng, members, off, wires)
     _same(r, o)
     rd, _ = _dev_call(eng, members, off, wires)
     _same(rd, o)
+    # the short list again, on the scratch the full one grew
+    _same(_dev_call(eng, members, off, wires[:3])[0], few)
     assert eng.guard_flags() == 0
 
 

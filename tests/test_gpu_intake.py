@@ -151,10 +151,14 @@ def test_every_status_and_output_matches_oracle(eng):
     cur = EPOCH * SPE + 7
     want = _oracle(wires, off, tree, current_slot=cur)
     assert set(want.status.tolist()) == set(range(14)), sorted(set(want.status.tolist()))
+    few = _oracle(wires[:3], off, tree, current_slot=cur)
+    _assert_equal(_dev(eng, wires[:3], off, EPOCH, cur, 64), few, 64)
     wire, woff = _wire(wires)
     got = eng.attestation_intake(wire, woff, off, EPOCH, cur, DOMAIN, CPS, SPE, 1, 64)
     _assert_equal(got, want, 64)
     _assert_equal(_dev(eng, wires, off, EPOCH, cur, 64), want, 64)
+    # the short list again, on the scratch the full one grew
+    _assert_equal(_dev(eng, wires[:3], off, EPOCH, cur, 64), few, 64)
     assert eng.guard_flags() == 0
 
 

@@ -131,10 +131,18 @@ def test_three_roots(minimal):
     wires, subnets = [wires[a] for a in order], [subnets[a] for a in order]
     want = M.validate(wires, subnets, cur, N_VAL, lambda v: pks[v], SLOT, domain)
     assert want.roots[0] == ROOT_C and len(want.roots) == 3
+    few = _dev(eng, wires[:4], subnets[:4], cur, SLOT, domain)
     host, dev = _run_both(eng, wires, subnets, cur, SLOT, domain)
     w = _expect_arrays(want, len(wires), 32)
     _assert_equal(host, w)
     _assert_equal(dev, w)
+    # a short list, the full one and the short one again on one engine: the same outputs as on a fresh engine
+    fresh = Engine(0)
+    fresh.registry_load(np.frombuffer(b"".join(pks), np.uint8).reshape(-1, 48), np.full(N_VAL, 32 * 10**9, np.uint64))
+    want_few = _dev(fresh, wires[:4], subnets[:4], cur, SLOT, domain)
+    fresh.close()
+    _assert_equal(few, want_few)
+    _assert_equal(_dev(eng, wires[:4], subnets[:4], cur, SLOT, domain), want_few)
     eng.sync_committee_load(np.frombuffer(b"".join(state.current_sync_committee.pubkeys), np.uint8).reshape(-1, 48), 32)
     msgs = np.frombuffer(b"".join(M.signing_root(r, domain) for r in want.roots), np.uint8).reshape(-1, 32)
     assert eng.sync_aggregate_verify(np.zeros(3, np.uint32), host.agg_bits, msgs, host.agg_sigs).tolist() == [1, 1, 1]
