@@ -638,6 +638,61 @@ int b2_sync_committee_messages(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_l
                                const uint8_t* domain32, int32_t* status_out, uint32_t* root_id_out, uint8_t* roots32_out, uint32_t* n_roots_out,
                                uint8_t* contrib_bits_out, uint8_t* contrib_sig96_out, uint8_t* contrib_present_out, uint8_t* agg_bits_out,
                                uint8_t* agg_sig96_out);
+/* ---- One slot of sync committee contributions from gossip: SignedContributionAndProof checked as the sync_committee_contribution_and_proof
+ * topic of the upstream Altair p2p spec requires, and per beacon_block_root the SyncAggregate process_sync_committee_contributions (upstream
+ * Altair validator spec) builds from the best accepted contribution of each subnet.  Inputs:
+ *   wire, woff[n+1], wire_len     the items' SSZ encodings back to back, 344 + ceil(sub / 8) bytes each (every field is fixed-size):
+ *                                 ContributionAndProof (aggregator_index u64 | SyncCommitteeContribution (slot u64 | beacon_block_root 32 |
+ *                                 subcommittee_index u64 | aggregation_bits Bitvector[sub] | signature 96) | selection_proof 96) | signature 96
+ *   position_validator[committee_size]   the registry index of each position of the sync committee, as for b2_sync_committee_messages
+ *   committee_size, subnet_count  sub = committee_size / subnet_count; subnet s holds positions [s * sub, (s + 1) * sub)
+ *   current_slot
+ *   domains96 (host)              get_domain of current_slot's epoch for DOMAIN_SYNC_COMMITTEE, DOMAIN_SYNC_COMMITTEE_SELECTION_PROOF and
+ *                                 DOMAIN_CONTRIBUTION_AND_PROOF, back to back
+ *   target_aggregators            TARGET_AGGREGATORS_PER_SYNC_SUBCOMMITTEE (> 0)
+ * Each item gets the first check it fails (IGNORE or REJECT as the p2p spec classes it):
+ *    0  accepted
+ *    1  REJECT  not 344 + ceil(sub / 8) bytes, a Bitvector bit at or past sub set, or a woff row that is reversed or ends past wire_len
+ *    2  IGNORE  contribution.slot != current_slot (clock disparity is the caller's)
+ *    3  REJECT  subcommittee_index >= subnet_count
+ *    4  REJECT  no aggregation bit set
+ *    5  REJECT  is_sync_committee_aggregator is false: bytes_to_uint64(hash(selection_proof)[0:8]) % max(1, sub // target_aggregators) != 0
+ *    6  REJECT  aggregator_index >= n_validators
+ *    7  REJECT  aggregator_index holds no position of subnet subcommittee_index (registry indices compared)
+ *    8  IGNORE  an earlier ACCEPTED item has the same (beacon_block_root, subcommittee_index) and bits that include this item's
+ *    9  IGNORE  an earlier ACCEPTED item has the same (aggregator_index, subcommittee_index), on any root
+ *   10  REJECT  the selection proof fails Verify(key(aggregator), compute_signing_root(SyncAggregatorSelectionData(slot, subcommittee_index),
+ *               selection domain))
+ *   11  REJECT  the signature fails Verify(key(aggregator), compute_signing_root(ContributionAndProof, contribution_and_proof domain))
+ *   12  REJECT  the contribution's signature fails FastAggregateVerify over the registry keys of the set positions of its subnet (a validator
+ *               at k positions counts k times) and compute_signing_root(beacon_block_root, sync committee domain)
+ * A key that failed KeyValidate fails 10, 11 or 12.  Checks 8 and 9 read only earlier items of the same call that end with status 0: each
+ * item gets the status it would get if the items arrived one by one in list order at a node whose seen-caches were empty when the call
+ * began (the caller keeps the caches across calls).
+ * Outputs (n items): status i32[n]; root_id u32[n], the accepted items' distinct roots numbered by first accepted occurrence, 0xFFFFFFFF for
+ * the others; roots32 u8[n][32] and n_roots u32[1] (rows >= n_roots are zero); best u32[n][subnet_count], per (root, subnet) the list index
+ * of the accepted item with the most set bits (ties to the smaller index), 0xFFFFFFFF where there is none; agg_bits u8[n][ceil(committee_size
+ * / 8)] and agg_sig96 u8[n][96], per root the SyncAggregate of its best contributions (bit s * sub + i = bit i of best[r][s]'s row, signature
+ * bls.Aggregate of their signatures): what a proposer includes, and what b2_sync_aggregate_verify accepts.  Rows of roots >= n_roots are
+ * zero.  The accepted contributions themselves are the caller's wire bytes.
+ * b2_sync_contribution_and_proof_intake_dev is asynchronous on `stream` and self-guarding: a reversed woff row or one past wire_len is status
+ * 1 (B2_GUARD_BAD_ROW), and a position_validator entry >= n_validators matches nothing (B2_GUARD_BAD_INDEX); nothing is read or written out
+ * of bounds.  It needs the registry (not b2_sync_committee_load's tables) and shares the AggregateVerify buffers and the verify buffers of
+ * pipeline slot 0 with b2_aggregate_verify[_pks, _dev], b2_fast_aggregate_verify[_pks, _dev], b2_epoch_dev and the intakes: enqueue those and
+ * this call on one stream.  b2_set_verify_mode applies to its FastAggregateVerify.  The registry must not change while a call is in flight.
+ * b2_sync_contribution_and_proof_intake takes host arrays and returns when done; a rejected call (B2_EINVAL: a woff that does not start at 0,
+ * decreases or ends past the wire, a position_validator entry >= n_validators, committee_size not a multiple of subnet_count or above 1024,
+ * target_aggregators == 0, no registry, n == 0 or n >= 2^24) writes no output and changes nothing. */
+int b2_sync_contribution_and_proof_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n,
+                                              const uint32_t* d_position_validator, uint32_t committee_size, uint32_t subnet_count,
+                                              uint64_t current_slot, const uint8_t* domains96, uint32_t target_aggregators, int32_t* d_status_out,
+                                              uint32_t* d_root_id_out, uint8_t* d_roots32_out, uint32_t* d_n_roots_out, uint32_t* d_best_out,
+                                              uint8_t* d_agg_bits_out, uint8_t* d_agg_sig96_out, void* stream);
+int b2_sync_contribution_and_proof_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n,
+                                          const uint32_t* position_validator, uint32_t committee_size, uint32_t subnet_count, uint64_t current_slot,
+                                          const uint8_t* domains96, uint32_t target_aggregators, int32_t* status_out, uint32_t* root_id_out,
+                                          uint8_t* roots32_out, uint32_t* n_roots_out, uint32_t* best_out, uint8_t* agg_bits_out,
+                                          uint8_t* agg_sig96_out);
 int b2_latest_messages_update_dev(b2_ctx* ctx, const uint32_t* d_members, const uint32_t* d_off, const uint8_t* d_bits,
                                   uint32_t bits_stride, const uint64_t* d_target_epoch, const uint32_t* d_block_idx,
                                   const uint8_t* d_accept, uint32_t n_agg, void* stream);

@@ -124,6 +124,12 @@ SIGNATURES = {
                                                c_void_p] + [c_void_p] * 10),
     "b2_sync_committee_messages": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_uint32, c_uint64,
                                            c_void_p] + [c_void_p] * 9),
+    # ctx, wire, wire_len, woff, n, position_validator, committee_size, subnet_count, current_slot, domains96, target_aggregators, seven
+    # outputs[, stream]
+    "b2_sync_contribution_and_proof_intake_dev": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_uint32, c_uint32, c_uint64,
+                                                          c_void_p, c_uint32] + [c_void_p] * 8),
+    "b2_sync_contribution_and_proof_intake": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_uint32, c_uint32, c_uint64,
+                                                      c_void_p, c_uint32] + [c_void_p] * 7),
     "b2_vote_weights_dev": (c_int, [c_void_p, c_void_p, c_void_p]),
     "b2_vote_weights_range_dev": (c_int, [c_void_p, c_uint64, c_uint64, c_void_p, c_void_p]),
     "b2_guard_flags": (c_int, [c_void_p, c_void_p]),

@@ -25,6 +25,7 @@
 #include "aggintake.cuh"
 #include "blockatt.cuh"
 #include "syncmsg.cuh"
+#include "synccontrib.cuh"
 
 using namespace b2;
 
@@ -194,8 +195,8 @@ struct b2_ctx {
     slasher_tables sl;
     ssz_tables ssz;
     // per-call scratch (struct scratch) of the attestation and aggregated-attestation intakes, block attestations, sync committee
-    // messages and block packing
-    std::vector<dbuf> in, api, ba, scm, pk;
+    // messages, sync committee contributions and block packing
+    std::vector<dbuf> in, api, ba, scm, scc, pk;
 };
 
 struct nvtx_scope {
@@ -1901,6 +1902,163 @@ int b2_sync_committee_messages(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_l
     if (st.rc) return st.rc;
     if ((rc = b2_sync_committee_messages_dev(ctx, dwire, wire_len, dwoff, n, dsub, dpv, committee_size, subnet_count, current_slot, domain32, dst, drid,
                                              droots, dnr, dcb, dcs, dcp, dab, das, ctx->s_main)))
+        return rc;
+    return st.finish();
+}
+
+// ------------------------------------------------------------------------------------------ sync committee contributions (synccontrib.cuh)
+// SignedContributionAndProof through the sync_committee_contribution_and_proof checks of the upstream Altair p2p spec, and each root's best
+// contribution per subnet into its SyncAggregate (process_sync_committee_contributions, upstream Altair validator spec).  The signature checks
+// share the AggregateVerify buffers and pipeline slot 0's verify buffers with the synchronous verify calls and the intakes: one stream for all.
+static int check_sync_contribution_and_proof_intake(b2_ctx* ctx, const void* wire, const void* woff, uint32_t n, const void* position_validator,
+                                                    uint32_t committee_size, uint32_t subnet_count, const void* domains96, uint32_t target_aggregators,
+                                                    const void* status_out, const void* root_id_out, const void* roots32_out, const void* n_roots_out,
+                                                    const void* best_out, const void* agg_bits_out, const void* agg_sig96_out) {
+    REQUIRE(ctx && wire && woff && position_validator && domains96 && status_out && root_id_out && roots32_out && n_roots_out && best_out &&
+                agg_bits_out && agg_sig96_out && n > 0 && n < (1u << 24) && committee_size > 0 && subnet_count > 0 &&
+                (uint64_t)n * (subnet_count + 1) < (1ull << 31),
+            "sync_contribution_and_proof_intake: bad arguments");
+    REQUIRE(committee_size % subnet_count == 0, "sync_contribution_and_proof_intake: committee_size must be a multiple of subnet_count");
+    REQUIRE(committee_size <= B2_SYNC_MAX_SIZE, "sync_contribution_and_proof_intake: committee_size above the kernels' limit (1024)");
+    REQUIRE(target_aggregators > 0, "sync_contribution_and_proof_intake: target_aggregators must be positive");
+    return ctx->n_val > 0 ? B2_OK : reject(ctx, "sync_contribution_and_proof_intake", "registry not loaded");
+}
+int b2_sync_contribution_and_proof_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n,
+                                              const uint32_t* d_position_validator, uint32_t committee_size, uint32_t subnet_count,
+                                              uint64_t current_slot, const uint8_t* domains96, uint32_t target_aggregators, int32_t* d_status_out,
+                                              uint32_t* d_root_id_out, uint8_t* d_roots32_out, uint32_t* d_n_roots_out, uint32_t* d_best_out,
+                                              uint8_t* d_agg_bits_out, uint8_t* d_agg_sig96_out, void* stream) {
+    B2_NVTX;
+    int rc;
+    if ((rc = check_sync_contribution_and_proof_intake(ctx, d_wire, d_woff, n, d_position_validator, committee_size, subnet_count, domains96,
+                                                       target_aggregators, d_status_out, d_root_id_out, d_roots32_out, d_n_roots_out, d_best_out,
+                                                       d_agg_bits_out, d_agg_sig96_out)))
+        return rc;
+    CK(cudaSetDevice(ctx->device));
+    const uint32_t sub = committee_size / subnet_count, sb = (sub + 7) / 8;
+    const uint64_t nc = (uint64_t)n * subnet_count;
+    uint32_t tab = 1;
+    while (tab < 2 * n) tab <<= 1;
+    scc_args A = {};
+    A.wire = d_wire;
+    A.wire_len = wire_len;
+    A.woff = d_woff;
+    A.n = n;
+    A.size = committee_size;
+    A.subnets = subnet_count;
+    A.sub = sub;
+    A.sb = sb;
+    A.sw = (sb + 3) / 4;
+    A.ab = (committee_size + 7) / 8;
+    A.target = target_aggregators;
+    A.current_slot = current_slot;
+    A.n_val = ctx->n_val;
+    memcpy(A.dom_sync.b, domains96, 32);
+    memcpy(A.dom_sel.b, domains96 + 32, 32);
+    memcpy(A.dom_cap.b, domains96 + 64, 32);
+    A.rtab_mask = tab - 1;
+    A.status = d_status_out;
+    A.root_id = d_root_id_out;
+    A.best = d_best_out;
+    A.abits = d_agg_bits_out;
+    A.guard = ctx->d_guard;
+    scm_args& M = A.M;
+    // k_scm_number reads a root at scm_item + SCM_ROOT: a contribution's root lies 8 bytes further into the item than a message's
+    M.wire = d_wire + (SCC_ROOT - SCM_ROOT);
+    M.woff = d_woff;
+    M.n = n;
+    M.pos_val = d_position_validator;
+    M.size = committee_size;
+    M.subnets = subnet_count;
+    M.sub = sub;
+    M.n_val = ctx->n_val;
+    M.status = d_status_out;
+    M.root_id = d_root_id_out;
+    M.n_roots = d_n_roots_out;
+    M.roots32 = d_roots32_out;
+    M.guard = ctx->d_guard;
+    // the verify verdicts (read by the kernels through A); the decompressed item signatures, the gathered ones and the root sums
+    uint8_t *av_ok, *fav_ok, *st, *gst;
+    uint32_t *aff, *gaff, *sumjac;
+    int32_t* segst;
+    scratch sc(ctx, ctx->scc);
+    sc(M.keys, committee_size); sc(A.subnet, n); sc(A.canon, n); sc(A.rslot, n); sc(A.rtab, tab); sc(A.bw, (size_t)n * A.sw); sc(A.ones, n);
+    sc(A.av_signer, 2 * (size_t)n); sc(A.av_off, 2 * (size_t)n + 1); sc(A.av_msg, (size_t)n * 64); sc(A.av_sig, (size_t)n * 192); sc(av_ok, 2 * (size_t)n);
+    sc(A.members, (size_t)n * sub); sc(A.item_off, (size_t)n + 1); sc(A.fbits, (size_t)n * sb, 16); sc(A.fmsg, (size_t)n * 32); sc(A.fsig, (size_t)n * 96);
+    sc(fav_ok, n); sc(A.taken, committee_size); sc(A.acc, committee_size); sc(M.slot_of, n); sc(M.rmin, tab); sc(M.rid, n);
+    sc(A.bestkey, nc); sc(A.cnt, (size_t)n + 1); sc(A.gsrc, n);
+    sc(aff, (size_t)n * 48, 16); sc(st, n, 16); sc(gaff, (size_t)n * 48, 16); sc(gst, n, 16); sc(sumjac, (size_t)n * 72); sc(segst, n);
+    if (sc.rc) return sc.rc;
+    A.av_ok = av_ok;
+    A.fav_ok = fav_ok;
+    cudaStream_t s = (cudaStream_t)stream;
+    CK(cudaMemsetAsync(A.rtab, 0xff, (size_t)tab * 4, s));
+    CK(cudaMemsetAsync(M.rmin, 0xff, (size_t)tab * 4, s));
+    CK(cudaMemsetAsync(A.taken, 0, committee_size, s));
+    CK(cudaMemsetAsync(A.bestkey, 0, nc * 8, s));
+    k_scm_index<<<1, 1024, 0, s>>>(M);
+    CKL(ctx);
+    k_scc_parse<<<blocks_for(n, 64), 64, 0, s>>>(A);
+    CKL(ctx);
+    // FastAggregateVerify of the contributions over their subnets' member rows, then AggregateVerify of the 2n single-key sets
+    pk_source P = {A.members, A.item_off, A.fbits, sb, nullptr, 0};
+    if ((rc = verify_fork(ctx, ctx->slot[0], P, A.fmsg, n, s)) || (rc = verify_main(ctx, ctx->slot[0], A.fsig, n, fav_ok, s))) return rc;
+    if ((rc = aggregate_verify_enqueue(ctx, A.av_signer, nullptr, A.av_msg, A.av_off, 2ull * n, A.av_sig, 2 * n, av_ok, s))) return rc;
+    k_scc_order<<<subnet_count, 32, 0, s>>>(A);
+    CKL(ctx);
+    k_scc_claim<<<blocks_for(n, 128), 128, 0, s>>>(A);
+    CKL(ctx);
+    k_scm_number<<<1, 1024, 0, s>>>(M);
+    CKL(ctx);
+    k_scc_best<<<blocks_for(n, 128), 128, 0, s>>>(A);
+    CKL(ctx);
+    k_scc_rows<<<blocks_for(n, 128), 128, 0, s>>>(A);
+    CKL(ctx);
+    k_intake_scan<<<1, 1024, 0, s>>>(A.cnt, n, nullptr);      // cnt[n] = the best items of every root
+    CKL(ctx);
+    k_scc_gather<<<blocks_for(n, 128), 128, 0, s>>>(A);
+    CKL(ctx);
+    // bls.Aggregate of each root's best contributions: the item signatures decompressed once (an item that was not accepted holds zero
+    // bytes and is never gathered), gathered in (root, subnet) order, one segment per root
+    k_g2_decompress<<<blocks_for(n, ctx->dec_block), ctx->dec_block, 0, s>>>(A.fsig, n, aff, st);
+    CKL(ctx);
+    k_pack_gather<<<blocks_for(n, 128), 128, 0, s>>>(aff, st, A.gsrc, A.cnt + n, gaff, gst);
+    CKL(ctx);
+    k_g2_segment_sum<<<n, 32, 0, s>>>(gaff, gst, A.cnt, n, sumjac, segst, n, ctx->d_guard);
+    CKL(ctx);
+    k_g2_finish<<<blocks_for(n, 32), 32, 0, s>>>(sumjac, segst, n, d_agg_sig96_out, nullptr, nullptr);
+    CKL(ctx);
+    return B2_OK;
+}
+
+int b2_sync_contribution_and_proof_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n,
+                                          const uint32_t* position_validator, uint32_t committee_size, uint32_t subnet_count, uint64_t current_slot,
+                                          const uint8_t* domains96, uint32_t target_aggregators, int32_t* status_out, uint32_t* root_id_out,
+                                          uint8_t* roots32_out, uint32_t* n_roots_out, uint32_t* best_out, uint8_t* agg_bits_out,
+                                          uint8_t* agg_sig96_out) {
+    B2_NVTX;
+    int rc;
+    if ((rc = check_sync_contribution_and_proof_intake(ctx, wire, woff, n, position_validator, committee_size, subnet_count, domains96, target_aggregators,
+                                                       status_out, root_id_out, roots32_out, n_roots_out, best_out, agg_bits_out, agg_sig96_out)) ||
+        (rc = check_wire(ctx, woff, n, wire_len, "sync_contribution_and_proof_intake")))
+        return rc;
+    for (uint32_t p = 0; p < committee_size; p++)
+        REQUIRE(position_validator[p] < ctx->n_val, "sync_contribution_and_proof_intake: a position_validator entry is outside the registry");
+    CK(cudaSetDevice(ctx->device));
+    staging st(ctx);
+    const uint8_t* dwire = st.in(wire, wire_len, 16);
+    const uint32_t* dwoff = st.in(woff, (size_t)n + 1);
+    const uint32_t* dpv = st.in(position_validator, committee_size);
+    int32_t* dst = st.out(status_out, n);
+    uint32_t* drid = st.out(root_id_out, n);
+    uint8_t* droots = st.out(roots32_out, (size_t)n * 32);
+    uint32_t* dnr = st.out(n_roots_out, 1);
+    uint32_t* dbest = st.out(best_out, (size_t)n * subnet_count);
+    uint8_t* dab = st.out(agg_bits_out, (size_t)n * ((committee_size + 7) / 8));
+    uint8_t* das = st.out(agg_sig96_out, (size_t)n * 96);
+    if (st.rc) return st.rc;
+    if ((rc = b2_sync_contribution_and_proof_intake_dev(ctx, dwire, wire_len, dwoff, n, dpv, committee_size, subnet_count, current_slot, domains96,
+                                                        target_aggregators, dst, drid, droots, dnr, dbest, dab, das, ctx->s_main)))
         return rc;
     return st.finish();
 }

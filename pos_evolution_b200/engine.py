@@ -30,6 +30,10 @@ BlockAttestationsResult = namedtuple("BlockAttestationsResult", "status flag_mas
 # subnet) the contribution's bit row, signature and present byte (uint8[n_roots, subnet_count, ...]); per root the SyncAggregate's bit row and
 # signature
 SyncMessagesResult = namedtuple("SyncMessagesResult", "status root_id roots contrib_bits contrib_sigs contrib_present agg_bits agg_sigs")
+# Engine.sync_contribution_and_proof_intake: per SignedContributionAndProof its status (0-12) and root id (0xFFFFFFFF: not accepted); the n_roots
+# distinct roots; per (root, subnet) the list index of the best accepted contribution (0xFFFFFFFF: none); per root the SyncAggregate's bit row
+# and signature
+SyncContributionsResult = namedtuple("SyncContributionsResult", "status root_id roots best agg_bits agg_sigs")
 
 
 def _c(a, dtype):
@@ -376,6 +380,29 @@ class Engine:
         k = int(n_roots[0])
         return r._replace(roots=r.roots[:k], contrib_bits=r.contrib_bits[:k], contrib_sigs=r.contrib_sigs[:k], contrib_present=r.contrib_present[:k],
                           agg_bits=r.agg_bits[:k], agg_sigs=r.agg_sigs[:k])
+
+    def sync_contribution_and_proof_intake(self, wire: bytes, woff, position_validator, subnet_count: int, current_slot: int, domains96: bytes,
+                                           target_aggregators: int = 16) -> SyncContributionsResult:
+        """One slot of SignedContributionAndProof messages (SSZ encodings back to back, woff their offsets) checked and verified against
+        the registry, and each root's SyncAggregate built from its best contribution per subnet (include/b200pos.h,
+        b2_sync_contribution_and_proof_intake: statuses 0-12).  position_validator: the registry index of each sync committee position;
+        domains96: the DOMAIN_SYNC_COMMITTEE, DOMAIN_SYNC_COMMITTEE_SELECTION_PROOF and DOMAIN_CONTRIBUTION_AND_PROOF domains of current_slot's
+        epoch, back to back.  Per-root outputs are trimmed to n_roots."""
+        woff, pv = _c(woff, np.uint32), _c(position_validator, np.uint32)
+        n, size, count = woff.shape[0] - 1, pv.shape[0], int(subnet_count)
+        assert count > 0
+        w = np.frombuffer(bytes(wire), dtype=np.uint8) if len(wire) else np.zeros(1, dtype=np.uint8)
+        dom = np.frombuffer(bytes(domains96), dtype=np.uint8)
+        assert dom.shape == (96,)
+        ab = (size + 7) // 8
+        r = SyncContributionsResult(np.zeros(n, np.int32), np.zeros(n, np.uint32), np.zeros((n, 32), np.uint8), np.zeros((n, count), np.uint32),
+                                    np.zeros((n, ab), np.uint8), np.zeros((n, 96), np.uint8))
+        n_roots = np.zeros(1, np.uint32)
+        self._ck(self.lib.b2_sync_contribution_and_proof_intake(self.h, _p(w), len(wire), _p(woff), n, _p(pv), size, count, int(current_slot),
+                                                                _p(dom), int(target_aggregators), _p(r.status), _p(r.root_id), _p(r.roots),
+                                                                _p(n_roots), _p(r.best), _p(r.agg_bits), _p(r.agg_sigs)))
+        k = int(n_roots[0])
+        return r._replace(roots=r.roots[:k], best=r.best[:k], agg_bits=r.agg_bits[:k], agg_sigs=r.agg_sigs[:k])
 
     def signing_roots(self, data128, domains32):
         """compute_signing_root for n attestations: data128 uint8[n,128] (SSZ-serialised AttestationData), domains32 uint8[32] or uint8[n,32]."""
@@ -808,6 +835,36 @@ class Engine:
         k = int(n_roots.item())
         return out._replace(roots=out.roots[:k], contrib_bits=out.contrib_bits[:k], contrib_sigs=out.contrib_sigs[:k],
                             contrib_present=out.contrib_present[:k], agg_bits=out.agg_bits[:k], agg_sigs=out.agg_sigs[:k])
+
+    def sync_contribution_and_proof_intake_dev(self, d_wire, d_woff, d_position_validator, subnet_count: int, current_slot: int,
+                                               domains96: bytes, target_aggregators: int = 16, out=None,
+                                               trim: bool = True) -> SyncContributionsResult:
+        """sync_contribution_and_proof_intake on device tensors (n = d_woff.numel() - 1, the wire's length is d_wire.numel(), committee_size
+        = d_position_validator.numel()), enqueued on the current stream.  `out`: (SyncContributionsResult of device tensors shaped as the
+        host form's untrimmed outputs, n_roots tensor of 4 bytes), or None to allocate them here (status, root_id and best int32: none is -1).
+        With trim (the default) the call waits for n_roots and returns the result with the per-root outputs trimmed to it; with trim=False
+        it stays asynchronous and returns the pair `out` takes."""
+        import torch
+        dom = np.frombuffer(bytes(domains96), dtype=np.uint8)
+        assert dom.shape == (96,)
+        n, size, count = d_woff.numel() - 1, d_position_validator.numel(), int(subnet_count)
+        assert count > 0
+        if out is None:
+            dev, u8, i32 = d_woff.device, torch.uint8, torch.int32
+            out = SyncContributionsResult(torch.empty(n, dtype=i32, device=dev), torch.empty(n, dtype=i32, device=dev),
+                                          torch.empty((n, 32), dtype=u8, device=dev), torch.empty((n, count), dtype=i32, device=dev),
+                                          torch.empty((n, (size + 7) // 8), dtype=u8, device=dev), torch.empty((n, 96), dtype=u8, device=dev))
+            n_roots = torch.empty(1, dtype=i32, device=dev)
+        else:
+            out, n_roots = out
+        self._ck(self.lib.b2_sync_contribution_and_proof_intake_dev(self.h, d_wire.data_ptr(), d_wire.numel(), d_woff.data_ptr(), n,
+                                                                    d_position_validator.data_ptr(), size, count, int(current_slot), _p(dom),
+                                                                    int(target_aggregators), *[x.data_ptr() for x in out[:3]],
+                                                                    n_roots.data_ptr(), *[x.data_ptr() for x in out[3:]], self._stream()))
+        if not trim:
+            return out, n_roots
+        k = int(n_roots.item())
+        return out._replace(roots=out.roots[:k], best=out.best[:k], agg_bits=out.agg_bits[:k], agg_sigs=out.agg_sigs[:k])
 
     def votes_empty_dev(self, d_bits, d_agg_sig, d_agg_status=None):
         """b2_votes_empty_dev on the current stream: every vote whose grouped bit row d_bits (uint8[n_votes, bits_stride]) has no attester

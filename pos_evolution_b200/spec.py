@@ -27,6 +27,8 @@ DOMAIN_BEACON_ATTESTER = bytes.fromhex("01000000")
 DOMAIN_SELECTION_PROOF = bytes.fromhex("05000000")             # upstream phase 0 validator spec
 DOMAIN_AGGREGATE_AND_PROOF = bytes.fromhex("06000000")
 DOMAIN_SYNC_COMMITTEE = bytes.fromhex("07000000")
+DOMAIN_SYNC_COMMITTEE_SELECTION_PROOF = bytes.fromhex("08000000")     # upstream Altair
+DOMAIN_CONTRIBUTION_AND_PROOF = bytes.fromhex("09000000")
 SYNC_REWARD_WEIGHT = 2
 TIMELY_SOURCE_FLAG_INDEX, TIMELY_TARGET_FLAG_INDEX, TIMELY_HEAD_FLAG_INDEX = 0, 1, 2
 PARTICIPATION_FLAG_WEIGHTS = [14, 26, 14]
@@ -61,6 +63,7 @@ class Preset:
     TARGET_AGGREGATORS_PER_COMMITTEE: int = 16    # upstream phase 0 validator spec (is_aggregator)
     ATTESTATION_PROPAGATION_SLOT_RANGE: int = 32  # upstream phase 0 p2p spec (beacon_aggregate_and_proof)
     SYNC_COMMITTEE_SUBNET_COUNT: int = 4          # upstream Altair validator spec (sync_committee_{subnet_id})
+    TARGET_AGGREGATORS_PER_SYNC_SUBCOMMITTEE: int = 16      # upstream Altair validator spec (is_sync_committee_aggregator)
 
 
 MAINNET = Preset("mainnet", 32, 64, 128, 90, 65536, 8192)
@@ -182,6 +185,25 @@ class SyncCommitteeContribution:       # upstream Altair validator spec
     beacon_block_root: bytes
     subcommittee_index: int
     aggregation_bits: List[bool]       # Bitvector[SYNC_COMMITTEE_SIZE // SYNC_COMMITTEE_SUBNET_COUNT]
+    signature: bytes
+
+
+@dataclass
+class SyncAggregatorSelectionData:     # upstream Altair validator spec: what a selection proof signs
+    slot: int
+    subcommittee_index: int
+
+
+@dataclass
+class ContributionAndProof:            # upstream Altair validator spec
+    aggregator_index: int
+    contribution: SyncCommitteeContribution
+    selection_proof: bytes
+
+
+@dataclass
+class SignedContributionAndProof:      # upstream Altair validator spec; the sync_committee_contribution_and_proof gossip message
+    message: ContributionAndProof
     signature: bytes
 
 
@@ -336,6 +358,15 @@ def serialize_signed_aggregate_and_proof(s: SignedAggregateAndProof) -> bytes:
 def serialize_sync_committee_message(m: SyncCommitteeMessage) -> bytes:
     """SSZ (:548-557): [slot u64][beacon_block_root][validator_index u64][signature], 144 bytes"""
     return int(m.slot).to_bytes(8, "little") + bytes(m.beacon_block_root) + int(m.validator_index).to_bytes(8, "little") + bytes(m.signature)
+
+
+def serialize_signed_contribution_and_proof(s: SignedContributionAndProof) -> bytes:
+    """SSZ, every field fixed (344 + ceil(len(aggregation_bits) / 8) bytes): [aggregator_index u64][slot u64][beacon_block_root]
+    [subcommittee_index u64][aggregation_bits Bitvector][contribution signature][selection_proof][signature]"""
+    m, c = s.message, s.message.contribution
+    return (int(m.aggregator_index).to_bytes(8, "little") + int(c.slot).to_bytes(8, "little") + bytes(c.beacon_block_root)
+            + int(c.subcommittee_index).to_bytes(8, "little") + pack_bits([list(c.aggregation_bits)])[0].tobytes() + bytes(c.signature)
+            + bytes(m.selection_proof) + bytes(s.signature))
 
 
 def serialize_validators(validators) -> np.ndarray:
@@ -1068,6 +1099,34 @@ class Spec:
                     contributions.append(SyncCommitteeContribution(current_slot, root, sc, [bool(b) for b in bits], r.contrib_sigs[k, sc].tobytes()))
             aggregates[root] = SyncAggregate([bool(b) for b in np.unpackbits(r.agg_bits[k], bitorder="little")[:size]], r.agg_sigs[k].tobytes())
         return [int(x) for x in r.status], contributions, aggregates
+
+    def validate_sync_contribution_and_proofs(self, state, items, current_slot=None):
+        """The sync_committee_contribution_and_proof gossip checks (upstream Altair p2p spec) of one slot's list of SignedContributionAndProof
+        on the GPU (b2_sync_contribution_and_proof_intake), and per root the SyncAggregate process_sync_committee_contributions (upstream
+        Altair validator spec) builds from its best accepted contribution per subnet.  current_slot defaults to state.slot; the committee is
+        sync_committee_for_messages' (get_sync_subcommittee_pubkeys' rule: the next committee when state.slot + 1 starts a new period); the
+        domains are those of current_slot's epoch.  Subcommittee membership compares registry indices, each committee key standing for its
+        first registry index.  Returns (status per item, 0-12 of include/b200pos.h; a SyncAggregates {root: SyncAggregate}, the empty
+        aggregate for a root with no accepted contribution).  Each call starts with empty seen-caches."""
+        current_slot = state.slot if current_slot is None else int(current_slot)
+        self.sync_registry(state)
+        committee = self.sync_committee_for_messages(state)
+        size, count = len(committee.pubkeys), self.p.SYNC_COMMITTEE_SUBNET_COUNT
+        aggregates = SyncAggregates(size)
+        if not items:
+            return [], aggregates
+        pv = self._position_validators(state, committee)
+        wires = [serialize_signed_contribution_and_proof(x) for x in items]
+        woff = np.cumsum([0] + [len(w) for w in wires]).astype(np.uint32)
+        epoch = self.compute_epoch_at_slot(current_slot)
+        domains = b"".join(self.get_domain(state, d, epoch) for d in (DOMAIN_SYNC_COMMITTEE, DOMAIN_SYNC_COMMITTEE_SELECTION_PROOF,
+                                                                      DOMAIN_CONTRIBUTION_AND_PROOF))
+        r = self.engine.sync_contribution_and_proof_intake(b"".join(wires), woff, pv, count, current_slot, domains,
+                                                           self.p.TARGET_AGGREGATORS_PER_SYNC_SUBCOMMITTEE)
+        for k in range(r.roots.shape[0]):
+            bits = np.unpackbits(r.agg_bits[k], bitorder="little")[:size]
+            aggregates[r.roots[k].tobytes()] = SyncAggregate([bool(b) for b in bits], r.agg_sigs[k].tobytes())
+        return [int(x) for x in r.status], aggregates
 
     # ------------------------------------------------------------------ fork choice
     def update_latest_messages(self, store, attesting_indices, attestation):   # :1435-1441
