@@ -674,7 +674,7 @@ int b2_sync_committee_messages(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_l
  * of the accepted item with the most set bits (ties to the smaller index), 0xFFFFFFFF where there is none; agg_bits u8[n][ceil(committee_size
  * / 8)] and agg_sig96 u8[n][96], per root the SyncAggregate of its best contributions (bit s * sub + i = bit i of best[r][s]'s row, signature
  * bls.Aggregate of their signatures): what a proposer includes, and what b2_sync_aggregate_verify accepts.  Rows of roots >= n_roots are
- * zero.  The accepted contributions themselves are the caller's wire bytes.
+ * zero, except best's, which are 0xFFFFFFFF (no item).  The accepted contributions themselves are the caller's wire bytes.
  * b2_sync_contribution_and_proof_intake_dev is asynchronous on `stream` and self-guarding: a reversed woff row or one past wire_len is status
  * 1 (B2_GUARD_BAD_ROW), and a position_validator entry >= n_validators matches nothing (B2_GUARD_BAD_INDEX); nothing is read or written out
  * of bounds.  It needs the registry (not b2_sync_committee_load's tables) and shares the AggregateVerify buffers and the verify buffers of

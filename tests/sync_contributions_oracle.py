@@ -21,6 +21,7 @@ from oracle.bls12_381 import R
 from oracle.ssz import compute_signing_root_from_object_root, merkleize, sha256, uint_chunk
 
 from sync_messages_oracle import SyncCommitteeContribution, pack, process_sync_committee_contributions
+from sync_oracle import G2_POINT_AT_INFINITY
 
 SUBNET_COUNT = 4
 FIXED = 344
@@ -80,9 +81,12 @@ def _bits(row: bytes, sub: int):
 
 
 def validate(wires, position_validator, n_validators, pubkey_of, current_slot, domains96, target=16, count=SUBNET_COUNT, verify=None,
-             fast_verify=None):
+             fast_verify=None, secret_key=None, closed_form=False):
     """verify(item, pubkey, message, signature, which) with which 0 (selection proof) or 1 (outer signature) defaults to bls.Verify;
-    fast_verify(item, pubkeys, message, signature) to bls.FastAggregateVerify"""
+    fast_verify(item, pubkeys, message, signature) to bls.FastAggregateVerify.  With secret_key(validator) given, each aggregate's
+    signature is computed in closed form, Sign(sum of the secret keys of its set positions, a validator at k positions k times, message):
+    the accepted contributions must then be honest ones.  With closed_form as well, it is left as the pair (sum mod r, signing root) for
+    the caller to sign in one batch (sync_messages_oracle.sign_closed_form)."""
     verify = verify or (lambda a, pk, m, s, which: B.Verify(pk, m, s))
     fast_verify = fast_verify or (lambda a, pks, m, s: B.FastAggregateVerify(pks, m, s))
     dom_sync, dom_sel, dom_cap = domains96[0:32], domains96[32:64], domains96[64:96]
@@ -141,7 +145,12 @@ def validate(wires, position_validator, n_validators, pubkey_of, current_slot, d
             if best[r][s] != NONE:
                 g, slot, _, _, row, sig, _, _ = decode(bytes(wires[best[r][s]]), sb)
                 present.append(SyncCommitteeContribution(slot, root, s, _bits(row, sub), sig))
-        aggregates.append(process_sync_committee_contributions(present, size, count))
+        agg = process_sync_committee_contributions(present, size, count, aggregate=secret_key is None)
+        if secret_key is not None:
+            k = sum(secret_key(position_validator[p]) for p, on in enumerate(agg.sync_committee_bits) if on) % R
+            msg = signing_root(root, dom_sync)
+            agg.sync_committee_signature = (k, msg) if closed_form else B.Sign(k, msg) if k else G2_POINT_AT_INFINITY
+        aggregates.append(agg)
     return Result(status, root_id, roots, best, aggregates)
 
 

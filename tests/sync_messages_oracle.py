@@ -58,9 +58,11 @@ def subnets_of(position_validator, validator_index: int, count: int = SUBNET_COU
 
 
 def validate(wires, subnets, position_validator, n_validators, pubkey_of, current_slot, domain32, count=SUBNET_COUNT, verify=None,
-             secret_key=None):
+             secret_key=None, closed_form=False):
     """verify(item, pubkey, message, signature) defaults to bls.Verify.  With secret_key(validator) given, every sum of accepted signatures
-    is computed in closed form, Sign(sum of the signers' secret keys, message): the accepted signatures must then be honest ones."""
+    is computed in closed form, Sign(sum of the signers' secret keys, message): the accepted signatures must then be honest ones.  With
+    closed_form as well, each such signature is left as its pair (sum of the secret keys mod r, signing root), for the caller to sign in one
+    batch (sign_closed_form)."""
     verify = verify or (lambda a, pk, msg, sig: B.Verify(pk, msg, sig))
     size = len(position_validator)
     sub = size // count
@@ -97,7 +99,8 @@ def validate(wires, subnets, position_validator, n_validators, pubkey_of, curren
 
     def sig_sum(items, signers, msg):
         if secret_key is not None:
-            return B.Sign(sum(secret_key(v) for v in signers) % R, msg)
+            k = sum(secret_key(v) for v in signers) % R
+            return (k, msg) if closed_form else B.Sign(k, msg)
         return B.Aggregate([bytes(wires[a])[48:144] for a in items])
 
     contributions, aggregates = {}, []
@@ -116,16 +119,37 @@ def validate(wires, subnets, position_validator, n_validators, pubkey_of, curren
             if items:
                 contributions[(r, s)] = SyncCommitteeContribution(current_slot, root, s, bits, sig_sum(items, signers, msg))
         present = [contributions[(r, s)] for s in range(count) if (r, s) in contributions]
-        agg = process_sync_committee_contributions(present, size, count)
+        agg = process_sync_committee_contributions(present, size, count, aggregate=secret_key is None)
         if secret_key is not None:      # the closed form of the same sum
             agg.sync_committee_signature = sig_sum(None, [position_validator[p] for p, b in enumerate(agg.sync_committee_bits) if b], msg)
         aggregates.append(agg)
     return Result(status, root_id, roots, contributions, aggregates)
 
 
-def process_sync_committee_contributions(contributions, size, count=SUBNET_COUNT) -> SyncAggregate:
+def closed_form_pairs(r):
+    """every (secret key, message) pair of a closed-form Result, in a fixed order (contributions by key, then aggregates)"""
+    out = [c.signature for _, c in sorted(r.contributions.items())] if hasattr(r, "contributions") else []
+    return out + [a.sync_committee_signature for a in r.aggregates]
+
+
+def sign_closed_form(r, sign):
+    """the Result with each (secret key, message) pair replaced by its signature: sign(keys, messages) -> signatures, one batch (a zero
+    key sums to the point at infinity)"""
+    pairs = [p for p in closed_form_pairs(r) if isinstance(p, tuple)]
+    live = [p for p in pairs if p[0] % R]
+    sigs = dict(zip(live, sign([k for k, _ in live], [m for _, m in live]))) if live else {}
+    done = lambda p: (sigs[p] if p[0] % R else G2_POINT_AT_INFINITY) if isinstance(p, tuple) else p      # noqa: E731
+    if hasattr(r, "contributions"):
+        for c in r.contributions.values():
+            c.signature = done(c.signature)
+    for a in r.aggregates:
+        a.sync_committee_signature = done(a.sync_committee_signature)
+    return r
+
+
+def process_sync_committee_contributions(contributions, size, count=SUBNET_COUNT, aggregate=True) -> SyncAggregate:
     """upstream Altair validator spec: the contributions' rows into the aggregate's bits, bls.Aggregate of their signatures (the G2
-    infinity encoding when there is none)"""
+    infinity encoding when there is none; None without `aggregate`, for a caller that fills in the closed form)"""
     bits, sigs = [False] * size, []
     sub = size // count
     for c in contributions:
@@ -133,6 +157,8 @@ def process_sync_committee_contributions(contributions, size, count=SUBNET_COUNT
             if on:
                 bits[sub * c.subcommittee_index + i] = True
         sigs.append(c.signature)
+    if not aggregate:
+        return SyncAggregate(bits, None)
     return SyncAggregate(bits, B.Aggregate(sigs) if sigs else G2_POINT_AT_INFINITY)
 
 
