@@ -596,6 +596,50 @@ int b2_block_attestations(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, c
                           uint32_t min_inclusion_delay, uint32_t bits_stride, uint64_t effective_balance_increment, uint64_t base_reward_per_increment,
                           int32_t* status_out, uint8_t* flag_mask_out, uint64_t* numerator_out, int32_t* block_status_out, uint32_t* block_first_out,
                           uint64_t* block_reward_out, uint32_t* n_applied_out);
+/* ---- process_attestation for the Electra (EIP-7549) on-chain Attestation, with Deneb's (EIP-7045) inclusion window and flags (upstream
+ * consensus-specs, Deneb and Electra beacon-chain.md), for the attestations of a run of blocks of one chain in one epoch e.  The inputs and
+ * outputs are b2_block_attestations', except:
+ *   wire                            Electra encodings: offset u32 | AttestationData 128 | signature 96 | committee_bits ceil(M / 8) |
+ *                                   aggregation_bits Bitlist[max_validators_per_committee * M], M = max_committees_per_slot (1..64)
+ *   max_validators_per_committee    with M, the Bitlist's limit (their product < 2^31)
+ *   row_max (device form only)      the largest member count of one slot's committees over e - 1 and e (> 0); the host form computes it
+ * An attestation names the committees (data.slot, i) of the bits i set in committee_bits, and its Bitlist is their bit rows back to back in
+ * increasing i.  Each attestation gets the first check it fails:
+ *    0  passes every check
+ *    1  malformed container (truncated, offset != fixed size, a committee_bits padding bit set), a woff row that is reversed or ends past
+ *       wire_len, or an attestation in no block's row
+ *    2  empty Bitlist or no delimiter                  3  more bits than max_validators_per_committee * M
+ *    4  target.epoch is neither e - 1 nor e            5  target.epoch != compute_epoch_at_slot(data.slot)
+ *    6  data.slot + MIN_ATTESTATION_INCLUSION_DELAY > block slot (no upper bound since Deneb)
+ *    7  data.index != 0
+ *    8-10  the committees by increasing index: 8 an index >= committees_per_slot of the target epoch; 10 its bit row runs past the Bitlist's
+ *       end; 9 no bit of its row set.  After them, 10 when the Bitlist's length is not their total size.
+ *   11  data.source != the justified checkpoint of the target epoch
+ *   12  no committee bit set (is_valid_indexed_attestation on empty indices)          13  FastAggregateVerify fails
+ * flag_mask is 0 unless checks 1-11 pass; its flags are Deneb's: timely source at inclusion delay <= integer_squareroot(slots_per_epoch),
+ * timely target whenever the target root matches, timely head when the target and head roots match at delay MIN_ATTESTATION_INCLUSION_DELAY.
+ * numerator, block_status, block_first, block_reward, n_applied, the two participation tables, block atomicity and b2_set_verify_mode are as
+ * in b2_block_attestations.  Committees are disjoint.
+ * b2_block_attestations_electra_dev is asynchronous on `stream` and self-guarding as b2_block_attestations_dev is; a committee row that is
+ * reversed or ends past n_sig, or whose committees add up to more than row_max members, is status 10 (B2_GUARD_BAD_ROW).  It shares pipeline
+ * slot 0's verify buffers as that call does.  b2_block_attestations_electra takes host arrays and returns when done; a rejected call (B2_EINVAL:
+ * b2_block_attestations' refusals without those on bits_stride, and M outside 1..64, max_validators_per_committee 0 or its product with M
+ * >= 2^31, n_att times the padded row >= 2^32 members) writes no output and changes nothing. */
+int b2_block_attestations_electra_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n_att,
+                                      const uint32_t* d_block_off, const uint64_t* d_block_slot, uint32_t n_blocks, const uint32_t* d_members,
+                                      const uint32_t* d_off, uint32_t n_committees, uint64_t n_sig, uint32_t cps_prev, uint32_t cps_cur,
+                                      const uint8_t* d_chain_roots, const uint8_t* justified80, const uint8_t* domains64, uint32_t slots_per_epoch,
+                                      uint32_t min_inclusion_delay, uint32_t max_committees_per_slot, uint32_t max_validators_per_committee,
+                                      uint32_t row_max, uint64_t effective_balance_increment, uint64_t base_reward_per_increment,
+                                      int32_t* d_status_out, uint8_t* d_flag_mask_out, uint64_t* d_numerator_out, int32_t* d_block_status_out,
+                                      uint32_t* d_block_first_out, uint64_t* d_block_reward_out, uint32_t* d_n_applied_out, void* stream);
+int b2_block_attestations_electra(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n_att, const uint32_t* block_off,
+                                  const uint64_t* block_slot, uint32_t n_blocks, const uint32_t* members, const uint32_t* off, uint32_t n_committees,
+                                  uint32_t cps_prev, uint32_t cps_cur, const uint8_t* chain_roots, const uint8_t* justified80, const uint8_t* domains64,
+                                  uint32_t slots_per_epoch, uint32_t min_inclusion_delay, uint32_t max_committees_per_slot,
+                                  uint32_t max_validators_per_committee, uint64_t effective_balance_increment, uint64_t base_reward_per_increment,
+                                  int32_t* status_out, uint8_t* flag_mask_out, uint64_t* numerator_out, int32_t* block_status_out,
+                                  uint32_t* block_first_out, uint64_t* block_reward_out, uint32_t* n_applied_out);
 /* ---- One slot of sync committee messages from gossip: SyncCommitteeMessage (pos-evolution.md:548-557) checked as the sync_committee_{subnet_id}
  * topics of the upstream Altair p2p spec require, grouped by beacon_block_root, and summed into each subnet's SyncCommitteeContribution and each
  * root's SyncAggregate as process_sync_committee_contributions of the upstream Altair validator spec builds them.  Inputs:

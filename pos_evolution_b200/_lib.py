@@ -119,6 +119,15 @@ SIGNATURES = {
                                           c_uint64] + [c_void_p] * 8),
     "b2_block_attestations": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p,
                                       c_uint32, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p, c_uint32, c_uint32, c_uint32, c_uint64, c_uint64] + [c_void_p] * 7),
+    # ctx, wire, wire_len, woff, n_att, block_off, block_slot, n_blocks, members, off, n_committees, [n_sig,] cps_prev, cps_cur, chain_roots, justified80,
+    # domains64, slots_per_epoch, min_inclusion_delay, max_committees_per_slot, max_validators_per_committee, [row_max,] increment,
+    # base_reward_per_increment, seven outputs[, stream]
+    "b2_block_attestations_electra_dev": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p,
+                                                  c_uint32, c_uint64, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p, c_uint32, c_uint32, c_uint32,
+                                                  c_uint32, c_uint32, c_uint64, c_uint64] + [c_void_p] * 8),
+    "b2_block_attestations_electra": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p,
+                                              c_uint32, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p, c_uint32, c_uint32, c_uint32, c_uint32,
+                                              c_uint64, c_uint64] + [c_void_p] * 7),
     # ctx, wire, wire_len, woff, n, subnet, position_validator, committee_size, subnet_count, current_slot, domain32, nine outputs[, stream]
     "b2_sync_committee_messages_dev": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_uint32, c_uint64,
                                                c_void_p] + [c_void_p] * 10),

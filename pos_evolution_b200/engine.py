@@ -24,7 +24,7 @@ IntakeResult = namedtuple("IntakeResult", "status vote vote_off sigs data128 msg
 AggregateIntakeResult = namedtuple("AggregateIntakeResult", "status committee data_id bits sigs msgs target_epoch block_idx members item_off")
 # Engine.block_attestations: per attestation its status (0-11), participation flag mask and proposer_reward_numerator; per block its status
 # (0 applied, 1 invalid, 2 after an invalid block), the list index of its first failing attestation (0xFFFFFFFF: none) and proposer reward;
-# the number of blocks applied
+# the number of blocks applied.  Engine.block_attestations_electra returns the same fields, its statuses 0-13.
 BlockAttestationsResult = namedtuple("BlockAttestationsResult", "status flag_mask numerator block_status block_first block_reward n_applied")
 # Engine.sync_committee_messages: per message its status (0-6) and root id (0xFFFFFFFF: not accepted); the n_roots distinct roots; per (root,
 # subnet) the contribution's bit row, signature and present byte (uint8[n_roots, subnet_count, ...]); per root the SyncAggregate's bit row and
@@ -356,6 +356,29 @@ class Engine:
                                                 off.shape[0] - 1, int(cps_prev), int(cps_cur), _p(roots), _p(j), _p(dom), int(slots_per_epoch),
                                                 int(min_inclusion_delay), int(bits_stride), int(increment), int(base_reward_per_increment),
                                                 *[_p(x) for x in r]))
+        return r._replace(n_applied=int(r.n_applied[0]))
+
+    def block_attestations_electra(self, wire: bytes, woff, block_off, block_slot, members, off, cps_prev: int, cps_cur: int, chain_roots,
+                                   justified80: bytes, domains64: bytes, slots_per_epoch: int, min_inclusion_delay: int,
+                                   max_committees_per_slot: int, max_validators_per_committee: int, increment: int,
+                                   base_reward_per_increment: int) -> BlockAttestationsResult:
+        """block_attestations for Electra encodings (include/b200pos.h, b2_block_attestations_electra: statuses 0-13, Deneb's window and
+        flags): an attestation names its committees of data.slot in committee_bits (max_committees_per_slot bits), and its Bitlist is their
+        bit rows back to back.  Applies the blocks before the first invalid one to the device participation tables (both must be loaded)."""
+        woff, block_off, members, off = _c(woff, np.uint32), _c(block_off, np.uint32), _c(members, np.uint32), _c(off, np.uint32)
+        block_slot = _c(block_slot, np.uint64)
+        roots = _c(chain_roots, np.uint8).reshape(-1)
+        n, n_b = woff.shape[0] - 1, block_off.shape[0] - 1
+        w = np.frombuffer(bytes(wire), dtype=np.uint8) if len(wire) else np.zeros(1, dtype=np.uint8)
+        mem = members if members.size else np.zeros(1, dtype=np.uint32)
+        j, dom = np.frombuffer(bytes(justified80), dtype=np.uint8), np.frombuffer(bytes(domains64), dtype=np.uint8)
+        assert j.shape == (80,) and dom.shape == (64,) and roots.shape == (64 * int(slots_per_epoch),) and block_slot.shape == (max(n_b, 0),)
+        r = BlockAttestationsResult(np.zeros(n, np.int32), np.zeros(n, np.uint8), np.zeros(n, np.uint64), np.zeros(n_b, np.int32),
+                                    np.zeros(n_b, np.uint32), np.zeros(n_b, np.uint64), np.zeros(1, np.uint32))
+        self._ck(self.lib.b2_block_attestations_electra(self.h, _p(w), len(wire), _p(woff), n, _p(block_off), _p(block_slot), n_b, _p(mem), _p(off),
+                                                        off.shape[0] - 1, int(cps_prev), int(cps_cur), _p(roots), _p(j), _p(dom), int(slots_per_epoch),
+                                                        int(min_inclusion_delay), int(max_committees_per_slot), int(max_validators_per_committee),
+                                                        int(increment), int(base_reward_per_increment), *[_p(x) for x in r]))
         return r._replace(n_applied=int(r.n_applied[0]))
 
     def sync_committee_messages(self, wire: bytes, woff, subnet, position_validator, subnet_count: int, current_slot: int,
@@ -803,6 +826,31 @@ class Engine:
                                                     int(base_reward_per_increment), d_status.data_ptr(), d_flag_mask.data_ptr(),
                                                     d_numerator.data_ptr(), d_block_status.data_ptr(), d_block_first.data_ptr(),
                                                     d_block_reward.data_ptr(), d_n_applied.data_ptr(), self._stream()))
+
+    def block_attestations_electra_dev(self, d_wire, d_woff, d_block_off, d_block_slot, d_members, d_off, cps_prev: int, cps_cur: int,
+                                       d_chain_roots, justified80: bytes, domains64: bytes, slots_per_epoch: int, min_inclusion_delay: int,
+                                       max_committees_per_slot: int, max_validators_per_committee: int, row_max: int, increment: int,
+                                       base_reward_per_increment: int, out=None) -> BlockAttestationsResult:
+        """block_attestations_electra on device tensors, asynchronous on the current stream: n_att = d_woff.numel() - 1, n_blocks =
+        d_block_off.numel() - 1, the wire's length is d_wire.numel(), n_sig = d_members.numel(); row_max, the largest member count of one
+        slot's committees.  `out`: a BlockAttestationsResult of device tensors (status int32[n_att], flag_mask uint8[n_att], numerator
+        uint64[n_att], block_status int32[n_blocks], block_first uint32[n_blocks], block_reward uint64[n_blocks], n_applied uint32[1]), or
+        None to allocate them here.  Returns the outputs."""
+        import torch
+        n, nb = d_woff.numel() - 1, d_block_off.numel() - 1
+        if out is None:
+            z = lambda k, dt: torch.zeros(k, dtype=dt, device=d_woff.device)      # noqa: E731
+            out = BlockAttestationsResult(z(n, torch.int32), z(n, torch.uint8), z(n, torch.uint64), z(nb, torch.int32), z(nb, torch.uint32),
+                                          z(nb, torch.uint64), z(1, torch.uint32))
+        j, dom = np.frombuffer(bytes(justified80), dtype=np.uint8), np.frombuffer(bytes(domains64), dtype=np.uint8)
+        assert j.shape == (80,) and dom.shape == (64,)
+        self._ck(self.lib.b2_block_attestations_electra_dev(self.h, d_wire.data_ptr(), d_wire.numel(), d_woff.data_ptr(), n, d_block_off.data_ptr(),
+                                                            d_block_slot.data_ptr(), nb, d_members.data_ptr(), d_off.data_ptr(), d_off.numel() - 1,
+                                                            d_members.numel(), int(cps_prev), int(cps_cur), d_chain_roots.data_ptr(), _p(j), _p(dom),
+                                                            int(slots_per_epoch), int(min_inclusion_delay), int(max_committees_per_slot),
+                                                            int(max_validators_per_committee), int(row_max), int(increment),
+                                                            int(base_reward_per_increment), *[x.data_ptr() for x in out], self._stream()))
+        return out
 
     def sync_committee_messages_dev(self, d_wire, d_woff, d_subnet, d_position_validator, subnet_count: int, current_slot: int, domain32: bytes,
                                     out=None, trim: bool = True) -> SyncMessagesResult:

@@ -107,6 +107,14 @@ class Attestation:                     # :714-717
 
 
 @dataclass
+class ElectraAttestation:              # upstream Electra beacon-chain.md (EIP-7549); SSZ field order as written
+    aggregation_bits: List[bool]       # the bit rows of the committees committee_bits names, back to back
+    data: AttestationData              # data.index == 0
+    signature: bytes
+    committee_bits: List[bool]         # Bitvector[MAX_COMMITTEES_PER_SLOT]
+
+
+@dataclass
 class BlockAttestations:               # the attestations of one block (BeaconBlockBody.attestations, :639) and what processing them needs
     slot: int                          # the block's slot: state.slot when process_block runs
     proposer_index: int                # the block's proposer, credited with the proposer rewards (:753-754)
@@ -343,6 +351,16 @@ def serialize_attestation(att: Attestation) -> bytes:
     bl = bytearray(pack_bits([list(att.aggregation_bits)], stride=n // 8 + 1)[0].tobytes())
     bl[n >> 3] |= 1 << (n & 7)
     return (228).to_bytes(4, "little") + serialize_attestation_data(att.data) + bytes(att.signature) + bytes(bl)
+
+
+def serialize_attestation_electra(att: ElectraAttestation) -> bytes:
+    """SSZ wire form: [offset of aggregation_bits = 228 + ceil(M / 8)][data][signature][committee_bits Bitvector[M]][Bitlist with its
+    delimiter bit], M = len(committee_bits)."""
+    M, n = len(att.committee_bits), len(att.aggregation_bits)
+    cb = pack_bits([list(att.committee_bits)], stride=(M + 7) // 8)[0].tobytes()
+    bl = bytearray(pack_bits([list(att.aggregation_bits)], stride=n // 8 + 1)[0].tobytes())
+    bl[n >> 3] |= 1 << (n & 7)
+    return (228 + len(cb)).to_bytes(4, "little") + serialize_attestation_data(att.data) + bytes(att.signature) + cb + bytes(bl)
 
 
 def serialize_aggregate_and_proof(m: AggregateAndProof) -> bytes:
@@ -888,6 +906,13 @@ class Spec:
         """The arguments of Engine.block_attestations for these blocks on this state (as process_block_attestations passes them): the
         attestations' encodings and offsets, the committees of epochs e - 1 and e, the chain's roots (state.block_roots below
         blocks[0].slot, block k's root for [slot_k, slot_{k+1})), the justified checkpoints, the attester domains and the scalars."""
+        args = self._block_attestations_args(state, blocks, serialize_attestation)
+        args["bits_stride"] = max(1, (int(np.diff(args["off"].astype(np.int64)).max()) + 7) // 8)
+        return args
+
+    def _block_attestations_args(self, state, blocks, serialize):
+        """what both block-attestation calls take: the encodings by `serialize` and their offsets, the block rows and slots, the
+        committees of epochs e - 1 and e, the chain's roots, the justified checkpoints, the attester domains and the scalars"""
         p = self.p
         spe = p.SLOTS_PER_EPOCH
         e = blocks[0].slot // spe
@@ -906,16 +931,44 @@ class Spec:
             else:
                 roots.append(bytes([b for b in blocks if b.slot <= s][-1].root))
         cps = lambda c: int(c.epoch).to_bytes(8, "little") + bytes(c.root)      # noqa: E731
-        wires = [serialize_attestation(a) for b in blocks for a in b.attestations]
+        wires = [serialize(a) for b in blocks for a in b.attestations]
         return dict(wire=b"".join(wires), woff=np.concatenate([[0], np.cumsum([len(w) for w in wires])]).astype(np.uint32),
                     block_off=np.concatenate([[0], np.cumsum([len(b.attestations) for b in blocks])]).astype(np.uint32),
                     block_slot=np.array([b.slot for b in blocks], dtype=np.uint64), members=members, off=off, cps_prev=cps_p, cps_cur=cps_c,
                     chain_roots=np.frombuffer(b"".join(roots), dtype=np.uint8),
                     justified80=cps(state.previous_justified_checkpoint) + cps(state.current_justified_checkpoint),
                     domains64=self.get_domain(state, DOMAIN_BEACON_ATTESTER, max(e, 1) - 1) + self.get_domain(state, DOMAIN_BEACON_ATTESTER, e),
-                    slots_per_epoch=spe, min_inclusion_delay=p.MIN_ATTESTATION_INCLUSION_DELAY,
-                    bits_stride=max(1, (int(np.diff(off.astype(np.int64)).max()) + 7) // 8), increment=p.EFFECTIVE_BALANCE_INCREMENT,
+                    slots_per_epoch=spe, min_inclusion_delay=p.MIN_ATTESTATION_INCLUSION_DELAY, increment=p.EFFECTIVE_BALANCE_INCREMENT,
                     base_reward_per_increment=self.get_base_reward_per_increment(state))
+
+    def process_block_attestations_electra(self, state, blocks):
+        """process_block_attestations for blocks whose attestations are ElectraAttestations (one GPU call, b2_block_attestations_electra):
+        Electra's process_attestation with Deneb's inclusion window and flags.  Block-atomic, the chain's roots, the proposers' rewards and
+        what is left unchanged as in process_block_attestations.  Returns (n_applied, statuses): per block, the status (0-13,
+        include/b200pos.h) of each attestation."""
+        assert blocks and state.slot == blocks[0].slot
+        block_off = np.concatenate([[0], np.cumsum([len(b.attestations) for b in blocks])]).astype(np.uint32)
+        if not block_off[-1]:
+            return len(blocks), [np.zeros(0, np.int32) for _ in blocks]
+        args = self.block_attestations_electra_inputs(state, blocks)
+        self.sync_registry(state)              # first: a registry reload drops the device participation tables
+        eng = self.engine
+        eng.participation_load(0, np.asarray(state.current_epoch_participation, dtype=np.uint8))
+        eng.participation_load(1, np.asarray(state.previous_epoch_participation, dtype=np.uint8))
+        res = eng.block_attestations_electra(**args)
+        if res.n_applied:
+            state.current_epoch_participation[:] = eng.participation_read(0).tolist()
+            state.previous_epoch_participation[:] = eng.participation_read(1).tolist()
+            for k in range(res.n_applied):
+                state.balances[blocks[k].proposer_index] += int(res.block_reward[k])
+        return res.n_applied, [res.status[block_off[k]:block_off[k + 1]] for k in range(len(blocks))]
+
+    def block_attestations_electra_inputs(self, state, blocks):
+        """The arguments of Engine.block_attestations_electra for these blocks of ElectraAttestations on this state: those of
+        block_attestations_inputs with the Electra encodings, MAX_COMMITTEES_PER_SLOT and MAX_VALIDATORS_PER_COMMITTEE in place of bits_stride."""
+        args = self._block_attestations_args(state, blocks, serialize_attestation_electra)
+        args.update(max_committees_per_slot=self.p.MAX_COMMITTEES_PER_SLOT, max_validators_per_committee=self.p.MAX_VALIDATORS_PER_COMMITTEE)
+        return args
 
     # ------------------------------------------------------------------ block packing (BeaconBlockBody.attestations :639, :659)
     def get_attestations_for_block(self, state, pool, max_attestations=None) -> List[Attestation]:
