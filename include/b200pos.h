@@ -473,6 +473,41 @@ int b2_attestation_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, c
                           uint64_t current_slot, const uint8_t* domain32, uint32_t max_votes, int32_t* status_out, uint32_t* vote_out,
                           uint32_t* vote_off_out, uint8_t* sig96_out, uint8_t* data128_out, uint8_t* msg32_out, uint64_t* source_epoch_out,
                           uint64_t* target_epoch_out, uint32_t* block_idx_out);
+/* ---- SingleAttestation intake: one epoch of Electra's unaggregated attestations (EIP-7549; the beacon_attestation_{subnet_id} topic of
+ * the upstream Electra p2p spec) checked and turned into the same vote form's inputs as b2_attestation_intake.  Container:
+ *   SingleAttestation{committee_index u64, attester_index u64, data AttestationData, signature BLSSignature}: 240 fixed bytes
+ * wire / woff = the encodings back to back and their byte offsets, wire_len the wire's bytes.  subnet[a] = the subnet id of the topic item
+ * a arrived on, subnet_count = ATTESTATION_SUBNET_COUNT.  Committee c of the epoch = (data.slot - start_slot(e)) * committees_per_slot +
+ * committee_index, members d_members[d_off[c] .. d_off[c+1]) (the layout of b2_attestation_intake; precondition: the committees are
+ * pairwise disjoint, as get_beacon_committee makes them).  Every item gets exactly one status, the first failing check:
+ *    0  kept
+ *    1  the item is not 240 bytes; also a woff row that is reversed or ends past wire_len
+ *    2  data.index != 0
+ *    3  committee_index >= committees_per_slot
+ *    4  data.slot outside epoch e
+ *    5  compute_subnet_for_attestation(committees_per_slot, data.slot, committee_index) != subnet[a]
+ *    6  data.target.epoch != e
+ *    7  current_slot < data.slot + 1
+ *    8  attester_index is not a member of committee (data.slot, committee_index); a malformed committee row (device form) has no members
+ *    9-12  b2_attestation_intake's 9-12 (the same tree walk)
+ *   13  duplicate: an earlier item in list order that passed checks 1-12 has the same attester_index (the same committee position)
+ * The attester's position is the smallest one of the committee that holds attester_index.  Signatures are not checked per item: the
+ * epoch pipeline verifies each vote's aggregate.  Outputs, max_votes, domain32, the device form's guards and the order of the calls
+ * sharing scratch are b2_attestation_intake's; data128 and msg32 are those of the data as signed (data.index == 0).  The host form
+ * refuses (B2_EINVAL, nothing written) what b2_attestation_intake refuses, and a missing subnet or members array or subnet_count == 0;
+ * both forms refuse n_att == 0, so every call they accept has items and needs its subnet array. */
+int b2_single_attestation_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n_att,
+                                     const uint32_t* d_subnet, uint32_t subnet_count, const uint32_t* d_members, const uint32_t* d_off,
+                                     uint32_t n_committees, uint64_t n_sig, uint32_t committees_per_slot, uint32_t slots_per_epoch, uint32_t bits_stride,
+                                     uint64_t epoch, uint64_t current_slot, const uint8_t* domain32, uint32_t max_votes, int32_t* d_status_out,
+                                     uint32_t* d_vote_out, uint32_t* d_vote_off_out, uint8_t* d_sig96_out, uint8_t* d_data128_out, uint8_t* d_msg32_out,
+                                     uint64_t* d_source_epoch_out, uint64_t* d_target_epoch_out, uint32_t* d_block_idx_out, void* stream);
+int b2_single_attestation_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n_att, const uint32_t* subnet,
+                                 uint32_t subnet_count, const uint32_t* members, const uint32_t* off, uint32_t n_committees, uint32_t committees_per_slot,
+                                 uint32_t slots_per_epoch, uint32_t bits_stride, uint64_t epoch, uint64_t current_slot, const uint8_t* domain32,
+                                 uint32_t max_votes, int32_t* status_out, uint32_t* vote_out, uint32_t* vote_off_out, uint8_t* sig96_out,
+                                 uint8_t* data128_out, uint8_t* msg32_out, uint64_t* source_epoch_out, uint64_t* target_epoch_out,
+                                 uint32_t* block_idx_out);
 /* ---- aggregated-attestation intake: one target epoch e of SignedAggregateAndProof messages from gossip (the beacon_aggregate_and_proof
  * topic of the upstream phase 0 p2p spec), checked and verified on the device.  Containers (upstream phase 0):
  *   AggregateAndProof{aggregator_index u64, aggregate Attestation, selection_proof BLSSignature}

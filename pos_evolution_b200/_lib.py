@@ -106,6 +106,12 @@ SIGNATURES = {
     "b2_attestation_intake": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_uint32, c_uint32, c_uint32, c_uint32, c_uint64,
                                       c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                       c_void_p]),
+    # ctx, wire, wire_len, woff, n_att, subnet, subnet_count, members, off, n_committees, [n_sig,] committees_per_slot, slots_per_epoch,
+    # bits_stride, epoch, current_slot, domain32, max_votes, nine outputs[, stream]
+    "b2_single_attestation_intake_dev": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32,
+                                                 c_uint64, c_uint32, c_uint32, c_uint32, c_uint64, c_uint64, c_void_p, c_uint32] + [c_void_p] * 10),
+    "b2_single_attestation_intake": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32,
+                                             c_uint32, c_uint32, c_uint32, c_uint64, c_uint64, c_void_p, c_uint32] + [c_void_p] * 9),
     # ctx, wire, wire_len, woff, n, members, off, n_committees, [n_sig,] committees_per_slot, slots_per_epoch, bits_stride, epoch, current_slot,
     # domains96, target_aggregators, propagation_slot_range, ten outputs[, stream]
     "b2_aggregate_and_proof_intake_dev": (c_int, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint32, c_void_p, c_void_p, c_uint32, c_uint64, c_uint32,

@@ -22,6 +22,7 @@
 #include "tree.cuh"
 #include "votes.cuh"
 #include "intake.cuh"
+#include "single_intake.cuh"
 #include "aggintake.cuh"
 #include "blockatt.cuh"
 #include "blockatt_electra.cuh"
@@ -1349,17 +1350,15 @@ static int check_attestation_intake(b2_ctx* ctx, const void* wire, const void* w
             "attestation_intake: bad arguments");
     return check_intake(ctx, n_committees, committees_per_slot, slots_per_epoch, epoch, current_slot, "attestation_intake");
 }
-int b2_attestation_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n_att, const uint32_t* d_off,
-                              uint32_t n_committees, uint64_t n_sig, uint32_t committees_per_slot, uint32_t slots_per_epoch, uint32_t bits_stride,
-                              uint64_t epoch, uint64_t current_slot, const uint8_t* domain32, uint32_t max_votes, int32_t* d_status_out,
-                              uint32_t* d_vote_out, uint32_t* d_vote_off_out, uint8_t* d_sig96_out, uint8_t* d_data128_out, uint8_t* d_msg32_out,
-                              uint64_t* d_source_epoch_out, uint64_t* d_target_epoch_out, uint32_t* d_block_idx_out, void* stream) {
-    B2_NVTX;
-    int rc;
-    if ((rc = check_attestation_intake(ctx, d_wire, d_woff, n_att, d_off, n_committees, committees_per_slot, slots_per_epoch, bits_stride, epoch, current_slot, domain32,
-                                       max_votes, d_status_out, d_vote_out, d_vote_off_out, d_sig96_out, d_data128_out, d_msg32_out, d_source_epoch_out,
-                                       d_target_epoch_out, d_block_idx_out)))
-        return rc;
+// Both attestation intakes after their argument checks: d_members == nullptr is the phase 0 form (k_intake_parse), otherwise the
+// SingleAttestation form (k_single_parse, which also writes the offset view the later kernels read as woff).
+static int attestation_intake_enqueue(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n_att,
+                                      const uint32_t* d_subnet, uint32_t subnet_count, const uint32_t* d_members, const uint32_t* d_off,
+                                      uint32_t n_committees, uint64_t n_sig, uint32_t committees_per_slot, uint32_t slots_per_epoch,
+                                      uint32_t bits_stride, uint64_t epoch, uint64_t current_slot, const uint8_t* domain32, uint32_t max_votes,
+                                      int32_t* d_status_out, uint32_t* d_vote_out, uint32_t* d_vote_off_out, uint8_t* d_sig96_out,
+                                      uint8_t* d_data128_out, uint8_t* d_msg32_out, uint64_t* d_source_epoch_out, uint64_t* d_target_epoch_out,
+                                      uint32_t* d_block_idx_out, void* stream) {
     REQUIRE(n_sig < (1ull << 32), "attestation_intake: n_sig does not fit 32 bits");      // the host form's n_sig is a u32 offset
     CK(cudaSetDevice(ctx->device));
     const tree_tables& t = ctx->tree;
@@ -1399,6 +1398,8 @@ int b2_attestation_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_
     sc(A.bucket, nc); sc(A.cursor, nc); sc(A.nkept, nc);
     sc(A.list, n_att); sc(A.lead, n_att); sc(A.gstat, n_att); sc(A.gblk, n_att); sc(A.gmin, n_att); sc(A.vgrp, n_att);
     sc(A.posatt, n_sig); sc(sorted, ctx->n_blocks);
+    single_args S = {};
+    if (d_members) sc(S.view, n_att);
     if (sc.rc) return sc.rc;
     A.sorted = sorted;
     cudaStream_t s = (cudaStream_t)stream;
@@ -1406,7 +1407,17 @@ int b2_attestation_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_
     k_intake_sorted<<<blocks_for(ctx->n_blocks, 256), 256, 0, s>>>(t.rank_id, ctx->n_blocks, sorted);
     CKL(ctx);
     CK(cudaMemsetAsync(A.bucket, 0, nc * 4, s));
-    k_intake_parse<<<blocks_for((uint64_t)n_att * 32, 128), 128, 0, s>>>(A);
+    if (d_members) {
+        A.woff = S.view;      // the later kernels read each SingleAttestation's data and signature through the offset view
+        S.T = A;
+        S.woff = d_woff;
+        S.members = d_members;
+        S.subnet = d_subnet;
+        S.subnet_count = subnet_count;
+        k_single_parse<<<blocks_for((uint64_t)n_att * 32, 128), 128, 0, s>>>(S);
+    } else {
+        k_intake_parse<<<blocks_for((uint64_t)n_att * 32, 128), 128, 0, s>>>(A);
+    }
     CKL(ctx);
     k_intake_scan<<<1, 1024, 0, s>>>(A.bucket, n_committees, A.cursor);      // bucket[n_committees] = the candidates
     CKL(ctx);
@@ -1423,18 +1434,61 @@ int b2_attestation_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_
     CK(cudaEventRecord(ctx->ev_intake, s));
     return B2_OK;
 }
-
-int b2_attestation_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n_att, const uint32_t* off,
-                          uint32_t n_committees, uint32_t committees_per_slot, uint32_t slots_per_epoch, uint32_t bits_stride, uint64_t epoch,
-                          uint64_t current_slot, const uint8_t* domain32, uint32_t max_votes, int32_t* status_out, uint32_t* vote_out,
-                          uint32_t* vote_off_out, uint8_t* sig96_out, uint8_t* data128_out, uint8_t* msg32_out, uint64_t* source_epoch_out,
-                          uint64_t* target_epoch_out, uint32_t* block_idx_out) {
+int b2_attestation_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n_att, const uint32_t* d_off,
+                              uint32_t n_committees, uint64_t n_sig, uint32_t committees_per_slot, uint32_t slots_per_epoch, uint32_t bits_stride,
+                              uint64_t epoch, uint64_t current_slot, const uint8_t* domain32, uint32_t max_votes, int32_t* d_status_out,
+                              uint32_t* d_vote_out, uint32_t* d_vote_off_out, uint8_t* d_sig96_out, uint8_t* d_data128_out, uint8_t* d_msg32_out,
+                              uint64_t* d_source_epoch_out, uint64_t* d_target_epoch_out, uint32_t* d_block_idx_out, void* stream) {
     B2_NVTX;
     int rc;
-    if ((rc = check_attestation_intake(ctx, wire, woff, n_att, off, n_committees, committees_per_slot, slots_per_epoch, bits_stride, epoch, current_slot, domain32, max_votes,
-                                       status_out, vote_out, vote_off_out, sig96_out, data128_out, msg32_out, source_epoch_out, target_epoch_out,
-                                       block_idx_out)) ||
-        (rc = check_wire(ctx, woff, n_att, wire_len, "attestation_intake")) ||
+    if ((rc = check_attestation_intake(ctx, d_wire, d_woff, n_att, d_off, n_committees, committees_per_slot, slots_per_epoch, bits_stride, epoch, current_slot, domain32,
+                                       max_votes, d_status_out, d_vote_out, d_vote_off_out, d_sig96_out, d_data128_out, d_msg32_out, d_source_epoch_out,
+                                       d_target_epoch_out, d_block_idx_out)))
+        return rc;
+    return attestation_intake_enqueue(ctx, d_wire, wire_len, d_woff, n_att, nullptr, 0, nullptr, d_off, n_committees, n_sig, committees_per_slot,
+                                      slots_per_epoch, bits_stride, epoch, current_slot, domain32, max_votes, d_status_out, d_vote_out, d_vote_off_out,
+                                      d_sig96_out, d_data128_out, d_msg32_out, d_source_epoch_out, d_target_epoch_out, d_block_idx_out, stream);
+}
+// the SingleAttestation form's arguments: the phase 0 form's, the members and the arrival subnets
+static int check_single_attestation_intake(b2_ctx* ctx, const void* wire, const void* woff, uint32_t n_att, const void* subnet, uint32_t subnet_count,
+                                           const void* members, const void* off, uint32_t n_committees, uint32_t committees_per_slot,
+                                           uint32_t slots_per_epoch, uint32_t bits_stride, uint64_t epoch, uint64_t current_slot, const void* domain32,
+                                           uint32_t max_votes, const void* status_out, const void* vote_out, const void* vote_off_out,
+                                           const void* sig96_out, const void* data128_out, const void* msg32_out, const void* source_epoch_out,
+                                           const void* target_epoch_out, const void* block_idx_out) {
+    REQUIRE(ctx && subnet && members && subnet_count > 0, "single_attestation_intake: bad arguments");
+    return check_attestation_intake(ctx, wire, woff, n_att, off, n_committees, committees_per_slot, slots_per_epoch, bits_stride, epoch, current_slot,
+                                    domain32, max_votes, status_out, vote_out, vote_off_out, sig96_out, data128_out, msg32_out, source_epoch_out,
+                                    target_epoch_out, block_idx_out);
+}
+int b2_single_attestation_intake_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n_att,
+                                     const uint32_t* d_subnet, uint32_t subnet_count, const uint32_t* d_members, const uint32_t* d_off,
+                                     uint32_t n_committees, uint64_t n_sig, uint32_t committees_per_slot, uint32_t slots_per_epoch, uint32_t bits_stride,
+                                     uint64_t epoch, uint64_t current_slot, const uint8_t* domain32, uint32_t max_votes, int32_t* d_status_out,
+                                     uint32_t* d_vote_out, uint32_t* d_vote_off_out, uint8_t* d_sig96_out, uint8_t* d_data128_out, uint8_t* d_msg32_out,
+                                     uint64_t* d_source_epoch_out, uint64_t* d_target_epoch_out, uint32_t* d_block_idx_out, void* stream) {
+    B2_NVTX;
+    int rc;
+    if ((rc = check_single_attestation_intake(ctx, d_wire, d_woff, n_att, d_subnet, subnet_count, d_members, d_off, n_committees, committees_per_slot,
+                                              slots_per_epoch, bits_stride, epoch, current_slot, domain32, max_votes, d_status_out, d_vote_out,
+                                              d_vote_off_out, d_sig96_out, d_data128_out, d_msg32_out, d_source_epoch_out, d_target_epoch_out,
+                                              d_block_idx_out)))
+        return rc;
+    return attestation_intake_enqueue(ctx, d_wire, wire_len, d_woff, n_att, d_subnet, subnet_count, d_members, d_off, n_committees, n_sig,
+                                      committees_per_slot, slots_per_epoch, bits_stride, epoch, current_slot, domain32, max_votes, d_status_out,
+                                      d_vote_out, d_vote_off_out, d_sig96_out, d_data128_out, d_msg32_out, d_source_epoch_out, d_target_epoch_out,
+                                      d_block_idx_out, stream);
+}
+
+// Both host forms after their argument checks: stage, zero the vote rows, enqueue (members == nullptr: the phase 0 form).
+static int attestation_intake_host(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n_att, const uint32_t* subnet,
+                                   uint32_t subnet_count, const uint32_t* members, const uint32_t* off, uint32_t n_committees,
+                                   uint32_t committees_per_slot, uint32_t slots_per_epoch, uint32_t bits_stride, uint64_t epoch, uint64_t current_slot,
+                                   const uint8_t* domain32, uint32_t max_votes, int32_t* status_out, uint32_t* vote_out, uint32_t* vote_off_out,
+                                   uint8_t* sig96_out, uint8_t* data128_out, uint8_t* msg32_out, uint64_t* source_epoch_out, uint64_t* target_epoch_out,
+                                   uint32_t* block_idx_out) {
+    int rc;
+    if ((rc = check_wire(ctx, woff, n_att, wire_len, "attestation_intake")) ||
         (rc = check_committees(ctx, off, n_committees, bits_stride, "attestation_intake")))
         return rc;
     const uint64_t n_sig = off[n_committees];
@@ -1442,6 +1496,8 @@ int b2_attestation_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, c
     staging st(ctx);
     const uint8_t* dwire = st.in(wire, wire_len, 16);
     const uint32_t* dwoff = st.in(woff, (size_t)n_att + 1);
+    const uint32_t* dsub = members ? st.in(subnet, n_att) : nullptr;
+    const uint32_t* dmem = members ? st.in(members, n_sig, 4) : nullptr;
     const uint32_t* doff = st.in(off, (size_t)n_committees + 1);
     int32_t* dst = st.out(status_out, n_att);
     uint32_t* dvote = st.out(vote_out, n_sig);
@@ -1459,10 +1515,40 @@ int b2_attestation_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, c
     CK(cudaMemsetAsync(dsrc, 0, (size_t)max_votes * 8, ctx->s_main));
     CK(cudaMemsetAsync(dtgt, 0, (size_t)max_votes * 8, ctx->s_main));
     CK(cudaMemsetAsync(dblk, 0, (size_t)max_votes * 4, ctx->s_main));
-    if ((rc = b2_attestation_intake_dev(ctx, dwire, wire_len, dwoff, n_att, doff, n_committees, n_sig, committees_per_slot, slots_per_epoch, bits_stride,
-                                        epoch, current_slot, domain32, max_votes, dst, dvote, dvoff, dsig, ddata, dmsg, dsrc, dtgt, dblk, ctx->s_main)))
+    if ((rc = attestation_intake_enqueue(ctx, dwire, wire_len, dwoff, n_att, dsub, subnet_count, dmem, doff, n_committees, n_sig, committees_per_slot,
+                                         slots_per_epoch, bits_stride, epoch, current_slot, domain32, max_votes, dst, dvote, dvoff, dsig, ddata, dmsg,
+                                         dsrc, dtgt, dblk, ctx->s_main)))
         return rc;
     return st.finish();
+}
+int b2_attestation_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n_att, const uint32_t* off,
+                          uint32_t n_committees, uint32_t committees_per_slot, uint32_t slots_per_epoch, uint32_t bits_stride, uint64_t epoch,
+                          uint64_t current_slot, const uint8_t* domain32, uint32_t max_votes, int32_t* status_out, uint32_t* vote_out,
+                          uint32_t* vote_off_out, uint8_t* sig96_out, uint8_t* data128_out, uint8_t* msg32_out, uint64_t* source_epoch_out,
+                          uint64_t* target_epoch_out, uint32_t* block_idx_out) {
+    B2_NVTX;
+    if (int rc = check_attestation_intake(ctx, wire, woff, n_att, off, n_committees, committees_per_slot, slots_per_epoch, bits_stride, epoch, current_slot,
+                                          domain32, max_votes, status_out, vote_out, vote_off_out, sig96_out, data128_out, msg32_out, source_epoch_out,
+                                          target_epoch_out, block_idx_out))
+        return rc;
+    return attestation_intake_host(ctx, wire, wire_len, woff, n_att, nullptr, 0, nullptr, off, n_committees, committees_per_slot, slots_per_epoch,
+                                   bits_stride, epoch, current_slot, domain32, max_votes, status_out, vote_out, vote_off_out, sig96_out, data128_out,
+                                   msg32_out, source_epoch_out, target_epoch_out, block_idx_out);
+}
+int b2_single_attestation_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n_att, const uint32_t* subnet,
+                                 uint32_t subnet_count, const uint32_t* members, const uint32_t* off, uint32_t n_committees, uint32_t committees_per_slot,
+                                 uint32_t slots_per_epoch, uint32_t bits_stride, uint64_t epoch, uint64_t current_slot, const uint8_t* domain32,
+                                 uint32_t max_votes, int32_t* status_out, uint32_t* vote_out, uint32_t* vote_off_out, uint8_t* sig96_out,
+                                 uint8_t* data128_out, uint8_t* msg32_out, uint64_t* source_epoch_out, uint64_t* target_epoch_out,
+                                 uint32_t* block_idx_out) {
+    B2_NVTX;
+    if (int rc = check_single_attestation_intake(ctx, wire, woff, n_att, subnet, subnet_count, members, off, n_committees, committees_per_slot,
+                                                 slots_per_epoch, bits_stride, epoch, current_slot, domain32, max_votes, status_out, vote_out,
+                                                 vote_off_out, sig96_out, data128_out, msg32_out, source_epoch_out, target_epoch_out, block_idx_out))
+        return rc;
+    return attestation_intake_host(ctx, wire, wire_len, woff, n_att, subnet, subnet_count, members, off, n_committees, committees_per_slot,
+                                   slots_per_epoch, bits_stride, epoch, current_slot, domain32, max_votes, status_out, vote_out, vote_off_out,
+                                   sig96_out, data128_out, msg32_out, source_epoch_out, target_epoch_out, block_idx_out);
 }
 
 // ------------------------------------------------------------------------------------------ aggregated-attestation intake (aggintake.cuh)

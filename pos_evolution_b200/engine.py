@@ -314,6 +314,28 @@ class Engine:
                                                 *[_p(x) for x in r]))
         return r
 
+    def single_attestation_intake(self, wire: bytes, woff, subnet, members, off, epoch: int, current_slot: int, domain32: bytes,
+                                  committees_per_slot: int, slots_per_epoch: int, bits_stride: int, max_votes: int,
+                                  subnet_count: int = 64) -> IntakeResult:
+        """One epoch of Electra SingleAttestations (240-byte encodings back to back, woff their offsets, subnet the subnet each arrived
+        on) checked against the device tree and turned into the vote form's inputs (include/b200pos.h, b2_single_attestation_intake:
+        statuses 0-13); committee c = members[off[c] .. off[c+1]]; subnet_count = ATTESTATION_SUBNET_COUNT."""
+        woff, subnet, members, off = _c(woff, np.uint32), _c(subnet, np.uint32), _c(members, np.uint32), _c(off, np.uint32)
+        n_att, n_c = woff.shape[0] - 1, off.shape[0] - 1
+        assert subnet.shape == (n_att,)
+        w = np.frombuffer(bytes(wire), dtype=np.uint8) if len(wire) else np.zeros(1, dtype=np.uint8)
+        mem = members if members.size else np.zeros(1, dtype=np.uint32)
+        dom = np.frombuffer(bytes(domain32), dtype=np.uint8)
+        assert dom.shape == (32,)
+        n_sig, mv = int(off[-1]), int(max_votes)
+        r = IntakeResult(np.zeros(n_att, np.int32), np.zeros(n_sig, np.uint32), np.zeros(n_c + 1, np.uint32), np.zeros((n_sig, 96), np.uint8),
+                         np.zeros((mv, 128), np.uint8), np.zeros((mv, 32), np.uint8), np.zeros(mv, np.uint64), np.zeros(mv, np.uint64),
+                         np.zeros(mv, np.uint32))
+        self._ck(self.lib.b2_single_attestation_intake(self.h, _p(w), len(wire), _p(woff), n_att, _p(subnet), int(subnet_count), _p(mem), _p(off),
+                                                       n_c, int(committees_per_slot), int(slots_per_epoch), int(bits_stride), int(epoch),
+                                                       int(current_slot), _p(dom), mv, *[_p(x) for x in r]))
+        return r
+
     def aggregate_and_proof_intake(self, wire: bytes, woff, members, off, epoch: int, current_slot: int, domains96: bytes,
                                    committees_per_slot: int, slots_per_epoch: int, bits_stride: int, target_aggregators: int = 16,
                                    propagation_slot_range: int = 32) -> AggregateIntakeResult:
@@ -787,6 +809,23 @@ class Engine:
                                                     d_msgs.shape[0], d_status.data_ptr(), d_vote.data_ptr(), d_vote_off.data_ptr(),
                                                     d_sigs.data_ptr(), d_data128.data_ptr(), d_msgs.data_ptr(), d_source_epoch.data_ptr(),
                                                     d_target_epoch.data_ptr(), d_block_idx.data_ptr(), self._stream()))
+
+    def single_attestation_intake_dev(self, d_wire, d_woff, d_subnet, d_members, d_off, epoch: int, current_slot: int, domain32: bytes,
+                                      committees_per_slot: int, slots_per_epoch: int, bits_stride: int, d_status, d_vote, d_vote_off, d_sigs,
+                                      d_data128, d_msgs, d_source_epoch, d_target_epoch, d_block_idx, subnet_count: int = 64):
+        """single_attestation_intake on device tensors (d_subnet int32/uint32[n_att]; the wire's length is d_wire.numel(); max_votes =
+        d_msgs.shape[0]; the outputs as attestation_intake_dev's), asynchronous on the current stream."""
+        dom = np.frombuffer(bytes(domain32), dtype=np.uint8)
+        assert dom.shape == (32,)
+        n_att = d_woff.numel() - 1
+        assert d_subnet.numel() == n_att and d_members.numel() == d_vote.numel()
+        self._ck(self.lib.b2_single_attestation_intake_dev(self.h, d_wire.data_ptr(), d_wire.numel(), d_woff.data_ptr(), n_att,
+                                                           d_subnet.data_ptr(), int(subnet_count), d_members.data_ptr(), d_off.data_ptr(),
+                                                           d_off.numel() - 1, d_vote.numel(), int(committees_per_slot), int(slots_per_epoch),
+                                                           int(bits_stride), int(epoch), int(current_slot), _p(dom), d_msgs.shape[0],
+                                                           d_status.data_ptr(), d_vote.data_ptr(), d_vote_off.data_ptr(), d_sigs.data_ptr(),
+                                                           d_data128.data_ptr(), d_msgs.data_ptr(), d_source_epoch.data_ptr(),
+                                                           d_target_epoch.data_ptr(), d_block_idx.data_ptr(), self._stream()))
 
     def aggregate_and_proof_intake_dev(self, d_wire, d_woff, d_members, d_off, epoch: int, current_slot: int, domains96: bytes,
                                        committees_per_slot: int, slots_per_epoch: int, d_status, d_committee, d_data_id, d_bits, d_sigs, d_msgs,

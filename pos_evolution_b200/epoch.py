@@ -45,6 +45,7 @@ of its committees [vote_off[c0_g], vote_off[c1_g]); the all-gather pads every ra
 Attestation intake (`intake_dev`): an epoch of unaggregated Attestations straight off the wire is checked against the device tree
 (process_attestation, validate_on_attestation), one kept per committee position, and turned into the vote form's inputs on the device
 (Engine.attestation_intake_dev); the returned tensors go to submit_dev / process_epoch_dev with votes=(r.vote, r.vote_off).
+`intake_single_dev` does the same for Electra's SingleAttestations (Engine.single_attestation_intake_dev).
 
 Equivocation discounting (`enable_slasher(..., discount=True)`, pos-evolution.md:1405-1461): right after each epoch's slasher update,
 every validator it flagged joins the device's Store.equivocating_indices, so from the next epoch on its votes neither move its latest
@@ -605,20 +606,38 @@ class EpochProcessor:
         contract of submit_dev once submitted.  Reading vote_off waits for the current stream's work up to the intake: enqueue it under a
         stream that carries no epoch (torch.cuda.stream(...)) and it waits for the intake alone.  An epoch with more than max_votes votes
         is then refused by submit_dev.  Not for a sharded processor."""
+        def call(r, d_vote_off):
+            self.eng.attestation_intake_dev(d_wire, d_woff, self.d_off, epoch, current_slot, domain32, committees_per_slot, slots_per_epoch,
+                                            self.bits_stride, r.status, r.vote, d_vote_off, r.sigs, r.data128, r.msgs, r.source_epoch,
+                                            r.target_epoch, r.block_idx)
+        return self._intake("intake_dev", call, d_woff.numel() - 1, committees_per_slot, slots_per_epoch)
+
+    def intake_single_dev(self, d_wire, d_woff, d_subnet, epoch, current_slot, domain32, committees_per_slot, slots_per_epoch,
+                          subnet_count=64) -> Intake:
+        """intake_dev for one epoch of Electra SingleAttestations (240-byte encodings on the device, d_woff their offsets, d_subnet
+        int32/uint32[n_att] the subnet each arrived on, subnet_count = ATTESTATION_SUBNET_COUNT) against this processor's committees
+        (Engine.single_attestation_intake_dev, on the current stream).  The same Intake, contract and refusals as intake_dev; status holds
+        b2_single_attestation_intake's statuses."""
+        def call(r, d_vote_off):
+            self.eng.single_attestation_intake_dev(d_wire, d_woff, d_subnet, self.d_members, self.d_off, epoch, current_slot, domain32,
+                                                   committees_per_slot, slots_per_epoch, self.bits_stride, r.status, r.vote, d_vote_off, r.sigs,
+                                                   r.data128, r.msgs, r.source_epoch, r.target_epoch, r.block_idx, subnet_count=subnet_count)
+        return self._intake("intake_single_dev", call, d_woff.numel() - 1, committees_per_slot, slots_per_epoch)
+
+    def _intake(self, name, call, n_att, committees_per_slot, slots_per_epoch) -> Intake:
+        """Both intakes: the refusals, fresh outputs, call(outputs, d_vote_off) on the current stream, then vote_off on the host"""
         if self.sharded:
-            raise ValueError("intake_dev: a sharded EpochProcessor is not supported")
+            raise ValueError("%s: a sharded EpochProcessor is not supported" % name)
         if self.max_votes is None:
-            raise ValueError("intake_dev needs an EpochProcessor constructed with max_votes")
+            raise ValueError("%s needs an EpochProcessor constructed with max_votes" % name)
         if int(committees_per_slot) * int(slots_per_epoch) != self.n_agg:
             raise ValueError("committees_per_slot * slots_per_epoch must be the processor's n_agg = %d" % self.n_agg)
         self._check_tree()
         z, mv = self._zeros, self.max_votes
         r = Intake(z((self.n_sig, 96), torch.uint8), torch.full((self.n_sig,), -1, dtype=torch.int32, device=self.dev), z((mv, 32), torch.uint8),
-                   z(mv, torch.int64), z(mv, torch.int32), z(mv, torch.int64), z((mv, 128), torch.uint8), z(d_woff.numel() - 1, torch.int32), None)
+                   z(mv, torch.int64), z(mv, torch.int32), z(mv, torch.int64), z((mv, 128), torch.uint8), z(n_att, torch.int32), None)
         d_vote_off = z(self.n_agg + 1, torch.int32)
-        self.eng.attestation_intake_dev(d_wire, d_woff, self.d_off, epoch, current_slot, domain32, committees_per_slot, slots_per_epoch,
-                                        self.bits_stride, r.status, r.vote, d_vote_off, r.sigs, r.data128, r.msgs, r.source_epoch,
-                                        r.target_epoch, r.block_idx)
+        call(r, d_vote_off)
         h = self._pinned(self.n_agg + 1, torch.int32)
         h.copy_(d_vote_off, non_blocking=True)
         self._record().synchronize()

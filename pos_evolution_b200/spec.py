@@ -115,6 +115,14 @@ class ElectraAttestation:              # upstream Electra beacon-chain.md (EIP-7
 
 
 @dataclass
+class SingleAttestation:               # upstream Electra beacon-chain.md (EIP-7549); the beacon_attestation_{subnet_id} gossip message
+    committee_index: int
+    attester_index: int
+    data: AttestationData              # data.index == 0
+    signature: bytes
+
+
+@dataclass
 class BlockAttestations:               # the attestations of one block (BeaconBlockBody.attestations, :639) and what processing them needs
     slot: int                          # the block's slot: state.slot when process_block runs
     proposer_index: int                # the block's proposer, credited with the proposer rewards (:753-754)
@@ -361,6 +369,12 @@ def serialize_attestation_electra(att: ElectraAttestation) -> bytes:
     bl = bytearray(pack_bits([list(att.aggregation_bits)], stride=n // 8 + 1)[0].tobytes())
     bl[n >> 3] |= 1 << (n & 7)
     return (228 + len(cb)).to_bytes(4, "little") + serialize_attestation_data(att.data) + bytes(att.signature) + cb + bytes(bl)
+
+
+def serialize_single_attestation(att: SingleAttestation) -> bytes:
+    """SSZ wire form, 240 fixed bytes: [committee_index u64][attester_index u64][data][signature]."""
+    return (int(att.committee_index).to_bytes(8, "little") + int(att.attester_index).to_bytes(8, "little") + serialize_attestation_data(att.data)
+            + bytes(att.signature))
 
 
 def serialize_aggregate_and_proof(m: AggregateAndProof) -> bytes:

@@ -4,6 +4,7 @@ vote a different head of the 10 000-block tree, each member signing its vote's r
 
     python tools/epoch_intake_bench.py [--epochs 20] [--rounds 3] [--depth 3]
     python tools/epoch_intake_bench.py --profile         # one torch.profiler pass per case: the split over the intake's kernels
+    python tools/epoch_intake_bench.py --form electra    # the same epochs also as Electra SingleAttestations, beside the phase 0 form
 
 Reported per case:
   intake_ms            device time of Engine.attestation_intake_dev (CUDA events around --epochs back-to-back calls, median and range
@@ -12,6 +13,9 @@ Reported per case:
                        each epoch ("intake"), against the same epoch fed the votes one intake produced beforehand ("precomputed"),
                        alternating in one process (CUDA events around each batch, fill and drain included);
   host_numpy_ms        the numpy oracle (tests/intake_oracle.intake_numpy) computing the same outputs on this host's CPU (one run).
+With --form electra every case also holds the same votes as 2^20 SingleAttestations (data.index = 0, signed as such, on their committees'
+subnets), and adds single_intake_ms (Engine.single_attestation_intake_dev, as intake_ms) and ms_per_epoch_single_intake (the pipelined
+epoch fed by EpochProcessor.intake_single_dev), alternating with the phase 0 rows; --profile then splits both calls.
 Every kept attestation must be status 0 and every vote must verify.  Prints one JSON line with the card's name and power limit, read in
 the same run.  Writes nothing."""
 import argparse
@@ -42,8 +46,9 @@ def _tree_slots(parent):
     return slot
 
 
-def _epoch(eng, W, slot, n_votes_per, epoch):
-    """uint8[n, L] wire records of one epoch in random order"""
+def _epoch(eng, W, slot, n_votes_per, epoch, electra=False):
+    """uint8[n, L] wire records of one epoch in random order and its vote count; electra: 240-byte SingleAttestations of data with
+    data.index = 0, and the subnet of each record"""
     import intake_oracle as IO
     parent, roots, _ = W["tree"]
     A, C = bench.N_AGG, bench.COMMITTEE_SIZE
@@ -57,12 +62,21 @@ def _epoch(eng, W, slot, n_votes_per, epoch):
         for v in range(n_votes_per):
             h = int(near[(k + 17 * v) % len(near)])
             t = IO.ancestor(parent, slot, h, start)
-            data[k, v] = np.frombuffer(IO.data128(s, k % cps, bytes(roots[h]), epoch - 1, bytes(roots[0]), epoch, bytes(roots[t])), np.uint8)
+            data[k, v] = np.frombuffer(IO.data128(s, 0 if electra else k % cps, bytes(roots[h]), epoch - 1, bytes(roots[0]), epoch,
+                                                  bytes(roots[t])), np.uint8)
     msgs = eng.signing_roots(data.reshape(-1, 128), np.frombuffer(DOMAIN, np.uint8))
     com = np.repeat(np.arange(A, dtype=np.int64), C)
     pos = np.tile(np.arange(C), A)
     vote = com * n_votes_per + rng.integers(0, n_votes_per, size=A * C)
     sigs = eng.sign(_secret_keys(W)[W["members"]], vote.astype(np.uint32), msgs)
+    if electra:                       # committee k's members are W["members"][k * C .. (k + 1) * C)
+        rec = np.zeros((A * C, 240), dtype=np.uint8)
+        rec[:, 0:8] = (com % cps).astype("<u8").view(np.uint8).reshape(-1, 8)
+        rec[:, 8:16] = W["members"].astype("<u8").view(np.uint8).reshape(-1, 8)
+        rec[:, 16:144] = data.reshape(-1, 128)[vote]
+        rec[:, 144:240] = sigs
+        order = rng.permutation(A * C)
+        return rec[order], A * n_votes_per, (com % 64).astype(np.uint32)[order]      # compute_subnet_for_attestation = k % 64 here
     L = 228 + C // 8 + 1
     rec = np.zeros((A * C, L), dtype=np.uint8)
     rec[:, 0] = 228
@@ -79,6 +93,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--depth", type=int, default=3)
     ap.add_argument("--profile", action="store_true")
+    ap.add_argument("--form", choices=("phase0", "electra"), default="phase0")
     a = ap.parse_args()
     import torch
     import intake_oracle as IO
@@ -99,7 +114,9 @@ def main():
     ep = EpochProcessor(eng, A, bench.N_VAL, C // 8, bench.N_BLOCKS, device=dev, depth=a.depth, max_votes=A * max(CASES))
     ep.set_committees(W["members"], W["off"])
     side = torch.cuda.Stream()
-    result = {"validators": bench.N_VAL, "committees": A, "committee_size": C, "depth": a.depth, "attestations": A * C}
+    electra = a.form == "electra"
+    assert not electra or np.array_equal(W["off"], np.arange(A + 1) * C)
+    result = {"validators": bench.N_VAL, "committees": A, "committee_size": C, "depth": a.depth, "attestations": A * C, "form": a.form}
     rows = {}
     for n_votes_per in CASES:
         rec, n_votes = _epoch(eng, W, slot, n_votes_per, epoch)
@@ -110,11 +127,24 @@ def main():
         with torch.cuda.stream(side):
             pre = ep.intake_dev(*args)
         assert bool((pre.status == 0).all()) and int(pre.vote_off[-1]) == n_votes
+        if electra:
+            rec1, _, sub1 = _epoch(eng, W, slot, n_votes_per, epoch, electra=True)
+            d_wire1 = torch.as_tensor(rec1.reshape(-1), device=dev)
+            d_woff1 = torch.as_tensor((np.arange(rec1.shape[0] + 1, dtype=np.int64) * 240).astype(np.int32), device=dev)
+            d_sub1 = torch.as_tensor(sub1.view(np.int32), device=dev)
+            args1 = (d_wire1, d_woff1, d_sub1, epoch, current_slot, DOMAIN, cps, spe)
+            with torch.cuda.stream(side):
+                pre1 = ep.intake_single_dev(*args1)
+            assert bool((pre1.status == 0).all()) and np.array_equal(pre1.vote_off, pre.vote_off)
+            assert torch.equal(pre1.vote, pre.vote)         # the same votes (the signatures differ: data.index is 0 in what they sign)
 
         def pipelined(n, fresh):
             out, inputs = [], []          # every epoch's intake stays alive until its ticket has been waited for
             for i in range(n):
-                if fresh:
+                if fresh == "single":
+                    with torch.cuda.stream(side):
+                        r = ep.intake_single_dev(*args1)
+                elif fresh:
                     with torch.cuda.stream(side):
                         r = ep.intake_dev(*args)
                 else:
@@ -135,37 +165,49 @@ def main():
             for _ in range(n):
                 eng.attestation_intake_dev(d_wire, d_woff, ep.d_off, epoch, current_slot, DOMAIN, cps, spe, C // 8, *outs)
 
-        for fresh in (True, False):                       # warm-up: every shape of the timed window
+        def single_intake_only(n):
+            for _ in range(n):
+                eng.single_attestation_intake_dev(d_wire1, d_woff1, d_sub1, ep.d_members, ep.d_off, epoch, current_slot, DOMAIN, cps, spe,
+                                                  C // 8, *outs)
+
+        feeds = (True, False, "single") if electra else (True, False)
+        for fresh in feeds:                               # warm-up: every shape of the timed window
             assert all(bool(x.all()) for x in pipelined(a.depth + 2, fresh)), "every vote of the warm-up must verify"
         intake_only(3)
+        if electra:
+            single_intake_only(3)
         torch.cuda.synchronize()
         row = {"n_votes": n_votes}
         if a.profile:
             from torch.profiler import ProfilerActivity, profile
-            with profile(activities=[ProfilerActivity.CUDA]) as prof:
-                intake_only(a.epochs)
-                torch.cuda.synchronize()
-            split = {}
-            for ev in prof.key_averages():
-                total_us = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0)
-                if total_us > 0 and ("k_intake" in ev.key or "Memset" in ev.key):
-                    split[ev.key.split("(")[0][:60]] = round(total_us / 1e3 / a.epochs, 4)
-            row["device_ms_per_intake"] = split
+            for name, fn in [("device_ms_per_intake", intake_only)] + ([("device_ms_per_single_intake", single_intake_only)] if electra else []):
+                with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                    fn(a.epochs)
+                    torch.cuda.synchronize()
+                split = {}
+                for ev in prof.key_averages():
+                    total_us = getattr(ev, "device_time_total", None) or getattr(ev, "cuda_time_total", 0)
+                    if total_us > 0 and ("k_intake" in ev.key or "k_single" in ev.key or "Memset" in ev.key):
+                        split[ev.key.split("(")[0][:60]] = round(total_us / 1e3 / a.epochs, 4)
+                row[name] = split
         else:
-            ms = {"intake": [], "precomputed": [], "intake_only": []}
+            names = ("intake", "precomputed", "intake_only") + (("single_intake", "single_intake_only") if electra else ())
+            ms = {name: [] for name in names}
             for _ in range(a.rounds):
-                for name in ("intake", "precomputed", "intake_only"):
+                for name in names:
                     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                     torch.cuda.synchronize()
                     e0.record()
                     if name == "intake_only":
                         intake_only(a.epochs)
+                    elif name == "single_intake_only":
+                        single_intake_only(a.epochs)
                     else:
-                        ok = pipelined(a.epochs, name == "intake")
+                        ok = pipelined(a.epochs, "single" if name == "single_intake" else name == "intake")
                     e1.record()
                     torch.cuda.synchronize()
                     ms[name].append(e0.elapsed_time(e1) / a.epochs)
-                    if name != "intake_only":
+                    if not name.endswith("intake_only"):
                         assert all(bool(x.all()) for x in ok), (name, n_votes_per, "every vote must verify")
             med = {k: float(np.median(v)) for k, v in ms.items()}
             t0 = time.perf_counter()
@@ -177,8 +219,15 @@ def main():
                         "ms_range_intake": [round(min(ms["intake"]), 3), round(max(ms["intake"]), 3)],
                         "ms_range_precomputed": [round(min(ms["precomputed"]), 3), round(max(ms["precomputed"]), 3)],
                         "host_numpy_ms": round(host_ms, 1)})
+            if electra:
+                row.update({"single_intake_ms": round(med["single_intake_only"], 3),
+                            "single_intake_ms_range": [round(min(ms["single_intake_only"]), 3), round(max(ms["single_intake_only"]), 3)],
+                            "ms_per_epoch_single_intake": round(med["single_intake"], 3),
+                            "ms_range_single_intake": [round(min(ms["single_intake"]), 3), round(max(ms["single_intake"]), 3)]})
         rows["%dv" % n_votes_per] = row
         del d_wire, pre
+        if electra:
+            del d_wire1, pre1
     result.update({"epochs_per_round": a.epochs, "rounds": a.rounds, "cases": rows, "host_cpu": os.cpu_count()})
     assert eng.guard_flags() == 0
     result["gpu"], result["power_limit"] = _card()
