@@ -1709,49 +1709,65 @@ int b2_aggregate_and_proof_intake(b2_ctx* ctx, const uint8_t* wire, uint64_t wir
     return st.finish();
 }
 
-// ------------------------------------------------------------------------------------------ block attestations (blockatt.cuh)
+// ------------------------------------------------------------------------------------------ block attestations (blockatt.cuh, blockatt_electra.cuh)
+// The phase 0 call (b2_block_attestations) and the Electra call (b2_block_attestations_electra) differ only in the decode and checks
+// 1-12 of each attestation (k_ba_parse, or k_bae_parse and k_bae_rows) and in the member rows those write; the argument checks, the
+// signature check, block atomicity, the flag scatter and the proposer rewards are one sequence for both.
 static uint32_t isqrt_u32(uint32_t n) {
     uint32_t x = 0;
     while ((uint64_t)(x + 1) * (x + 1) <= n) x++;
     return x;
 }
+// R: the Electra member rows' padded length, a whole number of split-sum chunks
+static uint64_t bae_row(uint32_t row_max) { return (uint64_t)BAE_CHUNK * (((uint64_t)row_max + BAE_CHUNK - 1) / BAE_CHUNK); }
 
-static int check_block_attestations(b2_ctx* ctx, const void* wire, const void* woff, uint32_t n_att, const void* block_off, const void* block_slot,
-                                    uint32_t n_blocks, const void* members, const void* off, uint32_t n_committees, uint32_t cps_prev, uint32_t cps_cur,
-                                    const void* chain_roots, const void* justified80, const void* domains64, uint32_t slots_per_epoch,
-                                    uint32_t min_inclusion_delay, uint32_t bits_stride, uint64_t effective_balance_increment, const void* status_out,
+// A call's form and member-row shape.  Phase 0: bits_stride, the committees' bit-row stride.  Electra: M committees per slot of at most
+// max_vpc members each, and row_max, the largest member count of one slot's committees (the host form derives it from off).
+struct ba_form {
+    bool electra;
+    uint32_t bits_stride, M, max_vpc, row_max;
+    const char* what() const { return electra ? "block_attestations_electra" : "block_attestations"; }
+    uint64_t width() const { return electra ? bae_row(row_max) : 8ull * bits_stride; }      // members per attestation row
+};
+
+// what both calls take alike: everything but the member-row shape
+static int check_block_attestations(b2_ctx* ctx, const char* what, const void* wire, const void* woff, uint32_t n_att, const void* block_off,
+                                    const void* block_slot, uint32_t n_blocks, const void* members, const void* off, uint32_t n_committees,
+                                    uint32_t cps_prev, uint32_t cps_cur, const void* chain_roots, const void* justified80, const void* domains64,
+                                    uint32_t slots_per_epoch, uint32_t min_inclusion_delay, uint64_t effective_balance_increment, const void* status_out,
                                     const void* flag_mask_out, const void* numerator_out, const void* block_status_out, const void* block_first_out,
                                     const void* block_reward_out, const void* n_applied_out) {
-    REQUIRE(ctx && wire && woff && block_off && block_slot && members && off && chain_roots && justified80 && domains64 && status_out && flag_mask_out &&
-                numerator_out && block_status_out && block_first_out && block_reward_out && n_applied_out && n_att > 0 && n_att < (1u << 28) &&
-                n_blocks > 0 && bits_stride > 0 && bits_stride <= 256 && (uint64_t)n_att * 8 * bits_stride < (1ull << 32) && slots_per_epoch > 0 &&
-                cps_cur > 0 && ((uint64_t)cps_prev + cps_cur) * slots_per_epoch < (1ull << 31) && min_inclusion_delay > 0 &&
-                effective_balance_increment > 0,
-            "block_attestations: bad arguments");
-    REQUIRE(((uint64_t)cps_prev + cps_cur) * slots_per_epoch == n_committees,
-            "block_attestations: n_committees must be slots_per_epoch * (cps_prev + cps_cur)");
-    REQUIRE(ctx->n_val > 0, "block_attestations: registry not loaded");
-    return ctx->reg.part[0] && ctx->reg.part[1] ? B2_OK
-                                                : reject(ctx, "block_attestations", "both participation tables must be loaded (b2_participation_load)");
+    if (!ctx) return B2_EINVAL;
+    if (!(wire && woff && block_off && block_slot && members && off && chain_roots && justified80 && domains64 && status_out && flag_mask_out &&
+          numerator_out && block_status_out && block_first_out && block_reward_out && n_applied_out && n_att > 0 && n_att < (1u << 28) &&
+          n_blocks > 0 && slots_per_epoch > 0 && cps_cur > 0 && ((uint64_t)cps_prev + cps_cur) * slots_per_epoch < (1ull << 31) &&
+          min_inclusion_delay > 0 && effective_balance_increment > 0))
+        return reject(ctx, what, "bad arguments");
+    if (((uint64_t)cps_prev + cps_cur) * slots_per_epoch != n_committees)
+        return reject(ctx, what, "n_committees must be slots_per_epoch * (cps_prev + cps_cur)");
+    if (ctx->n_val == 0) return reject(ctx, what, "registry not loaded");
+    return ctx->reg.part[0] && ctx->reg.part[1] ? B2_OK : reject(ctx, what, "both participation tables must be loaded (b2_participation_load)");
 }
-int b2_block_attestations_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n_att, const uint32_t* d_block_off,
-                              const uint64_t* d_block_slot, uint32_t n_blocks, const uint32_t* d_members, const uint32_t* d_off, uint32_t n_committees,
-                              uint64_t n_sig,
-                              uint32_t cps_prev, uint32_t cps_cur, const uint8_t* d_chain_roots, const uint8_t* justified80, const uint8_t* domains64,
-                              uint32_t slots_per_epoch, uint32_t min_inclusion_delay, uint32_t bits_stride, uint64_t effective_balance_increment,
-                              uint64_t base_reward_per_increment, int32_t* d_status_out, uint8_t* d_flag_mask_out, uint64_t* d_numerator_out,
-                              int32_t* d_block_status_out, uint32_t* d_block_first_out, uint64_t* d_block_reward_out, uint32_t* d_n_applied_out,
-                              void* stream) {
-    B2_NVTX;
-    int rc;
-    if ((rc = check_block_attestations(ctx, d_wire, d_woff, n_att, d_block_off, d_block_slot, n_blocks, d_members, d_off, n_committees, cps_prev, cps_cur, d_chain_roots,
-                                       justified80, domains64, slots_per_epoch, min_inclusion_delay, bits_stride, effective_balance_increment, d_status_out,
-                                       d_flag_mask_out, d_numerator_out, d_block_status_out, d_block_first_out, d_block_reward_out, d_n_applied_out)))
-        return rc;
-    REQUIRE(n_sig < (1ull << 32), "block_attestations: n_sig does not fit 32 bits");      // the host form's n_sig is a u32 offset
+// the form's member-row shape; every row of the call fits u32 member offsets
+static int check_ba_shape(b2_ctx* ctx, uint32_t n_att, const ba_form& f) {
+    const bool ok = f.electra ? f.M >= 1 && f.M <= 64 && f.max_vpc > 0 && (uint64_t)f.max_vpc * f.M < (1ull << 31) && f.row_max > 0
+                              : f.bits_stride > 0 && f.bits_stride <= 256;
+    return ok && n_att * f.width() < (1ull << 32) ? B2_OK : reject(ctx, f.what(), "bad arguments");
+}
+
+// Both calls after their argument checks; only the parse step depends on the form.
+static int block_attestations_enqueue(b2_ctx* ctx, const ba_form& f, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n_att,
+                                      const uint32_t* d_block_off, const uint64_t* d_block_slot, uint32_t n_blocks, const uint32_t* d_members,
+                                      const uint32_t* d_off, uint64_t n_sig, uint32_t cps_prev, uint32_t cps_cur, const uint8_t* d_chain_roots,
+                                      const uint8_t* justified80, const uint8_t* domains64, uint32_t slots_per_epoch, uint32_t min_inclusion_delay,
+                                      uint64_t effective_balance_increment, uint64_t base_reward_per_increment, int32_t* d_status_out,
+                                      uint8_t* d_flag_mask_out, uint64_t* d_numerator_out, int32_t* d_block_status_out, uint32_t* d_block_first_out,
+                                      uint64_t* d_block_reward_out, uint32_t* d_n_applied_out, void* stream) {
+    if (n_sig >= (1ull << 32)) return reject(ctx, f.what(), "n_sig does not fit 32 bits");      // the host form's n_sig is a u32 offset
     CK(cudaSetDevice(ctx->device));
-    const size_t n = n_att, W = 8ull * bits_stride;
-    ba_args A = {};
+    const size_t n = n_att, W = f.width();
+    bae_args E = {};      // the Electra kernels' arguments; the phase 0 ones are E.B
+    ba_args& A = E.B;
     A.wire = d_wire;
     A.wire_len = wire_len;
     A.woff = d_woff;
@@ -1762,11 +1778,11 @@ int b2_block_attestations_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_
     A.members = d_members;
     A.T.off = d_off;
     A.T.n_sig = n_sig;
-    A.T.bits_stride = bits_stride;
+    A.T.bits_stride = (uint32_t)(W / 8);
     A.cps_prev = cps_prev;
     A.cps_cur = cps_cur;
     A.slots_per_epoch = slots_per_epoch;
-    A.bits_stride = bits_stride;
+    A.bits_stride = (uint32_t)(W / 8);
     A.min_delay = min_inclusion_delay;
     A.isqrt_spe = isqrt_u32(slots_per_epoch);
     A.chain_roots = d_chain_roots;
@@ -1783,108 +1799,77 @@ int b2_block_attestations_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_
     A.guard = ctx->d_guard;
     uint8_t* msg32;
     scratch sc(ctx, ctx->ba);
-    sc(A.blk_of, n); sc(A.cur, n); sc(A.fav_ok, n); sc(A.accept, 2 * n); sc(A.num1, n); sc(A.bits, n * bits_stride, 16);
+    sc(A.blk_of, n); sc(A.cur, n); sc(A.fav_ok, n); sc(A.accept, 2 * n); sc(A.num1, n); sc(A.bits, n * W / 8, 16);
     sc(A.sig96, n * 96); sc(A.data128, n * 128); sc(A.dom32, n * 32); sc(msg32, n * 32); sc(A.members_out, n * W); sc(A.item_off, n + 1);
+    // FastAggregateVerify's keys: each member row, or in the Electra form the split sum over its BAE_CHUNK-member chunks
+    pk_source P = {A.members_out, A.item_off, A.bits, A.bits_stride, nullptr, 0};
+    if (f.electra) {
+        E.M = f.M;
+        E.max_vpc = f.max_vpc;
+        E.row_max = f.row_max;
+        E.R = (uint32_t)W;
+        E.n_chunks = (uint32_t)(W / BAE_CHUNK);
+        E.n_sig = n_sig;
+        E.off = d_off;
+        uint8_t* part_st;
+        uint32_t* part_jac;
+        sc(E.nbits, n); sc(E.c0, n); sc(E.cmask, n); sc(E.chunk_off, n * E.n_chunks + 1); sc(part_jac, n * E.n_chunks * 36); sc(part_st, n * E.n_chunks);
+        P = {A.members_out, E.chunk_off, A.bits, BAE_CHUNK / 8, nullptr, 0, nullptr, nullptr, E.n_chunks, part_jac, part_st};
+    }
     if (sc.rc) return sc.rc;
     cudaStream_t s = (cudaStream_t)stream;
-    k_ba_parse<<<blocks_for((uint64_t)n_att * 32, 128), 128, 0, s>>>(A);
+    if (f.electra) {
+        k_bae_parse<<<blocks_for((uint64_t)n_att * 32, 128), 128, 0, s>>>(E);
+        CKL(ctx);
+        k_bae_rows<<<n_att, 256, 0, s>>>(E);
+    } else {
+        k_ba_parse<<<blocks_for((uint64_t)n_att * 32, 128), 128, 0, s>>>(A);
+    }
     CKL(ctx);
     k_signing_roots<<<blocks_for(n_att, 64), 64, 0, s>>>(A.data128, A.dom32, 32u, n_att, msg32);
     CKL(ctx);
-    pk_source P = {A.members_out, A.item_off, A.bits, bits_stride, nullptr, 0};
+    int rc;
     if ((rc = verify_fork(ctx, ctx->slot[0], P, msg32, n_att, s)) || (rc = verify_main(ctx, ctx->slot[0], A.sig96, n_att, A.fav_ok, s))) return rc;
-    k_ba_blocks<<<1, BA_BLOCKS_THREADS, 0, s>>>(A);
+    k_ba_blocks<<<1, BA_BLOCKS_THREADS, 0, s>>>(A, f.electra ? 13 : 11);      // the status of a failed FastAggregateVerify
     CKL(ctx);
     // the flag scatter of :745-749, order-exact over (block, list) order: table 0 (target e) writes `numerator`, table 1 (target e - 1) num1
     const registry_tables& R = ctx->reg;
-    const uint8_t* db = A.bits;
     for (int which = 0; which < 2; which++) {
         const uint8_t* acc = A.accept + (size_t)which * n;
-        unsigned long long* num = which == 0 ? (unsigned long long*)d_numerator_out : A.num1;
-        k_part_phase1<<<n_att, 128, 0, s>>>(A.members_out, A.item_off, db, bits_stride, d_flag_mask_out, acc, n_att, R.part[which], R.part_first);
+        unsigned long long* num = which == 0 ? A.numerator : A.num1;
+        k_part_phase1<<<n_att, 128, 0, s>>>(A.members_out, A.item_off, A.bits, A.bits_stride, d_flag_mask_out, acc, n_att, R.part[which], R.part_first);
         CKL(ctx);
-        k_part_phase2<<<n_att, 128, 0, s>>>(A.members_out, A.item_off, db, bits_stride, d_flag_mask_out, acc, n_att, R.part_first, R.eff,
+        k_part_phase2<<<n_att, 128, 0, s>>>(A.members_out, A.item_off, A.bits, A.bits_stride, d_flag_mask_out, acc, n_att, R.part_first, R.eff,
                                             effective_balance_increment, base_reward_per_increment, num);
         CKL(ctx);
-        k_part_phase3<<<n_att, 128, 0, s>>>(A.members_out, A.item_off, db, bits_stride, d_flag_mask_out, acc, n_att, R.part_first, R.part[which]);
+        k_part_phase3<<<n_att, 128, 0, s>>>(A.members_out, A.item_off, A.bits, A.bits_stride, d_flag_mask_out, acc, n_att, R.part_first, R.part[which]);
         CKL(ctx);
     }
     k_ba_rewards<<<blocks_for((uint64_t)n_blocks * 32, 128), 128, 0, s>>>(A);
     CKL(ctx);
     return B2_OK;
 }
-
-int b2_block_attestations(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n_att, const uint32_t* block_off,
-                          const uint64_t* block_slot, uint32_t n_blocks, const uint32_t* members, const uint32_t* off, uint32_t n_committees, uint32_t cps_prev,
-                          uint32_t cps_cur, const uint8_t* chain_roots, const uint8_t* justified80, const uint8_t* domains64, uint32_t slots_per_epoch,
-                          uint32_t min_inclusion_delay, uint32_t bits_stride, uint64_t effective_balance_increment, uint64_t base_reward_per_increment,
-                          int32_t* status_out, uint8_t* flag_mask_out, uint64_t* numerator_out, int32_t* block_status_out, uint32_t* block_first_out,
-                          uint64_t* block_reward_out, uint32_t* n_applied_out) {
+int b2_block_attestations_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n_att, const uint32_t* d_block_off,
+                              const uint64_t* d_block_slot, uint32_t n_blocks, const uint32_t* d_members, const uint32_t* d_off, uint32_t n_committees,
+                              uint64_t n_sig,
+                              uint32_t cps_prev, uint32_t cps_cur, const uint8_t* d_chain_roots, const uint8_t* justified80, const uint8_t* domains64,
+                              uint32_t slots_per_epoch, uint32_t min_inclusion_delay, uint32_t bits_stride, uint64_t effective_balance_increment,
+                              uint64_t base_reward_per_increment, int32_t* d_status_out, uint8_t* d_flag_mask_out, uint64_t* d_numerator_out,
+                              int32_t* d_block_status_out, uint32_t* d_block_first_out, uint64_t* d_block_reward_out, uint32_t* d_n_applied_out,
+                              void* stream) {
     B2_NVTX;
+    const ba_form f = {false, bits_stride, 0, 0, 0};
     int rc;
-    if ((rc = check_block_attestations(ctx, wire, woff, n_att, block_off, block_slot, n_blocks, members, off, n_committees, cps_prev, cps_cur, chain_roots, justified80,
-                                       domains64, slots_per_epoch, min_inclusion_delay, bits_stride, effective_balance_increment, status_out, flag_mask_out,
-                                       numerator_out, block_status_out, block_first_out, block_reward_out, n_applied_out)) ||
-        (rc = check_wire(ctx, woff, n_att, wire_len, "block_attestations")) ||
-        (rc = check_offsets(ctx, block_off, n_blocks, "block_attestations", "block_off")))
+    if ((rc = check_block_attestations(ctx, f.what(), d_wire, d_woff, n_att, d_block_off, d_block_slot, n_blocks, d_members, d_off, n_committees, cps_prev,
+                                       cps_cur, d_chain_roots, justified80, domains64, slots_per_epoch, min_inclusion_delay, effective_balance_increment,
+                                       d_status_out, d_flag_mask_out, d_numerator_out, d_block_status_out, d_block_first_out, d_block_reward_out,
+                                       d_n_applied_out)) ||
+        (rc = check_ba_shape(ctx, n_att, f)))
         return rc;
-    REQUIRE(block_off[n_blocks] == n_att, "block_attestations: block_off must end at n_att");
-    const uint64_t e = block_slot[0] / slots_per_epoch;
-    REQUIRE(block_slot[0] < (1ull << 63), "block_attestations: block slot out of range");
-    for (uint32_t b = 1; b < n_blocks; b++)
-        REQUIRE(block_slot[b] > block_slot[b - 1] && block_slot[b] / slots_per_epoch == e,
-                "block_attestations: block slots must increase strictly and lie in one epoch");
-    REQUIRE(e > 0 ? cps_prev > 0 : cps_prev == 0, "block_attestations: cps_prev must be 0 exactly at epoch 0");
-    if ((rc = check_committees(ctx, off, n_committees, bits_stride, "block_attestations"))) return rc;
-    const uint64_t n_sig = off[n_committees];
-    CK(cudaSetDevice(ctx->device));
-    staging st(ctx);
-    const uint8_t* dwire = st.in(wire, wire_len, 16);
-    const uint32_t* dwoff = st.in(woff, (size_t)n_att + 1);
-    const uint32_t* dboff = st.in(block_off, (size_t)n_blocks + 1);
-    const uint64_t* dbslot = st.in(block_slot, n_blocks);
-    const uint32_t* dmem = st.in(members, n_sig, 4);
-    const uint32_t* doff = st.in(off, (size_t)n_committees + 1);
-    const uint8_t* droots = st.in(chain_roots, 64ull * slots_per_epoch);
-    int32_t* dst = st.out(status_out, n_att);
-    uint8_t* dmask = st.out(flag_mask_out, n_att);
-    uint64_t* dnum = st.out(numerator_out, n_att);
-    int32_t* dbst = st.out(block_status_out, n_blocks);
-    uint32_t* dbfirst = st.out(block_first_out, n_blocks);
-    uint64_t* dbrew = st.out(block_reward_out, n_blocks);
-    uint32_t* dnapp = st.out(n_applied_out, 1);
-    if (st.rc) return st.rc;
-    if ((rc = b2_block_attestations_dev(ctx, dwire, wire_len, dwoff, n_att, dboff, dbslot, n_blocks, dmem, doff, n_committees, n_sig, cps_prev, cps_cur, droots,
-                                        justified80, domains64, slots_per_epoch, min_inclusion_delay, bits_stride, effective_balance_increment,
-                                        base_reward_per_increment, dst, dmask, dnum, dbst, dbfirst, dbrew, dnapp, ctx->s_main)))
-        return rc;
-    return st.finish();
-}
-
-// ------------------------------------------------------------------------------------------ Electra block attestations (blockatt_electra.cuh)
-// R: the member rows' padded length, a whole number of split-sum chunks
-static uint64_t bae_row(uint32_t row_max) { return (uint64_t)BAE_CHUNK * (((uint64_t)row_max + BAE_CHUNK - 1) / BAE_CHUNK); }
-
-static int check_block_attestations_electra(b2_ctx* ctx, const void* wire, const void* woff, uint32_t n_att, const void* block_off, const void* block_slot,
-                                            uint32_t n_blocks, const void* members, const void* off, uint32_t n_committees, uint32_t cps_prev,
-                                            uint32_t cps_cur, const void* chain_roots, const void* justified80, const void* domains64,
-                                            uint32_t slots_per_epoch, uint32_t min_inclusion_delay, uint32_t max_committees_per_slot,
-                                            uint32_t max_validators_per_committee, uint32_t row_max, uint64_t effective_balance_increment,
-                                            const void* status_out, const void* flag_mask_out, const void* numerator_out, const void* block_status_out,
-                                            const void* block_first_out, const void* block_reward_out, const void* n_applied_out) {
-    REQUIRE(ctx && wire && woff && block_off && block_slot && members && off && chain_roots && justified80 && domains64 && status_out && flag_mask_out &&
-                numerator_out && block_status_out && block_first_out && block_reward_out && n_applied_out && n_att > 0 && n_att < (1u << 28) &&
-                n_blocks > 0 && max_committees_per_slot >= 1 && max_committees_per_slot <= 64 && max_validators_per_committee > 0 &&
-                (uint64_t)max_validators_per_committee * max_committees_per_slot < (1ull << 31) && row_max > 0 &&
-                (uint64_t)n_att * bae_row(row_max) < (1ull << 32) && slots_per_epoch > 0 && cps_cur > 0 &&
-                ((uint64_t)cps_prev + cps_cur) * slots_per_epoch < (1ull << 31) && min_inclusion_delay > 0 && effective_balance_increment > 0,
-            "block_attestations_electra: bad arguments");
-    REQUIRE(((uint64_t)cps_prev + cps_cur) * slots_per_epoch == n_committees,
-            "block_attestations_electra: n_committees must be slots_per_epoch * (cps_prev + cps_cur)");
-    REQUIRE(ctx->n_val > 0, "block_attestations_electra: registry not loaded");
-    return ctx->reg.part[0] && ctx->reg.part[1]
-               ? B2_OK
-               : reject(ctx, "block_attestations_electra", "both participation tables must be loaded (b2_participation_load)");
+    return block_attestations_enqueue(ctx, f, d_wire, wire_len, d_woff, n_att, d_block_off, d_block_slot, n_blocks, d_members, d_off, n_sig, cps_prev,
+                                      cps_cur, d_chain_roots, justified80, domains64, slots_per_epoch, min_inclusion_delay, effective_balance_increment,
+                                      base_reward_per_increment, d_status_out, d_flag_mask_out, d_numerator_out, d_block_status_out, d_block_first_out,
+                                      d_block_reward_out, d_n_applied_out, stream);
 }
 int b2_block_attestations_electra_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64_t wire_len, const uint32_t* d_woff, uint32_t n_att,
                                       const uint32_t* d_block_off, const uint64_t* d_block_slot, uint32_t n_blocks, const uint32_t* d_members,
@@ -1895,122 +1880,52 @@ int b2_block_attestations_electra_dev(b2_ctx* ctx, const uint8_t* d_wire, uint64
                                       int32_t* d_status_out, uint8_t* d_flag_mask_out, uint64_t* d_numerator_out, int32_t* d_block_status_out,
                                       uint32_t* d_block_first_out, uint64_t* d_block_reward_out, uint32_t* d_n_applied_out, void* stream) {
     B2_NVTX;
+    const ba_form f = {true, 0, max_committees_per_slot, max_validators_per_committee, row_max};
     int rc;
-    if ((rc = check_block_attestations_electra(ctx, d_wire, d_woff, n_att, d_block_off, d_block_slot, n_blocks, d_members, d_off, n_committees, cps_prev,
-                                               cps_cur, d_chain_roots, justified80, domains64, slots_per_epoch, min_inclusion_delay,
-                                               max_committees_per_slot, max_validators_per_committee, row_max, effective_balance_increment,
-                                               d_status_out, d_flag_mask_out, d_numerator_out, d_block_status_out, d_block_first_out,
-                                               d_block_reward_out, d_n_applied_out)))
+    if ((rc = check_block_attestations(ctx, f.what(), d_wire, d_woff, n_att, d_block_off, d_block_slot, n_blocks, d_members, d_off, n_committees, cps_prev,
+                                       cps_cur, d_chain_roots, justified80, domains64, slots_per_epoch, min_inclusion_delay, effective_balance_increment,
+                                       d_status_out, d_flag_mask_out, d_numerator_out, d_block_status_out, d_block_first_out, d_block_reward_out,
+                                       d_n_applied_out)) ||
+        (rc = check_ba_shape(ctx, n_att, f)))
         return rc;
-    REQUIRE(n_sig < (1ull << 32), "block_attestations_electra: n_sig does not fit 32 bits");      // the host form's n_sig is a u32 offset
-    CK(cudaSetDevice(ctx->device));
-    const size_t n = n_att, R = bae_row(row_max), n_chunks = R / BAE_CHUNK;
-    bae_args A = {};
-    ba_args& B = A.B;
-    B.wire = d_wire;
-    B.wire_len = wire_len;
-    B.woff = d_woff;
-    B.n = n_att;
-    B.block_off = d_block_off;
-    B.block_slot = d_block_slot;
-    B.n_blocks = n_blocks;
-    B.members = d_members;
-    B.cps_prev = cps_prev;
-    B.cps_cur = cps_cur;
-    B.slots_per_epoch = slots_per_epoch;
-    B.bits_stride = (uint32_t)(R / 8);
-    B.min_delay = min_inclusion_delay;
-    B.isqrt_spe = isqrt_u32(slots_per_epoch);
-    B.chain_roots = d_chain_roots;
-    memcpy(B.justified.b, justified80, 80);
-    memcpy(B.dom[0].b, domains64, 32);
-    memcpy(B.dom[1].b, domains64 + 32, 32);
-    B.status = d_status_out;
-    B.flag_mask = d_flag_mask_out;
-    B.numerator = (unsigned long long*)d_numerator_out;
-    B.block_status = d_block_status_out;
-    B.block_first = d_block_first_out;
-    B.block_reward = (unsigned long long*)d_block_reward_out;
-    B.n_applied = d_n_applied_out;
-    B.guard = ctx->d_guard;
-    A.M = max_committees_per_slot;
-    A.max_vpc = max_validators_per_committee;
-    A.row_max = row_max;
-    A.R = (uint32_t)R;
-    A.n_chunks = (uint32_t)n_chunks;
-    A.n_sig = n_sig;
-    A.off = d_off;
-    uint8_t *msg32, *part_st;
-    uint32_t* part_jac;
-    scratch sc(ctx, ctx->ba);
-    sc(B.blk_of, n); sc(B.cur, n); sc(B.fav_ok, n); sc(B.accept, 2 * n); sc(B.num1, n); sc(B.bits, n * R / 8, 16);
-    sc(B.sig96, n * 96); sc(B.data128, n * 128); sc(B.dom32, n * 32); sc(msg32, n * 32); sc(B.members_out, n * R); sc(B.item_off, n + 1);
-    sc(A.nbits, n); sc(A.c0, n); sc(A.cmask, n); sc(A.chunk_off, n * n_chunks + 1); sc(part_jac, n * n_chunks * 36); sc(part_st, n * n_chunks);
-    if (sc.rc) return sc.rc;
-    cudaStream_t s = (cudaStream_t)stream;
-    k_bae_parse<<<blocks_for((uint64_t)n_att * 32, 128), 128, 0, s>>>(A);
-    CKL(ctx);
-    k_bae_rows<<<n_att, 256, 0, s>>>(A);
-    CKL(ctx);
-    k_signing_roots<<<blocks_for(n_att, 64), 64, 0, s>>>(B.data128, B.dom32, 32u, n_att, msg32);
-    CKL(ctx);
-    pk_source P = {B.members_out, A.chunk_off, B.bits, BAE_CHUNK / 8, nullptr, 0, nullptr, nullptr, A.n_chunks, part_jac, part_st};
-    if ((rc = verify_fork(ctx, ctx->slot[0], P, msg32, n_att, s)) || (rc = verify_main(ctx, ctx->slot[0], B.sig96, n_att, B.fav_ok, s))) return rc;
-    k_bae_verdicts<<<blocks_for(n_att, 128), 128, 0, s>>>(B.status, B.fav_ok, n_att);
-    CKL(ctx);
-    k_ba_blocks<<<1, BA_BLOCKS_THREADS, 0, s>>>(B);
-    CKL(ctx);
-    // the flag scatter, order-exact over (block, list) order: table 0 (target e) writes `numerator`, table 1 (target e - 1) num1
-    const registry_tables& T = ctx->reg;
-    const uint32_t stride = B.bits_stride;
-    for (int which = 0; which < 2; which++) {
-        const uint8_t* acc = B.accept + (size_t)which * n;
-        unsigned long long* num = which == 0 ? (unsigned long long*)d_numerator_out : B.num1;
-        k_part_phase1<<<n_att, 128, 0, s>>>(B.members_out, B.item_off, B.bits, stride, d_flag_mask_out, acc, n_att, T.part[which], T.part_first);
-        CKL(ctx);
-        k_part_phase2<<<n_att, 128, 0, s>>>(B.members_out, B.item_off, B.bits, stride, d_flag_mask_out, acc, n_att, T.part_first, T.eff,
-                                            effective_balance_increment, base_reward_per_increment, num);
-        CKL(ctx);
-        k_part_phase3<<<n_att, 128, 0, s>>>(B.members_out, B.item_off, B.bits, stride, d_flag_mask_out, acc, n_att, T.part_first, T.part[which]);
-        CKL(ctx);
-    }
-    k_ba_rewards<<<blocks_for((uint64_t)n_blocks * 32, 128), 128, 0, s>>>(B);
-    CKL(ctx);
-    return B2_OK;
+    return block_attestations_enqueue(ctx, f, d_wire, wire_len, d_woff, n_att, d_block_off, d_block_slot, n_blocks, d_members, d_off, n_sig, cps_prev,
+                                      cps_cur, d_chain_roots, justified80, domains64, slots_per_epoch, min_inclusion_delay, effective_balance_increment,
+                                      base_reward_per_increment, d_status_out, d_flag_mask_out, d_numerator_out, d_block_status_out, d_block_first_out,
+                                      d_block_reward_out, d_n_applied_out, stream);
 }
 
-int b2_block_attestations_electra(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n_att, const uint32_t* block_off,
-                                  const uint64_t* block_slot, uint32_t n_blocks, const uint32_t* members, const uint32_t* off, uint32_t n_committees,
-                                  uint32_t cps_prev, uint32_t cps_cur, const uint8_t* chain_roots, const uint8_t* justified80, const uint8_t* domains64,
-                                  uint32_t slots_per_epoch, uint32_t min_inclusion_delay, uint32_t max_committees_per_slot,
-                                  uint32_t max_validators_per_committee, uint64_t effective_balance_increment, uint64_t base_reward_per_increment,
-                                  int32_t* status_out, uint8_t* flag_mask_out, uint64_t* numerator_out, int32_t* block_status_out,
-                                  uint32_t* block_first_out, uint64_t* block_reward_out, uint32_t* n_applied_out) {
-    B2_NVTX;
+// Both host forms: the argument checks, the checks that read the host arrays (the Electra form derives row_max here), stage, enqueue.
+static int block_attestations_host(b2_ctx* ctx, ba_form f, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n_att,
+                                   const uint32_t* block_off, const uint64_t* block_slot, uint32_t n_blocks, const uint32_t* members, const uint32_t* off,
+                                   uint32_t n_committees, uint32_t cps_prev, uint32_t cps_cur, const uint8_t* chain_roots, const uint8_t* justified80,
+                                   const uint8_t* domains64, uint32_t slots_per_epoch, uint32_t min_inclusion_delay, uint64_t effective_balance_increment,
+                                   uint64_t base_reward_per_increment, int32_t* status_out, uint8_t* flag_mask_out, uint64_t* numerator_out,
+                                   int32_t* block_status_out, uint32_t* block_first_out, uint64_t* block_reward_out, uint32_t* n_applied_out) {
+    const char* what = f.what();
     int rc;
-    if ((rc = check_block_attestations_electra(ctx, wire, woff, n_att, block_off, block_slot, n_blocks, members, off, n_committees, cps_prev, cps_cur,
-                                               chain_roots, justified80, domains64, slots_per_epoch, min_inclusion_delay, max_committees_per_slot,
-                                               max_validators_per_committee, 1, effective_balance_increment, status_out, flag_mask_out,
-                                               numerator_out, block_status_out, block_first_out, block_reward_out, n_applied_out)) ||
-        (rc = check_wire(ctx, woff, n_att, wire_len, "block_attestations_electra")) ||
-        (rc = check_offsets(ctx, block_off, n_blocks, "block_attestations_electra", "block_off")) ||
-        (rc = check_offsets(ctx, off, n_committees, "block_attestations_electra")))
+    if ((rc = check_block_attestations(ctx, what, wire, woff, n_att, block_off, block_slot, n_blocks, members, off, n_committees, cps_prev, cps_cur,
+                                       chain_roots, justified80, domains64, slots_per_epoch, min_inclusion_delay, effective_balance_increment, status_out,
+                                       flag_mask_out, numerator_out, block_status_out, block_first_out, block_reward_out, n_applied_out)) ||
+        (rc = check_wire(ctx, woff, n_att, wire_len, what)) || (rc = check_offsets(ctx, block_off, n_blocks, what, "block_off")))
         return rc;
-    REQUIRE(block_off[n_blocks] == n_att, "block_attestations_electra: block_off must end at n_att");
+    if (block_off[n_blocks] != n_att) return reject(ctx, what, "block_off must end at n_att");
     const uint64_t e = block_slot[0] / slots_per_epoch;
-    REQUIRE(block_slot[0] < (1ull << 63), "block_attestations_electra: block slot out of range");
+    if (block_slot[0] >= (1ull << 63)) return reject(ctx, what, "block slot out of range");
     for (uint32_t b = 1; b < n_blocks; b++)
-        REQUIRE(block_slot[b] > block_slot[b - 1] && block_slot[b] / slots_per_epoch == e,
-                "block_attestations_electra: block slots must increase strictly and lie in one epoch");
-    REQUIRE(e > 0 ? cps_prev > 0 : cps_prev == 0, "block_attestations_electra: cps_prev must be 0 exactly at epoch 0");
-    // the largest member count of one slot's committees: the slots of e - 1 (cps_prev rows each), then those of e (cps_cur rows each)
-    uint32_t row_max = 1;
-    for (uint32_t s = 0; s < 2 * slots_per_epoch; s++) {
-        const uint32_t cps = s < slots_per_epoch ? cps_prev : cps_cur;
-        const uint32_t c = s < slots_per_epoch ? s * cps_prev : cps_prev * slots_per_epoch + (s - slots_per_epoch) * cps_cur;
-        row_max = std::max(row_max, off[c + cps] - off[c]);
+        if (block_slot[b] <= block_slot[b - 1] || block_slot[b] / slots_per_epoch != e)
+            return reject(ctx, what, "block slots must increase strictly and lie in one epoch");
+    if (e > 0 ? cps_prev == 0 : cps_prev != 0) return reject(ctx, what, "cps_prev must be 0 exactly at epoch 0");
+    if (f.electra) {
+        if ((rc = check_offsets(ctx, off, n_committees, what))) return rc;
+        // the largest member count of one slot's committees: the slots of e - 1 (cps_prev rows each), then those of e (cps_cur rows each)
+        f.row_max = 1;
+        for (uint32_t s = 0; s < 2 * slots_per_epoch; s++) {
+            const uint32_t cps = s < slots_per_epoch ? cps_prev : cps_cur;
+            const uint32_t c = s < slots_per_epoch ? s * cps_prev : cps_prev * slots_per_epoch + (s - slots_per_epoch) * cps_cur;
+            f.row_max = std::max(f.row_max, off[c + cps] - off[c]);
+        }
     }
-    REQUIRE((uint64_t)n_att * bae_row(row_max) < (1ull << 32), "block_attestations_electra: n_att times the padded row exceeds 2^32 members");
+    if ((rc = check_ba_shape(ctx, n_att, f)) || (!f.electra && (rc = check_committees(ctx, off, n_committees, f.bits_stride, what)))) return rc;
     const uint64_t n_sig = off[n_committees];
     CK(cudaSetDevice(ctx->device));
     staging st(ctx);
@@ -2029,12 +1944,36 @@ int b2_block_attestations_electra(b2_ctx* ctx, const uint8_t* wire, uint64_t wir
     uint64_t* dbrew = st.out(block_reward_out, n_blocks);
     uint32_t* dnapp = st.out(n_applied_out, 1);
     if (st.rc) return st.rc;
-    if ((rc = b2_block_attestations_electra_dev(ctx, dwire, wire_len, dwoff, n_att, dboff, dbslot, n_blocks, dmem, doff, n_committees, n_sig, cps_prev,
-                                                cps_cur, droots, justified80, domains64, slots_per_epoch, min_inclusion_delay, max_committees_per_slot,
-                                                max_validators_per_committee, row_max, effective_balance_increment, base_reward_per_increment, dst,
-                                                dmask, dnum, dbst, dbfirst, dbrew, dnapp, ctx->s_main)))
+    if ((rc = block_attestations_enqueue(ctx, f, dwire, wire_len, dwoff, n_att, dboff, dbslot, n_blocks, dmem, doff, n_sig, cps_prev, cps_cur, droots,
+                                         justified80, domains64, slots_per_epoch, min_inclusion_delay, effective_balance_increment,
+                                         base_reward_per_increment, dst, dmask, dnum, dbst, dbfirst, dbrew, dnapp, ctx->s_main)))
         return rc;
     return st.finish();
+}
+int b2_block_attestations(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n_att, const uint32_t* block_off,
+                          const uint64_t* block_slot, uint32_t n_blocks, const uint32_t* members, const uint32_t* off, uint32_t n_committees, uint32_t cps_prev,
+                          uint32_t cps_cur, const uint8_t* chain_roots, const uint8_t* justified80, const uint8_t* domains64, uint32_t slots_per_epoch,
+                          uint32_t min_inclusion_delay, uint32_t bits_stride, uint64_t effective_balance_increment, uint64_t base_reward_per_increment,
+                          int32_t* status_out, uint8_t* flag_mask_out, uint64_t* numerator_out, int32_t* block_status_out, uint32_t* block_first_out,
+                          uint64_t* block_reward_out, uint32_t* n_applied_out) {
+    B2_NVTX;
+    return block_attestations_host(ctx, {false, bits_stride, 0, 0, 0}, wire, wire_len, woff, n_att, block_off, block_slot, n_blocks, members, off,
+                                   n_committees, cps_prev, cps_cur, chain_roots, justified80, domains64, slots_per_epoch, min_inclusion_delay,
+                                   effective_balance_increment, base_reward_per_increment, status_out, flag_mask_out, numerator_out, block_status_out,
+                                   block_first_out, block_reward_out, n_applied_out);
+}
+int b2_block_attestations_electra(b2_ctx* ctx, const uint8_t* wire, uint64_t wire_len, const uint32_t* woff, uint32_t n_att, const uint32_t* block_off,
+                                  const uint64_t* block_slot, uint32_t n_blocks, const uint32_t* members, const uint32_t* off, uint32_t n_committees,
+                                  uint32_t cps_prev, uint32_t cps_cur, const uint8_t* chain_roots, const uint8_t* justified80, const uint8_t* domains64,
+                                  uint32_t slots_per_epoch, uint32_t min_inclusion_delay, uint32_t max_committees_per_slot,
+                                  uint32_t max_validators_per_committee, uint64_t effective_balance_increment, uint64_t base_reward_per_increment,
+                                  int32_t* status_out, uint8_t* flag_mask_out, uint64_t* numerator_out, int32_t* block_status_out,
+                                  uint32_t* block_first_out, uint64_t* block_reward_out, uint32_t* n_applied_out) {
+    B2_NVTX;
+    return block_attestations_host(ctx, {true, 0, max_committees_per_slot, max_validators_per_committee, 0}, wire, wire_len, woff, n_att, block_off,
+                                   block_slot, n_blocks, members, off, n_committees, cps_prev, cps_cur, chain_roots, justified80, domains64,
+                                   slots_per_epoch, min_inclusion_delay, effective_balance_increment, base_reward_per_increment, status_out, flag_mask_out,
+                                   numerator_out, block_status_out, block_first_out, block_reward_out, n_applied_out);
 }
 
 // ------------------------------------------------------------------------------------------ sync committee messages (syncmsg.cuh)

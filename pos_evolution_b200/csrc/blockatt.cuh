@@ -158,11 +158,12 @@ __global__ void __launch_bounds__(128) k_ba_parse(ba_args A) {
 
 // One CTA.  A block is invalid when its row is malformed (reversed, past n, a slot outside e or not above the previous block's, or an
 // attestation of its row that ba_block_of gave to another block: B2_GUARD_BAD_ROW) or when it holds an attestation with a nonzero status.
-__global__ void __launch_bounds__(BA_BLOCKS_THREADS) k_ba_blocks(ba_args A) {
+// An attestation that passed the parse's checks and failed FastAggregateVerify gets fav_status (11; 13 in the Electra form).
+__global__ void __launch_bounds__(BA_BLOCKS_THREADS) k_ba_blocks(ba_args A, int32_t fav_status) {
     __shared__ uint32_t first_bad;
     if (threadIdx.x == 0) first_bad = A.n_blocks;
     for (uint32_t a = threadIdx.x; a < A.n; a += blockDim.x)
-        if (A.status[a] == 0 && !A.fav_ok[a]) A.status[a] = 11;
+        if (A.status[a] == 0 && !A.fav_ok[a]) A.status[a] = fav_status;
     __syncthreads();
     const uint64_t spe = A.slots_per_epoch, e = A.block_slot[0] / spe;
     for (uint32_t b = threadIdx.x; b < A.n_blocks; b += blockDim.x) {

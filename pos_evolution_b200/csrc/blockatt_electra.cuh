@@ -12,8 +12,8 @@
 //   FastAggregateVerify with the split key sum: k_g1_gather_tma<false> (gather.cuh, unchanged) with one warp per BAE_CHUNK members of a
 //   row, each chunk taken as an aggregate of its own, then k_bae_pk_combine (warp per attestation) adds the partial sums with the
 //   complete Jacobian addition into the aggregate keys verify_main pairs
-//   k_bae_verdicts  thread per attestation: a failed FastAggregateVerify is status 13
-//   k_ba_blocks, k_part_phase1-3, k_ba_rewards (blockatt.cuh, kernels.cuh) unchanged, over the padded rows
+//   k_ba_blocks, k_part_phase1-3, k_ba_rewards (blockatt.cuh, kernels.cuh) as for phase 0, over the padded rows; a failed
+//                   FastAggregateVerify is status 13
 //
 // Wire form: offset u32 | data 128 | signature 96 | committee_bits ceil(M / 8) | aggregation_bits Bitlist, M = max_committees_per_slot.
 #pragma once
@@ -247,12 +247,6 @@ __global__ void __launch_bounds__(128) k_bae_pk_combine(const uint32_t* __restri
     status = __reduce_or_sync(B2_FULL_MASK, status);
     cnt = __reduce_add_sync(B2_FULL_MASK, cnt);
     if (lane == 0) core_g1_finish(acc, status, cnt, a, out_jac, out_status);
-}
-
-// thread per attestation: a FastAggregateVerify failure is status 13 (k_ba_blocks then finds no status 0 with a failed verdict)
-__global__ void __launch_bounds__(128) k_bae_verdicts(int32_t* status, const uint8_t* fav_ok, uint32_t n) {
-    const uint32_t a = blockIdx.x * blockDim.x + threadIdx.x;
-    if (a < n && status[a] == 0 && !fav_ok[a]) status[a] = 13;
 }
 
 }  // namespace b2

@@ -364,21 +364,9 @@ class Engine:
         SSZ encodings back to back (woff their offsets), block b = attestations [block_off[b], block_off[b+1]) included at block_slot[b];
         committee c = members[off[c] .. off[c+1]], those of epoch e - 1 then those of e; chain_roots uint8[2 * slots_per_epoch, 32].
         Applies the blocks before the first invalid one to the device participation tables (both must be loaded)."""
-        woff, block_off, members, off = _c(woff, np.uint32), _c(block_off, np.uint32), _c(members, np.uint32), _c(off, np.uint32)
-        block_slot = _c(block_slot, np.uint64)
-        roots = _c(chain_roots, np.uint8).reshape(-1)
-        n, n_b = woff.shape[0] - 1, block_off.shape[0] - 1
-        w = np.frombuffer(bytes(wire), dtype=np.uint8) if len(wire) else np.zeros(1, dtype=np.uint8)
-        mem = members if members.size else np.zeros(1, dtype=np.uint32)
-        j, dom = np.frombuffer(bytes(justified80), dtype=np.uint8), np.frombuffer(bytes(domains64), dtype=np.uint8)
-        assert j.shape == (80,) and dom.shape == (64,) and roots.shape == (64 * int(slots_per_epoch),) and block_slot.shape == (max(n_b, 0),)
-        r = BlockAttestationsResult(np.zeros(n, np.int32), np.zeros(n, np.uint8), np.zeros(n, np.uint64), np.zeros(n_b, np.int32),
-                                    np.zeros(n_b, np.uint32), np.zeros(n_b, np.uint64), np.zeros(1, np.uint32))
-        self._ck(self.lib.b2_block_attestations(self.h, _p(w), len(wire), _p(woff), n, _p(block_off), _p(block_slot), n_b, _p(mem), _p(off),
-                                                off.shape[0] - 1, int(cps_prev), int(cps_cur), _p(roots), _p(j), _p(dom), int(slots_per_epoch),
-                                                int(min_inclusion_delay), int(bits_stride), int(increment), int(base_reward_per_increment),
-                                                *[_p(x) for x in r]))
-        return r._replace(n_applied=int(r.n_applied[0]))
+        return self._block_attestations(self.lib.b2_block_attestations, (int(bits_stride),), wire, woff, block_off, block_slot, members, off,
+                                        cps_prev, cps_cur, chain_roots, justified80, domains64, slots_per_epoch, min_inclusion_delay, increment,
+                                        base_reward_per_increment)
 
     def block_attestations_electra(self, wire: bytes, woff, block_off, block_slot, members, off, cps_prev: int, cps_cur: int, chain_roots,
                                    justified80: bytes, domains64: bytes, slots_per_epoch: int, min_inclusion_delay: int,
@@ -387,6 +375,13 @@ class Engine:
         """block_attestations for Electra encodings (include/b200pos.h, b2_block_attestations_electra: statuses 0-13, Deneb's window and
         flags): an attestation names its committees of data.slot in committee_bits (max_committees_per_slot bits), and its Bitlist is their
         bit rows back to back.  Applies the blocks before the first invalid one to the device participation tables (both must be loaded)."""
+        return self._block_attestations(self.lib.b2_block_attestations_electra, (int(max_committees_per_slot), int(max_validators_per_committee)),
+                                        wire, woff, block_off, block_slot, members, off, cps_prev, cps_cur, chain_roots, justified80, domains64,
+                                        slots_per_epoch, min_inclusion_delay, increment, base_reward_per_increment)
+
+    def _block_attestations(self, fn, shape, wire, woff, block_off, block_slot, members, off, cps_prev, cps_cur, chain_roots, justified80,
+                            domains64, slots_per_epoch, min_inclusion_delay, increment, base_reward_per_increment):
+        """both host block-attestation calls: `shape` is what fn takes between min_inclusion_delay and the increment"""
         woff, block_off, members, off = _c(woff, np.uint32), _c(block_off, np.uint32), _c(members, np.uint32), _c(off, np.uint32)
         block_slot = _c(block_slot, np.uint64)
         roots = _c(chain_roots, np.uint8).reshape(-1)
@@ -397,10 +392,9 @@ class Engine:
         assert j.shape == (80,) and dom.shape == (64,) and roots.shape == (64 * int(slots_per_epoch),) and block_slot.shape == (max(n_b, 0),)
         r = BlockAttestationsResult(np.zeros(n, np.int32), np.zeros(n, np.uint8), np.zeros(n, np.uint64), np.zeros(n_b, np.int32),
                                     np.zeros(n_b, np.uint32), np.zeros(n_b, np.uint64), np.zeros(1, np.uint32))
-        self._ck(self.lib.b2_block_attestations_electra(self.h, _p(w), len(wire), _p(woff), n, _p(block_off), _p(block_slot), n_b, _p(mem), _p(off),
-                                                        off.shape[0] - 1, int(cps_prev), int(cps_cur), _p(roots), _p(j), _p(dom), int(slots_per_epoch),
-                                                        int(min_inclusion_delay), int(max_committees_per_slot), int(max_validators_per_committee),
-                                                        int(increment), int(base_reward_per_increment), *[_p(x) for x in r]))
+        self._ck(fn(self.h, _p(w), len(wire), _p(woff), n, _p(block_off), _p(block_slot), n_b, _p(mem), _p(off), off.shape[0] - 1, int(cps_prev),
+                    int(cps_cur), _p(roots), _p(j), _p(dom), int(slots_per_epoch), int(min_inclusion_delay), *shape, int(increment),
+                    int(base_reward_per_increment), *[_p(x) for x in r]))
         return r._replace(n_applied=int(r.n_applied[0]))
 
     def sync_committee_messages(self, wire: bytes, woff, subnet, position_validator, subnet_count: int, current_slot: int,
@@ -856,15 +850,10 @@ class Engine:
         d_block_off.numel() - 1, the wire's length is d_wire.numel(), n_sig = d_members.numel().  Outputs: d_status int32[n_att],
         d_flag_mask uint8[n_att], d_numerator uint64[n_att], d_block_status int32[n_blocks], d_block_first uint32[n_blocks], d_block_reward
         uint64[n_blocks], d_n_applied uint32[1]."""
-        j, dom = np.frombuffer(bytes(justified80), dtype=np.uint8), np.frombuffer(bytes(domains64), dtype=np.uint8)
-        assert j.shape == (80,) and dom.shape == (64,)
-        self._ck(self.lib.b2_block_attestations_dev(self.h, d_wire.data_ptr(), d_wire.numel(), d_woff.data_ptr(), d_woff.numel() - 1,
-                                                    d_block_off.data_ptr(), d_block_slot.data_ptr(), d_block_off.numel() - 1, d_members.data_ptr(),
-                                                    d_off.data_ptr(), d_off.numel() - 1, d_members.numel(), int(cps_prev), int(cps_cur), d_chain_roots.data_ptr(), _p(j),
-                                                    _p(dom), int(slots_per_epoch), int(min_inclusion_delay), int(bits_stride), int(increment),
-                                                    int(base_reward_per_increment), d_status.data_ptr(), d_flag_mask.data_ptr(),
-                                                    d_numerator.data_ptr(), d_block_status.data_ptr(), d_block_first.data_ptr(),
-                                                    d_block_reward.data_ptr(), d_n_applied.data_ptr(), self._stream()))
+        self._block_attestations_dev(self.lib.b2_block_attestations_dev, (int(bits_stride),), d_wire, d_woff, d_block_off, d_block_slot, d_members,
+                                     d_off, cps_prev, cps_cur, d_chain_roots, justified80, domains64, slots_per_epoch, min_inclusion_delay, increment,
+                                     base_reward_per_increment, BlockAttestationsResult(d_status, d_flag_mask, d_numerator, d_block_status,
+                                                                                        d_block_first, d_block_reward, d_n_applied))
 
     def block_attestations_electra_dev(self, d_wire, d_woff, d_block_off, d_block_slot, d_members, d_off, cps_prev: int, cps_cur: int,
                                        d_chain_roots, justified80: bytes, domains64: bytes, slots_per_epoch: int, min_inclusion_delay: int,
@@ -875,21 +864,27 @@ class Engine:
         slot's committees.  `out`: a BlockAttestationsResult of device tensors (status int32[n_att], flag_mask uint8[n_att], numerator
         uint64[n_att], block_status int32[n_blocks], block_first uint32[n_blocks], block_reward uint64[n_blocks], n_applied uint32[1]), or
         None to allocate them here.  Returns the outputs."""
-        import torch
-        n, nb = d_woff.numel() - 1, d_block_off.numel() - 1
         if out is None:
+            import torch
+            n, nb = d_woff.numel() - 1, d_block_off.numel() - 1
             z = lambda k, dt: torch.zeros(k, dtype=dt, device=d_woff.device)      # noqa: E731
             out = BlockAttestationsResult(z(n, torch.int32), z(n, torch.uint8), z(n, torch.uint64), z(nb, torch.int32), z(nb, torch.uint32),
                                           z(nb, torch.uint64), z(1, torch.uint32))
+        shape = (int(max_committees_per_slot), int(max_validators_per_committee), int(row_max))
+        self._block_attestations_dev(self.lib.b2_block_attestations_electra_dev, shape, d_wire, d_woff, d_block_off, d_block_slot, d_members, d_off,
+                                     cps_prev, cps_cur, d_chain_roots, justified80, domains64, slots_per_epoch, min_inclusion_delay, increment,
+                                     base_reward_per_increment, out)
+        return out
+
+    def _block_attestations_dev(self, fn, shape, d_wire, d_woff, d_block_off, d_block_slot, d_members, d_off, cps_prev, cps_cur, d_chain_roots,
+                                justified80, domains64, slots_per_epoch, min_inclusion_delay, increment, base_reward_per_increment, out):
+        """both device block-attestation calls: `shape` as in _block_attestations, `out` a BlockAttestationsResult of device tensors"""
         j, dom = np.frombuffer(bytes(justified80), dtype=np.uint8), np.frombuffer(bytes(domains64), dtype=np.uint8)
         assert j.shape == (80,) and dom.shape == (64,)
-        self._ck(self.lib.b2_block_attestations_electra_dev(self.h, d_wire.data_ptr(), d_wire.numel(), d_woff.data_ptr(), n, d_block_off.data_ptr(),
-                                                            d_block_slot.data_ptr(), nb, d_members.data_ptr(), d_off.data_ptr(), d_off.numel() - 1,
-                                                            d_members.numel(), int(cps_prev), int(cps_cur), d_chain_roots.data_ptr(), _p(j), _p(dom),
-                                                            int(slots_per_epoch), int(min_inclusion_delay), int(max_committees_per_slot),
-                                                            int(max_validators_per_committee), int(row_max), int(increment),
-                                                            int(base_reward_per_increment), *[x.data_ptr() for x in out], self._stream()))
-        return out
+        self._ck(fn(self.h, d_wire.data_ptr(), d_wire.numel(), d_woff.data_ptr(), d_woff.numel() - 1, d_block_off.data_ptr(), d_block_slot.data_ptr(),
+                    d_block_off.numel() - 1, d_members.data_ptr(), d_off.data_ptr(), d_off.numel() - 1, d_members.numel(), int(cps_prev), int(cps_cur),
+                    d_chain_roots.data_ptr(), _p(j), _p(dom), int(slots_per_epoch), int(min_inclusion_delay), *shape, int(increment),
+                    int(base_reward_per_increment), *[x.data_ptr() for x in out], self._stream()))
 
     def sync_committee_messages_dev(self, d_wire, d_woff, d_subnet, d_position_validator, subnet_count: int, current_slot: int, domain32: bytes,
                                     out=None, trim: bool = True) -> SyncMessagesResult:

@@ -899,16 +899,20 @@ class Spec:
         each block's proposer reward credited to its proposer_index), nothing of that block or of a later one.  The chain's roots below
         blocks[0].slot come from state.block_roots; block k's root stands for the slots [slot_k, slot_{k+1}).  state.slot and block_roots
         are left as they are.  Returns (n_applied, statuses): per block, the status (0-11, include/b200pos.h) of each attestation."""
+        return self._process_block_attestations(state, blocks, self.block_attestations_inputs, self.engine.block_attestations)
+
+    def _process_block_attestations(self, state, blocks, inputs, call):
+        """both block-attestation calls: the arguments by inputs(state, blocks), the Engine method `call`, then the results into the state"""
         assert blocks and state.slot == blocks[0].slot
         block_off = np.concatenate([[0], np.cumsum([len(b.attestations) for b in blocks])]).astype(np.uint32)
         if not block_off[-1]:
             return len(blocks), [np.zeros(0, np.int32) for _ in blocks]
-        args = self.block_attestations_inputs(state, blocks)
+        args = inputs(state, blocks)
         self.sync_registry(state)              # first: a registry reload drops the device participation tables
         eng = self.engine
         eng.participation_load(0, np.asarray(state.current_epoch_participation, dtype=np.uint8))
         eng.participation_load(1, np.asarray(state.previous_epoch_participation, dtype=np.uint8))
-        res = eng.block_attestations(**args)
+        res = call(**args)
         if res.n_applied:
             state.current_epoch_participation[:] = eng.participation_read(0).tolist()
             state.previous_epoch_participation[:] = eng.participation_read(1).tolist()
@@ -960,22 +964,7 @@ class Spec:
         Electra's process_attestation with Deneb's inclusion window and flags.  Block-atomic, the chain's roots, the proposers' rewards and
         what is left unchanged as in process_block_attestations.  Returns (n_applied, statuses): per block, the status (0-13,
         include/b200pos.h) of each attestation."""
-        assert blocks and state.slot == blocks[0].slot
-        block_off = np.concatenate([[0], np.cumsum([len(b.attestations) for b in blocks])]).astype(np.uint32)
-        if not block_off[-1]:
-            return len(blocks), [np.zeros(0, np.int32) for _ in blocks]
-        args = self.block_attestations_electra_inputs(state, blocks)
-        self.sync_registry(state)              # first: a registry reload drops the device participation tables
-        eng = self.engine
-        eng.participation_load(0, np.asarray(state.current_epoch_participation, dtype=np.uint8))
-        eng.participation_load(1, np.asarray(state.previous_epoch_participation, dtype=np.uint8))
-        res = eng.block_attestations_electra(**args)
-        if res.n_applied:
-            state.current_epoch_participation[:] = eng.participation_read(0).tolist()
-            state.previous_epoch_participation[:] = eng.participation_read(1).tolist()
-            for k in range(res.n_applied):
-                state.balances[blocks[k].proposer_index] += int(res.block_reward[k])
-        return res.n_applied, [res.status[block_off[k]:block_off[k + 1]] for k in range(len(blocks))]
+        return self._process_block_attestations(state, blocks, self.block_attestations_electra_inputs, self.engine.block_attestations_electra)
 
     def block_attestations_electra_inputs(self, state, blocks):
         """The arguments of Engine.block_attestations_electra for these blocks of ElectraAttestations on this state: those of

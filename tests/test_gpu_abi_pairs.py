@@ -11,6 +11,7 @@ import pytest
 import torch
 
 import aggregate_intake_oracle as AIO
+import block_attestations_electra_oracle as BAE
 import intake_oracle as IO
 import scenarios
 import sync_messages_oracle as SM
@@ -124,8 +125,9 @@ def _aggregate_and_proof_intake(eng, roots):
     return args, bad, ()
 
 
-def _block_attestations(eng, roots):
-    wires = [IO.encode([True] * CSIZE, _data128(roots), bytes(96)), IO.encode([True] * CSIZE, _data128(roots), bytes(96))]
+def _block_attestation_args(wires, roots, shape):
+    """both block-attestation calls: two attestations in one block of epoch EPOCH, one committee per slot; `shape` the form's
+    member-row arguments, which sit between min_inclusion_delay and effective_balance_increment"""
     wire, wire_len, woff = _wire(wires)
     n_c = 2 * SPE
     n_sig = n_c * CSIZE
@@ -133,13 +135,37 @@ def _block_attestations(eng, roots):
                 block_slot=In(np.array([EPOCH * SPE + 2], np.uint64)), n_blocks=1, members=In(np.arange(n_sig, dtype=np.uint32) % N_VAL),
                 off=In(np.arange(0, n_sig + 1, CSIZE, dtype=np.uint32)), n_committees=n_c, n_sig=DevOnly(n_sig), cps_prev=1, cps_cur=1,
                 chain_roots=In(np.tile(roots[:2].reshape(1, 64), (SPE, 1))), justified80=HostIn(np.zeros(80, np.uint8)),
-                domains64=HostIn(np.full(64, 3, np.uint8)), slots_per_epoch=SPE, min_inclusion_delay=1, bits_stride=1,
+                domains64=HostIn(np.full(64, 3, np.uint8)), slots_per_epoch=SPE, min_inclusion_delay=1, **shape,
                 effective_balance_increment=10**9, base_reward_per_increment=100, status_out=Out(4 * 2), flag_mask_out=Out(2),
                 numerator_out=Out(8 * 2), block_status_out=Out(4), block_first_out=Out(4), block_reward_out=Out(8), n_applied_out=Out(4))
-    bad = {"n_att=0": dict(n_att=0), "n_att=2^28": dict(n_att=1 << 28), "n_blocks=0": dict(n_blocks=0), "bits_stride=0": dict(bits_stride=0),
-           "bits_stride=257": dict(bits_stride=257), "slots_per_epoch=0": dict(slots_per_epoch=0), "cps_cur=0": dict(cps_cur=0),
-           "min_inclusion_delay=0": dict(min_inclusion_delay=0), "effective_balance_increment=0": dict(effective_balance_increment=0),
-           "committees >= 2^31": dict(cps_cur=1 << 30), "n_committees wrong": dict(n_committees=n_c + 1)}
+    bad = {"n_att=0": dict(n_att=0), "n_att=2^28": dict(n_att=1 << 28), "n_blocks=0": dict(n_blocks=0), "slots_per_epoch=0": dict(slots_per_epoch=0),
+           "cps_cur=0": dict(cps_cur=0), "min_inclusion_delay=0": dict(min_inclusion_delay=0),
+           "effective_balance_increment=0": dict(effective_balance_increment=0), "committees >= 2^31": dict(cps_cur=1 << 30),
+           "n_committees wrong": dict(n_committees=n_c + 1)}
+    return args, bad
+
+
+def _block_attestations(eng, roots):
+    args, bad = _block_attestation_args([IO.encode([True] * CSIZE, _data128(roots), bytes(96))] * 2, roots, dict(bits_stride=1))
+    return args, {**bad, "bits_stride=0": dict(bits_stride=0), "bits_stride=257": dict(bits_stride=257)}, ()
+
+
+def _block_attestations_electra(eng, roots):
+    # the device form also takes row_max, which the host form derives from off
+    shape = dict(max_committees_per_slot=1, max_validators_per_committee=CSIZE, row_max=DevOnly(CSIZE))
+    args, bad = _block_attestation_args([BAE.encode([True] * CSIZE, _data128(roots), bytes(96), [True])] * 2, roots, shape)
+    # n_att times the padded row at 2^32 members: one slot of 2 049 members pads to 4 096 (BAE_CHUNK 2 048), 2^20 attestations in one block
+    sizes = [CSIZE] * (2 * SPE)
+    sizes[SPE + 1] = 2049
+    off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.uint32)
+    assert BAE.row_max(off, 1, 1, SPE) == 2049
+    n_att = 1 << 20
+    wide = dict(woff=In(np.zeros(n_att + 1, np.uint32)), n_att=n_att, block_off=In(np.array([0, n_att], np.uint32)),
+                members=In(np.arange(off[-1], dtype=np.uint32) % N_VAL), off=In(off), n_sig=DevOnly(int(off[-1])), row_max=DevOnly(2049))
+    bad.update({"max_committees_per_slot=0": dict(max_committees_per_slot=0), "max_committees_per_slot=65": dict(max_committees_per_slot=65),
+                "max_validators_per_committee=0": dict(max_validators_per_committee=0),
+                "M * max_validators_per_committee >= 2^31": dict(max_committees_per_slot=64, max_validators_per_committee=1 << 25),
+                "n_att * padded row >= 2^32": wide})
     return args, bad, ()
 
 
@@ -205,7 +231,8 @@ def _pack_attestations(eng, roots):
 
 
 PAIRS = {f.__name__[1:]: f for f in (_aggregate, _fast_aggregate_verify, _aggregate_verify, _sync_aggregate_verify, _attestation_intake,
-                                     _aggregate_and_proof_intake, _block_attestations, _sync_committee_messages, _shuffle_committees,
+                                     _aggregate_and_proof_intake, _block_attestations, _block_attestations_electra, _sync_committee_messages,
+                                     _shuffle_committees,
                                      _latest_messages_update, _slasher_advance, _slasher_update, _slasher_discount, _pack_attestations)}
 
 
@@ -301,6 +328,7 @@ PRECONDITIONS = [
     ("sync_aggregate_verify", "registry", "no sync committee loaded"), ("attestation_intake", "registry", "no tree loaded"),
     ("aggregate_and_proof_intake", "registry", "no tree loaded"), ("aggregate_and_proof_intake", "tree", "registry not loaded"),
     ("block_attestations", "", "registry not loaded"), ("block_attestations", "registry", "participation tables"),
+    ("block_attestations_electra", "", "registry not loaded"), ("block_attestations_electra", "registry", "participation tables"),
     ("sync_committee_messages", "", "registry not loaded"), ("latest_messages_update", "", "registry not loaded"),
     ("slasher_advance", "registry", "b2_slasher_init"), ("slasher_update", "registry", "b2_slasher_init"),
     ("slasher_discount", "", "registry not loaded"), ("slasher_discount", "registry", "b2_slasher_init"),
@@ -324,7 +352,7 @@ def test_missing_state_is_rejected_alike(loaded, name, holds, why):
         fresh.close()
 
 
-@pytest.mark.parametrize("name", ["attestation_intake", "aggregate_and_proof_intake", "block_attestations"])
+@pytest.mark.parametrize("name", ["attestation_intake", "aggregate_and_proof_intake", "block_attestations", "block_attestations_electra"])
 def test_device_form_refuses_n_sig_past_32_bits(loaded, name):
     """n_sig is the one count only the device form receives (the host form derives it from u32 offsets): 2^32 is refused, nothing
     launched, no output written"""
